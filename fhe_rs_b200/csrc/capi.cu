@@ -458,6 +458,17 @@ void key_switch_core(const fhe_b200_params* par, const fhe_b200_ksk* k, const u6
   // with the TMA kernels the transform deposits the digits of one (ciphertext, limb) in adjacent rows, which the
   // inner product streams fastest (bench_micro/stride_read.cu)
   adjacent = Lk > 1 && ntt_uses_tma(cts * L * Lk, kl.ctx_ids, par->logn, Lk, c2, inter);
+  // default: the rows pass of the digit transforms and the inner product run as one kernel, so the transformed digits
+  // never go through HBM.  FHE_B200_KSMAC=tma keeps the unfused TMA chain (rows pass, then ksmac_tma_kernel),
+  // =classic the per-thread inner product.
+  static const bool fused = [] {
+    const char* e = getenv("FHE_B200_KSMAC");
+    return !e || (strcmp(e, "tma") && strcmp(e, "classic"));
+  }();
+  if (adjacent && fused &&
+      launch_key_switch_tma(c2, inter, k->k0, k->k1, base0, base1, out0, out1, cts, L, Lk, out_ct_rows, kl.ctx_ids,
+                            par->d_limbs, par->logn, reduce, st))
+    return;
   launch_ntt(c2, inter, cts * L * Lk, kl.ctx_ids, par->d_limbs, par->logn, false, Lk, reduce, st, true, adjacent, L);
   }
   launch_ksmac(inter, k->k0, k->k1, base0, base1, out0, out1, cts, L, Lk, out_ct_rows, kl.ctx_ids, par->d_limbs,

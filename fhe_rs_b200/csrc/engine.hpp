@@ -106,6 +106,13 @@ void launch_ksmac(const u64* inter, const u64* k0, const u64* k1, const u64* bas
 // whether launch_ntt will take the TMA kernels for this shape (they can write the digit-adjacent layout)
 bool ntt_uses_tma(u32 n_rows, const RowIds& ids, u32 logn, u32 in_div, const u64* in, const u64* out);
 
+// the RNS-digit key switch on the TMA kernels: digit broadcast + forward cols pass of c2 [cts][n_dig][N] into
+// `inter` (scratch, cts*n_dig*Lk rows, digit-adjacent), then the forward rows pass fused with the inner product of
+// launch_ksmac (same outputs, same indexing).  Returns false, having launched nothing, outside the kernels' domain.
+bool launch_key_switch_tma(const u64* c2, u64* inter, const u64* k0, const u64* k1, const u64* base0,
+                           const u64* base1, u64* out0, u64* out1, u32 cts, u32 n_dig, u32 Lk, u32 out_ct_rows,
+                           const RowIds& ids, const LimbDev* limbs, u32 logn, bool reduce, cudaStream_t st);
+
 // base-2^log_base digit decomposition of single-limb polynomials (key_switching_key.rs:339-345):
 // in [polys][N] -> out [polys][n_dig][N]
 void launch_decompose(const u64* in, u64* out, size_t polys, u32 n_dig, u32 log_base, u32 logn, cudaStream_t st);

@@ -259,6 +259,16 @@ void run_tma_cols_for(const u64* in, u64 in_rows, u64* out, u64 out_rows, const 
   }
 }
 
+// digit-broadcast cols passes walk their tiles limb-innermost (cols_tile, ntt_tma.cuh): each source tile leaves DRAM
+// once instead of once per limb.  FHE_B200_BCAST_WALK=limb_major keeps the limb-major walk.
+bool bcast_limb_inner() {
+  static const bool v = [] {
+    const char* e = getenv("FHE_B200_BCAST_WALK");
+    return !(e && !strcmp(e, "limb_major"));
+  }();
+  return v;
+}
+
 // Both passes through the TMA kernels.  Returns false when the shape is outside their domain (the caller then uses
 // the register-resident kernels).
 bool launch_ntt_tma(const u64* in, u64* out, u32 n_rows, const RowIds& ids, const LimbDev* limbs, u32 logn, bool inverse,
@@ -281,6 +291,7 @@ bool launch_ntt_tma(const u64* in, u64* out, u32 n_rows, const RowIds& ids, cons
   try {
     NttTmaArgs first = A, second = A;
     first.in_bcast = in_div != 1;
+    first.limb_inner = first.in_bcast && bcast_limb_inner();
     if (!inverse) {
       first.reduce_on_load = reduce_on_load;
       second.lazy_out = lazy_out;
@@ -340,6 +351,34 @@ bool launch_tensor_intt_tma(const u64* a, const u64* b, const u64* xa, const u64
   return true;
 }
 
+template <int STAGES>
+void run_ks_rows_mac(const CUtensorMap& mi, const CUtensorMap& m0, const CUtensorMap& m1, const KsRowsArgs& A,
+                     cudaStream_t st) {
+  using Cfg = KsRowsCfg<STAGES>;
+  auto k = ks_rows_mac_tma_kernel<STAGES, 3>;
+  const size_t smem = Cfg::smem(A.n_dig);
+  ensure_dynamic_smem((const void*)k, smem);
+  int per_sm = 0;
+  FHE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)k, Cfg::NT + 32, smem));
+  const u32 grid = (u32)std::min<u64>(A.items_total, (u64)sm_count() * std::max(per_sm, 1));
+  k<<<grid, Cfg::NT + 32, smem, st>>>(mi, m0, m1, A);
+  g_launches++;
+}
+
+// a key [Lk][n_dig][N] as {128-coefficient, n_dig-row} boxes, no swizzle
+CUtensorMap key_map(const u64* base, u64 rows, u32 logn, u32 box_cols, u32 box_rows) {
+  CUtensorMap m;
+  const cuuint64_t gdim[2] = {(cuuint64_t)1 << logn, rows};
+  const cuuint64_t gstride[1] = {(cuuint64_t)8 << logn};
+  const cuuint32_t box[2] = {box_cols, box_rows};
+  const cuuint32_t es[2] = {1, 1};
+  if (tensor_map_encoder()(&m, CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, (void*)base, gdim, gstride, box, es,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+    throw TmaFail{};
+  return m;
+}
+
 int tma_mode() {
   static const int mode = [] {
     const char* e = getenv("FHE_B200_NTT");
@@ -372,6 +411,55 @@ bool launch_tensor_inverse_ntt(const u64* a, const u64* b, const u64* xa, const 
        reinterpret_cast<uintptr_t>(xb)) & 127)
     return false;
   return launch_tensor_intt_tma(a, b, xa, xb, T, cts, L, K, mul_ids, limbs, logn, st);
+}
+
+bool launch_key_switch_tma(const u64* c2, u64* inter, const u64* k0, const u64* k1, const u64* base0,
+                           const u64* base1, u64* out0, u64* out1, u32 cts, u32 n_dig, u32 Lk, u32 out_ct_rows,
+                           const RowIds& ids, const LimbDev* limbs, u32 logn, bool reduce, cudaStream_t st) {
+  // ring depth of the digit tiles: 2 (default) or 3 (FHE_B200_KS_STAGES >= 3); both keep 3 CTAs per SM at n_dig = 14
+  static const int stages = tma_variant("FHE_B200_KS_STAGES", 2) >= 3 ? 3 : 2;
+  using Cfg = KsRowsCfg<2>;
+  const u32 n_rows = cts * n_dig * Lk;
+  if (logn < 13 || logn > 15 || !tensor_map_encoder() || ids.limbs_per_poly != Lk || n_dig == 0 || n_dig > 256)
+    return false;
+  if ((reinterpret_cast<uintptr_t>(c2) | reinterpret_cast<uintptr_t>(inter) | reinterpret_cast<uintptr_t>(k0) |
+       reinterpret_cast<uintptr_t>(k1)) & 127)
+    return false;
+  if ((stages == 3 ? KsRowsCfg<3>::smem(n_dig) : Cfg::smem(n_dig)) > 227 * 1024) return false;
+  try {
+    // every tensor map first: a shape the TMA cannot describe launches nothing
+    const CUtensorMap mi = rows_map(inter, n_rows, logn, 4 * Cfg::R);
+    const CUtensorMap m0 = key_map(k0, (u64)Lk * n_dig, logn, Cfg::TC, n_dig);
+    const CUtensorMap m1 = key_map(k1, (u64)Lk * n_dig, logn, Cfg::TC, n_dig);
+    // digit broadcast + large-stride stages: inter [ct][j][d][N] (in_bcast: the source row of polynomial (ct, d) is
+    // row ct*n_dig + d of c2 for every limb j)
+    NttTmaArgs C;
+    std::memset(&C, 0, sizeof(C));
+    C.limbs = limbs;
+    C.n_polys = cts * n_dig;
+    C.lpp = Lk;
+    C.in_bcast = 1;
+    C.limb_inner = bcast_limb_inner();
+    C.digit_adjacent = 1;
+    C.n_dig = n_dig;
+    C.reduce_on_load = reduce ? 1 : 0;
+    C.logn = logn;
+    for (int i = 0; i < kMaxPos; i++) C.ids[i] = ids.ids[i];
+    run_tma_cols_for<false>(c2, (u64)cts * n_dig, inter, n_rows, C, st);
+    KsRowsArgs A;
+    std::memset(&A, 0, sizeof(A));
+    A.limbs = limbs;
+    A.base0 = base0; A.base1 = base1; A.out0 = out0; A.out1 = out1;
+    A.cts = cts; A.n_dig = n_dig; A.Lk = Lk; A.out_ct_rows = out_ct_rows; A.logn = logn;
+    A.tiles_per_row = (1u << logn) / Cfg::TC;
+    A.items_total = Lk * A.tiles_per_row * cts;
+    for (int i = 0; i < kMaxPos; i++) A.ids[i] = ids.ids[i];
+    if (stages == 3) run_ks_rows_mac<3>(mi, m0, m1, A, st);
+    else run_ks_rows_mac<2>(mi, m0, m1, A, st);
+  } catch (const TmaFail&) {
+    return false;
+  }
+  return true;
 }
 
 void launch_ntt(const u64* in, u64* out, u32 n_rows, const RowIds& ids, const LimbDev* limbs, u32 logn,

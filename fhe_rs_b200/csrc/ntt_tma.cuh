@@ -38,6 +38,7 @@ struct NttTmaArgs {
   u32 logn;
   u32 tiles_per_row;
   u32 tiles_total;     // lpp * tiles_per_row * n_polys; tile index = (j*tiles_per_row + tau)*n_polys + p
+  u32 limb_inner;      // cols pass only: tile index = (tau*n_polys + p)*lpp + j instead (see ntt_tma_cols_kernel)
   unsigned short ids[kMaxPos];
 };
 
@@ -143,6 +144,25 @@ __device__ __forceinline__ void fwd_stages(u64* v, const ulonglong2* tw, u64 p, 
       for (int e = 0; e < half; e++) {
         const int jj = m * 2 * half + e;
         bf_fwd<false>(v[jj], v[jj + half], w.x, w.y, p, p2, 0);
+      }
+    }
+  }
+}
+// fwd_stages<3> with the twiddle pair of (stage u, block m) fetched by tw(u, m) right before the stage that uses it
+template <class TW>
+__device__ __forceinline__ void fwd_stages3_staged(u64* v, u64 p, u64 p2, const TW& tw) {
+#pragma unroll
+  for (int u = 0; u < 3; u++) {
+    const int half = 8 >> (u + 1);
+    ulonglong2 w[4];
+#pragma unroll
+    for (int m = 0; m < (1 << u); m++) w[m] = tw(u, m);
+#pragma unroll
+    for (int m = 0; m < (1 << u); m++) {
+#pragma unroll
+      for (int e = 0; e < half; e++) {
+        const int jj = m * 2 * half + e;
+        bf_fwd<false>(v[jj], v[jj + half], w[m].x, w[m].y, p, p2, 0);
       }
     }
   }
@@ -846,6 +866,200 @@ __global__ void __launch_bounds__(TensorRowsCfg<RLOG, STAGES>::NT + 32, MINB)
   }
 }
 
+// ------------------------------------------------------------------------------------------------ key-switch rows + inner product
+// The last pass of the digit transforms of a key switch fused with the inner product that consumes them
+// (key_switching_key.rs:256-268: out{0,1} = base{0,1} + sum_d NTT_j(digit_d) * k{0,1}[j][d]).  Every digit of one
+// (ciphertext, limb j) is transformed modulo the same q_j, so all of them share the rows-pass twiddles of (j, tau) and
+// the key tiles of (j, tau); the cols pass has left them in adjacent rows (digit-adjacent layout, [ct][j][d][N]).
+//   work item = (limb j, 128-coefficient tile tau, ciphertext ct), ct innermost: twiddles and the two key tiles of
+//   (j, tau) ({128, n_dig} boxes) are staged once per run of ciphertexts; the n_dig digit tiles of each item arrive
+//   through a ring of STAGES buffers.  Per item: the six small-stride forward stages on each digit tile (16 threads per
+//   tile, 16 tiles side by side, lazy outputs in [0,4q_j) as the unfused pass leaves them), a CTA barrier, then one
+//   thread per (output, coefficient) accumulates sum_d digit_d * key_d with Acc192, adds the base and reduces once.
+// The transformed digits never travel to HBM and back: the unfused chain wrote and re-read all of them.
+struct KsRowsArgs {
+  const LimbDev* limbs;
+  const u64 *base0, *base1;   // nullable, indexed like out0 / out1
+  u64 *out0, *out1;           // row (ct, j) at (ct*out_ct_rows + j)*N
+  u32 cts, n_dig, Lk, out_ct_rows, logn;
+  u32 tiles_per_row;
+  u32 items_total;            // Lk * tiles_per_row * cts; item = (j*tiles_per_row + tau)*cts + ct
+  unsigned short ids[kMaxPos];
+};
+
+template <int STAGES>
+struct KsRowsCfg {
+  static constexpr u32 R = 2;                 // matrix rows of 64 points per tile: 128 coefficients
+  static constexpr u32 TC = 64 * R;
+  static constexpr u32 TILE_BYTES = 512 * R;  // one digit tile, 1024-byte aligned for the 128-byte swizzle
+  static constexpr u32 GROUPS = 16;           // digit tiles transformed side by side (8R = 16 threads each)
+  static constexpr u32 NT = GROUPS * 8 * R;   // 256 consumers = one per (output, coefficient) of the inner product
+  static constexpr u32 TW_PAIRS = 63 * R;
+  static constexpr size_t smem(u32 nd) {
+    return (size_t)STAGES * nd * TILE_BYTES + 2 * (size_t)nd * TC * 8 + TW_PAIRS * 16 + 2 * STAGES * 8 + 8 + 1024;
+  }
+};
+
+template <int STAGES, int MINB>
+__global__ void __launch_bounds__(KsRowsCfg<STAGES>::NT + 32, MINB)
+    ks_rows_mac_tma_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_k0,
+                           const __grid_constant__ CUtensorMap tm_k1, const KsRowsArgs A) {
+  using namespace tma;
+  using Cfg = KsRowsCfg<STAGES>;
+  constexpr u32 R = Cfg::R, TC = Cfg::TC, NT = Cfg::NT, TILE_BYTES = Cfg::TILE_BYTES, GROUPS = Cfg::GROUPS;
+  extern __shared__ unsigned char smem_raw[];
+  const u32 nd = A.n_dig;
+  const u32 base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // the 128-byte swizzle works on absolute address bits
+  const u32 stage_bytes = nd * TILE_BYTES;
+  const u32 k0_base = base + STAGES * stage_bytes;         // [n_dig][TC] u64, no swizzle
+  const u32 k1_base = k0_base + nd * TC * 8;
+  const u32 tw_base = k1_base + nd * TC * 8;
+  const u32 bar_full = tw_base + Cfg::TW_PAIRS * 16;
+  const u32 bar_done = bar_full + STAGES * 8;
+  const u32 bar_key = bar_done + STAGES * 8;
+
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int s = 0; s < STAGES; s++) {
+      mbar_init(bar_full + 8 * s, 1);
+      mbar_init(bar_done + 8 * s, NT);
+    }
+    mbar_init(bar_key, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  const u32 lo = (u32)(((u64)A.items_total * blockIdx.x) / gridDim.x);
+  const u32 hi = (u32)(((u64)A.items_total * (blockIdx.x + 1)) / gridDim.x);
+  const u32 n = hi - lo;
+  const u32 box_rows_per_row = (1u << A.logn) >> 4;   // 128-byte box rows per polynomial row
+
+  if (threadIdx.x >= NT) {
+    // ---------------- producer: the digit tiles of every item of this CTA, STAGES items ahead of the consumers
+    if (threadIdx.x != NT) return;
+    prefetch_map(&tm_in);
+    TileWalk wl;
+    wl.init(lo, A.cts);
+    for (u32 i = 0; i < n; i++) {
+      const u32 s = i % STAGES;
+      if (i >= (u32)STAGES) mbar_wait(bar_done + 8 * s, (i / STAGES - 1) & 1);   // item i - STAGES consumed
+      const u32 j = wl.jt / A.tiles_per_row, tau = wl.jt - j * A.tiles_per_row;
+      const u32 row0 = (wl.p * A.Lk + j) * nd;
+      mbar_expect_tx(bar_full + 8 * s, stage_bytes);
+      for (u32 d = 0; d < nd; d++)
+        load_2d(base + s * stage_bytes + d * TILE_BYTES, &tm_in, 0, (row0 + d) * box_rows_per_row + tau * (4 * R),
+                bar_full + 8 * s);
+      wl.next();
+    }
+    return;
+  }
+
+  // ---------------- consumers
+  const u32 tid = threadIdx.x;
+  const u32 g = tid >> 4, lt = tid & 15;            // transform: digit group, thread inside the digit tile
+  const u32 hmask = 0xffffu << (tid & 16);          // the half warp that owns one digit tile
+  const u32 x = lt & 7, b = lt >> 3;
+  // Offsets inside a (1024-byte aligned) digit tile with the TMA 128-byte swizzle, as in the rows pass.  With two
+  // matrix rows per tile the offset of word e differs from that of word 0 by a compile-time XOR mask, so only word 0's
+  // offset is kept in a register: round 0 reads words 64b + x + 8e, round 1 the pairs (64b + 8x + 2k, +1).
+  const u32 off0 = ((4 * b) << 7) | ((((x >> 1) & 7) ^ (4 * b)) << 4) | ((x & 1) << 3);
+  const u32 off1 = ((4 * b + (x >> 1)) << 7) | (((4 * (x & 1)) ^ (4 * b + (x >> 1))) << 4);
+  auto x0 = [](int e) -> u32 { return ((u32)(e >> 1) << 7) | ((u32)((e >> 1) ^ (4 * (e & 1))) << 4); };
+  const u32 tw0 = tw_base + 16 * (b);
+  const u32 tw1 = tw_base + 16 * (R * 1 + (b << 1));
+  const u32 tw2 = tw_base + 16 * (R * 3 + (b << 2));
+  const u32 tw3 = tw_base + 16 * (R * 7 + lt);
+  const u32 tw4 = tw_base + 16 * (R * 15 + lt);
+  const u32 tw5 = tw_base + 16 * (R * 31 + lt);
+  // inner product: coefficient c of output o
+  const u32 c = tid & (TC - 1), o = tid / TC;
+  const u32 offc = ((c >> 4) << 7) | ((((c >> 1) & 7) ^ ((c >> 4) & 7)) << 4) | ((c & 1) << 3);
+  const u32 key_c = (o ? k1_base : k0_base) + 8 * c;
+  const u64* bsrc = o ? A.base1 : A.base0;
+  u64* dst = o ? A.out1 : A.out0;
+
+  TileWalk w;
+  w.init(lo, A.cts);
+  bool fresh = true;
+  u32 key_phase = 0;
+  const LimbDev* Mp = A.limbs;
+  u64 p = 0, p2 = 0;
+  const u32 logn1 = A.logn - 6;
+  for (u32 i = 0; i < n; i++) {
+    const u32 j = w.jt / A.tiles_per_row, tau = w.jt - j * A.tiles_per_row;
+    const bool new_keys = fresh;
+    if (fresh) {
+      // new (limb, tile position): its key tiles and 63R twiddle pairs replace the previous ones
+      Mp = A.limbs + A.ids[j];
+      p = Mp->p;
+      p2 = Mp->p2;
+      if (i) consumer_sync<NT>();   // nobody still reads the previous twiddles or key tiles
+      if (tid == 0) {
+        mbar_expect_tx(bar_key, 2 * nd * TC * 8);
+        load_2d(k0_base, &tm_k0, tau * TC, j * nd, bar_key);
+        load_2d(k1_base, &tm_k1, tau * TC, j * nd, bar_key);
+      }
+      const u32 row0 = tau * R;
+#pragma unroll
+      for (int tl = 0; tl < 6; tl++) {
+        const u32 s = logn1 + tl;
+        const u32 g0 = (1u << s) + (row0 << tl);
+        if (tid < (R << tl)) {
+          const ulonglong2 v = __ldg(Mp->om + g0 + tid);
+          const u32 k = tid;
+          const u32 dst_pair = tl < 3 ? k : (k & ((1u << (tl >= 3 ? tl - 3 : 0)) - 1)) * (8 * R) + (k >> (tl >= 3 ? tl - 3 : 0));
+          sts128(tw_base + 16 * (R * ((1u << tl) - 1) + dst_pair), v.x, v.y);
+        }
+      }
+      consumer_sync<NT>();
+    }
+    const size_t oi = (((size_t)w.p * A.out_ct_rows + j) << A.logn) + tau * TC + c;
+    const u64 bv = bsrc ? bsrc[oi] : 0;   // in flight while the digits are transformed
+    const u32 s = i % STAGES;
+    const u32 ring = base + s * stage_bytes;
+    mbar_wait(bar_full + 8 * s, (i / STAGES) & 1);
+    // the six small-stride forward stages of every digit tile, outputs lazy in [0, 4q_j) (forward_vt_lazy)
+    // (each stage's twiddles are read from shared memory just before it: holding all seven pairs of a round spilled
+    // at the 72 registers that three 288-thread CTAs per SM leave)
+    for (u32 d = g; d < nd; d += GROUPS) {
+      const u32 a0 = ring + d * TILE_BYTES + off0, a1 = ring + d * TILE_BYTES + off1;
+      u64 v[8];
+#pragma unroll
+      for (int e = 0; e < 8; e++) v[e] = lds64(a0 ^ x0(e));
+      fwd_stages3_staged(v, p, p2, [&](int u, int m) {
+        return lds128(u == 0 ? tw0 : u == 1 ? tw1 + 16 * m : tw2 + 16 * m);
+      });
+#pragma unroll
+      for (int e = 0; e < 8; e++) sts64(a0 ^ x0(e), v[e]);
+      __syncwarp(hmask);
+#pragma unroll
+      for (int k = 0; k < 4; k++) {
+        const ulonglong2 t = lds128(a1 ^ (k << 4));
+        v[2 * k] = t.x;
+        v[2 * k + 1] = t.y;
+      }
+      fwd_stages3_staged(v, p, p2, [&](int u, int m) {
+        return lds128(u == 0 ? tw3 : u == 1 ? tw4 + 16 * 8 * R * m : tw5 + 16 * 8 * R * m);
+      });
+#pragma unroll
+      for (int k = 0; k < 4; k++) sts128(a1 ^ (k << 4), v[2 * k], v[2 * k + 1]);
+    }
+    if (new_keys) {
+      mbar_wait(bar_key, key_phase);
+      key_phase ^= 1;
+    }
+    consumer_sync<NT>();   // every digit tile of the item is transformed
+    Acc192 acc;
+    acc.clear();
+#pragma unroll 2
+    for (u32 d = 0; d < nd; d++) acc.mac(lds64(ring + d * TILE_BYTES + offc), lds64(key_c + d * TC * 8));
+    acc.add64(bv);
+    dst[oi] = acc.reduce(*Mp);
+    mbar_arrive(bar_done + 8 * s);   // the ring stage may take the item STAGES ahead
+    fresh = w.next();
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ cols pass
 // The log2(N1) large-stride stages on tiles of all N1 = 2^LOGP points x 16 adjacent columns (128-byte segments at
 // stride 512 bytes).  2^LOGP consumer threads + one producer warp; radix-8 rounds in place, 16 / 8 words per thread
@@ -910,6 +1124,25 @@ __device__ __forceinline__ void cols_round(u32 buf, u32 tw_base, u64 p, u64 p2, 
   }
 }
 
+// tile index -> (limb j, tile position tau, polynomial p).  Limb-major by default: consecutive tiles of a CTA share
+// the limb's twiddles.  A.limb_inner puts the limb innermost, for the digit broadcast (in_bcast): there the Lk tiles
+// (tau, p, j = 0 .. Lk-1) read the SAME source tile, so back to back only the first read reaches DRAM and the rest
+// hit L2 (limb-major, one limb's pass over a chunk's c2 is far larger than L2 and every limb refetches it), for the
+// price of restaging the 2^LOGP twiddle pairs per tile.
+__device__ __forceinline__ void cols_tile(const NttTmaArgs& A, u32 idx, u32& j, u32& tau, u32& p) {
+  if (A.limb_inner) {
+    const u32 r = idx / A.lpp;
+    j = idx - r * A.lpp;
+    tau = r / A.n_polys;
+    p = r - tau * A.n_polys;
+  } else {
+    const u32 jt = idx / A.n_polys;
+    p = idx - jt * A.n_polys;
+    j = jt / A.tiles_per_row;
+    tau = jt - j * A.tiles_per_row;
+  }
+}
+
 template <int LOGP, bool INV, int STAGES, int MINB, bool REDUCE, bool ROLL = false>
 __global__ void __launch_bounds__(ColsCfg<LOGP, STAGES>::NT + 32, MINB)
     ntt_tma_cols_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_out,
@@ -942,33 +1175,30 @@ __global__ void __launch_bounds__(ColsCfg<LOGP, STAGES>::NT + 32, MINB)
     if (threadIdx.x != NT) return;
     prefetch_map(&tm_in);
     prefetch_map(&tm_out);
-    TileWalk wl, ws;
-    wl.init(lo, A.n_polys);
-    ws.init(lo, A.n_polys);
     u32 loaded = 0;
     auto load_next = [&]() {
       const u32 s = loaded % STAGES;
-      const u32 j = wl.jt / A.tiles_per_row, tau = wl.jt - j * A.tiles_per_row;
-      const u32 row = A.in_bcast ? wl.p : out_row_of(A, wl.p, j);
+      u32 j, tau, pp;
+      cols_tile(A, lo + loaded, j, tau, pp);
+      const u32 row = A.in_bcast ? pp : out_row_of(A, pp, j);
       mbar_expect_tx(bar_full + 8 * s, TILE_BYTES);
 #pragma unroll
       for (u32 h = 0; h < Cfg::BOXES; h++)
         load_3d(base + s * TILE_BYTES + h * Cfg::BOX_ROWS * 128, &tm_in, tau * 16, h * Cfg::BOX_ROWS, row,
                 bar_full + 8 * s);
-      wl.next();
       loaded++;
     };
     while (loaded < n && loaded < (u32)STAGES) load_next();
     for (u32 i = 0; i < n; i++) {
       const u32 s = i % STAGES;
       mbar_wait(bar_done + 8 * s, (i / STAGES) & 1);
-      const u32 j = ws.jt / A.tiles_per_row, tau = ws.jt - j * A.tiles_per_row;
-      const u32 row = out_row_of(A, ws.p, j);
+      u32 j, tau, pp;
+      cols_tile(A, lo + i, j, tau, pp);
+      const u32 row = out_row_of(A, pp, j);
 #pragma unroll
       for (u32 h = 0; h < Cfg::BOXES; h++)
         store_3d(&tm_out, tau * 16, h * Cfg::BOX_ROWS, row, base + s * TILE_BYTES + h * Cfg::BOX_ROWS * 128);
       bulk_commit();
-      ws.next();
       if (loaded < n) {
         bulk_wait_read<0>();
         load_next();
@@ -979,14 +1209,13 @@ __global__ void __launch_bounds__(ColsCfg<LOGP, STAGES>::NT + 32, MINB)
   }
 
   const u32 tid = threadIdx.x;
-  TileWalk w;
-  w.init(lo, A.n_polys);
   u32 cur_j = 0xffffffffu;
   const LimbDev* Lp = A.limbs;
   u64 p = 0, p2 = 0, bhi = 0, blo = 0;
   LastStage ls = {0, 0, 0, 0};
   for (u32 i = 0; i < n; i++) {
-    const u32 j = w.jt / A.tiles_per_row;
+    u32 j, tau_unused, p_unused;
+    cols_tile(A, lo + i, j, tau_unused, p_unused);
     if (j != cur_j) {
       // new limb: stage the 2^LOGP - 1 twiddle pairs of the large-stride stages (the same for every tile of the limb)
       Lp = A.limbs + A.ids[j];
@@ -1028,7 +1257,6 @@ __global__ void __launch_bounds__(ColsCfg<LOGP, STAGES>::NT + 32, MINB)
     }
     fence_proxy_async();
     mbar_arrive(bar_done + 8 * s);
-    w.next();
   }
 }
 
