@@ -18,6 +18,7 @@ CONTEXT_MISMATCH, INVALID_LEVEL, BAD_POLY_COUNT, INVALID_REPRESENTATION = -5, -6
 NO_MORE_CONTEXT, INVALID_EXPONENT, UNSUPPORTED = -9, -10, -11
 CUDA_ERROR, OUT_OF_MEMORY, NO_DEVICE = -20, -21, -22
 POWER_BASIS, NTT = 0, 1
+ENCODING_POLY, ENCODING_SIMD = 0, 1
 
 # every symbol declared in include/fhe_b200.h: name -> (restype, argtypes)
 _u32, _u64, _vp, _i = C.c_uint32, C.c_uint64, C.c_void_p, C.c_int
@@ -55,6 +56,11 @@ SYMBOLS = {
     "fhe_b200_mul_plain": (_i, [_vp, _vp, _u32, _vp]),
     "fhe_b200_add_plain": (_i, [_vp, _vp, _u32, _i, _vp]),
     "fhe_b200_dot_product_scalar": (_i, [_vp, _vp, _u32, _vp, _vp]),
+    "fhe_b200_encoder_create": (_i, [_vp, _vp, _pp]),
+    "fhe_b200_encoder_free": (_i, [_vp]),
+    "fhe_b200_encode": (_i, [_vp, _i, _i, _vp, C.c_size_t, _vp, _vp]),
+    "fhe_b200_mul_plain_batch": (_i, [_vp, _vp, _vp]),
+    "fhe_b200_add_plain_batch": (_i, [_vp, _vp, _i, _vp]),
     "fhe_b200_mul": (_i, [_vp, _vp, _vp, _vp]),
     "fhe_b200_relinearize": (_i, [_vp, _vp, _vp, _vp]),
     "fhe_b200_mul_relin": (_i, [_vp, _vp, _vp, _i, _vp, _vp]),
@@ -75,6 +81,7 @@ SYMBOLS = {
     "fhe_b200_launch_count": (_u64, []),
     "fhe_b200_debug_scaler_tables": (_i, [_vp, _u32, _i, _pu32, _pu32, _pu32] + [_vp] * 8),
     "fhe_b200_debug_ntt_tables": (_i, [_vp, _u64, _vp, _vp, _vp, _vp, _pu64]),
+    "fhe_b200_debug_encoder_tables": (_i, [_vp, _u32, _vp, _vp, _vp, _pu64, _vp]),
 }
 
 _lib = None

@@ -21,7 +21,8 @@ from ._capi import NTT, POWER_BASIS, FheError, check
 from .wire import WireError
 
 __all__ = ["BfvParameters", "BfvParametersBuilder", "Ciphertext", "KeySwitchingKey", "RelinearizationKey", "RGSWCiphertext",
-           "GaloisKey", "EvaluationKey", "Multiplicator", "ScalingFactor", "dot_product_scalar", "FheError", "WireError", "NTT", "POWER_BASIS"]
+           "GaloisKey", "EvaluationKey", "Multiplicator", "ScalingFactor", "dot_product_scalar", "FheError", "WireError", "NTT", "POWER_BASIS",
+           "Encoding", "Plaintext", "PlaintextVec"]
 
 
 def _release(free_name: str, handle) -> None:
@@ -44,8 +45,13 @@ class BfvParameters:
 
     def __init__(self, degree: int, plaintext_modulus: int, moduli: Optional[Sequence[int]] = None,
                  moduli_sizes: Optional[Sequence[int]] = None, psi: Optional[Sequence[int]] = None,
-                 device: int = 0):
+                 device: int = 0, plaintext_psi: Optional[int] = None):
+        """plaintext_psi: the 2N-th root of unity for the plaintext modulus (the reference's
+        NttOperator::new(t).omegas[N/2], for SIMD words interchangeable with a Rust process); None selects the
+        default rule of fhe_b200_params_create."""
         L = _capi.lib()
+        self._enc = None
+        self._plaintext_psi = plaintext_psi
         if (moduli is None) == (moduli_sizes is None):
             # parameters.rs:455-466
             raise FheError(_capi.INVALID_ARGUMENT, "exactly one of moduli / moduli_sizes must be given")
@@ -80,9 +86,36 @@ class BfvParameters:
         self._moduli = [int(x) for x in out]
 
     def __del__(self):
+        e, self._enc = getattr(self, "_enc", None), None
+        if e:
+            _release("fhe_b200_encoder_free", e)
         h, self._h = getattr(self, "_h", None), None
         if h:
             _release("fhe_b200_params_destroy", h)
+
+    def encoder(self):
+        """the fhe_b200_encoder handle (ntt_operator + matrix_reps_index_map, parameters.rs:71-75, :713-726),
+        created on first use"""
+        if self._enc is None:
+            h = C.c_void_p()
+            psi = C.c_uint64(int(self._plaintext_psi)) if self._plaintext_psi is not None else None
+            check(_capi.lib().fhe_b200_encoder_create(self._h, C.byref(psi) if psi is not None else None, C.byref(h)))
+            self._enc = h
+        return self._enc
+
+    def encoder_tables(self, level: int = 0) -> Dict[str, object]:
+        """Host precompute inspection: SIMD index map, NTT tables of t (None when t has no NTT operator), and the
+        level's q_mod_t and delta residues."""
+        L, n = _capi.lib(), self._degree
+        imap, om, zi = np.zeros(n, np.uint32), np.zeros(n, np.uint64), np.zeros(n, np.uint64)
+        qmt, delta = C.c_uint64(), np.zeros(len(self._moduli) - level, np.uint64)
+        code = L.fhe_b200_debug_encoder_tables(self.encoder(), level, None, _ptr(om), _ptr(zi), None, None)
+        if code not in (_capi.OK, _capi.NTT_UNAVAILABLE):
+            check(code)
+        check(L.fhe_b200_debug_encoder_tables(self.encoder(), level, _ptr(imap), None, None, C.byref(qmt), _ptr(delta)))
+        has_ntt = code == _capi.OK
+        return dict(index_map=imap, omegas=om if has_ntt else None, zetas_inv=zi if has_ntt else None,
+                    q_mod_t=qmt.value, delta=delta)
 
     def degree(self) -> int:  # parameters.rs:130
         return self._degree
@@ -386,9 +419,13 @@ class Ciphertext:
         check(_capi.lib().fhe_b200_mul(self._h, rhs._h, out._h, self.stream))
         return out
 
-    def mul_plain(self, poly_ntt: np.ndarray) -> "Ciphertext":
-        """Ciphertext *= &Plaintext (ops/mod.rs:229-238), in place.  poly_ntt: the plaintext's `poly_ntt` words,
-        [limbs][N] (shared by the batch) or [count][limbs][N] (one plaintext per ciphertext)."""
+    def mul_plain(self, poly_ntt) -> "Ciphertext":
+        """Ciphertext *= &Plaintext (ops/mod.rs:229-238), in place.  poly_ntt: a device `Plaintext` / `PlaintextVec`
+        (1 or count entries), or the plaintext's `poly_ntt` words, [limbs][N] (shared by the batch) or
+        [count][limbs][N] (one plaintext per ciphertext)."""
+        if isinstance(poly_ntt, PlaintextVec):
+            check(_capi.lib().fhe_b200_mul_plain_batch(self._h, poly_ntt.batch._h, self.stream))
+            return self
         w = np.ascontiguousarray(poly_ntt, dtype=np.uint64)
         n = 1 if w.ndim == 2 else w.shape[0]
         check(_capi.lib().fhe_b200_mul_plain(self._h, _ptr(w), n, self.stream))
@@ -399,9 +436,13 @@ class Ciphertext:
         check(_capi.lib().fhe_b200_switch_down(self._h, self.stream))
         return self
 
-    def add_plain(self, poly: np.ndarray, subtract: bool = False) -> "Ciphertext":
-        """Ciphertext += &Plaintext / -= &Plaintext (ops/mod.rs:88-97, :188-197), in place: `poly` is the plaintext's
-        `to_poly()` words (delta-scaled, NTT), [limbs][N] shared by the batch or [count][limbs][N]."""
+    def add_plain(self, poly, subtract: bool = False) -> "Ciphertext":
+        """Ciphertext += &Plaintext / -= &Plaintext (ops/mod.rs:88-97, :188-197), in place: `poly` is a device
+        `Plaintext` / `PlaintextVec` (to_poly() is derived on the device), or the plaintext's `to_poly()` words
+        (delta-scaled, NTT), [limbs][N] shared by the batch or [count][limbs][N]."""
+        if isinstance(poly, PlaintextVec):
+            check(_capi.lib().fhe_b200_add_plain_batch(self._h, poly.batch._h, 1 if subtract else 0, self.stream))
+            return self
         w = np.ascontiguousarray(poly, dtype=np.uint64)
         n = 1 if w.ndim == 2 else w.shape[0]
         check(_capi.lib().fhe_b200_add_plain(self._h, _ptr(w), n, 1 if subtract else 0, self.stream))
@@ -434,6 +475,100 @@ class Ciphertext:
         out = Ciphertext(self.par, c, p, lv, r, self.stream, mul_basis=(which == 0))
         check(_capi.lib().fhe_b200_scale(self._h, which, out._h, self.stream))
         return out
+
+
+class Encoding:
+    """fhe::bfv::Encoding (bfv/encoding.rs): Poly or Simd, at a level."""
+
+    def __init__(self, kind: int, level: int = 0):
+        self.kind, self.level = kind, level
+
+    @staticmethod
+    def poly() -> "Encoding":
+        return Encoding(_capi.ENCODING_POLY)
+
+    @staticmethod
+    def simd() -> "Encoding":
+        return Encoding(_capi.ENCODING_SIMD)
+
+    @staticmethod
+    def poly_at_level(level: int) -> "Encoding":
+        return Encoding(_capi.ENCODING_POLY, level)
+
+    @staticmethod
+    def simd_at_level(level: int) -> "Encoding":
+        return Encoding(_capi.ENCODING_SIMD, level)
+
+    def __eq__(self, o):
+        return isinstance(o, Encoding) and (self.kind, self.level) == (o.kind, o.level)
+
+    def __repr__(self):
+        return "Encoding(%s, level=%d)" % ("simd" if self.kind == _capi.ENCODING_SIMD else "poly", self.level)
+
+
+def _values_source(values):
+    """(pointer, count, is_signed, keep-alive) of the values to encode.  numpy arrays (and sequences) live in
+    pageable host memory; a torch tensor may be pinned host or CUDA memory.  The signedness is the dtype's: signed
+    64-bit words are reduced into [0, t) first (the reference's &[i64] encoders), unsigned ones are not."""
+    if hasattr(values, "data_ptr") and hasattr(values, "is_cuda"):   # torch.Tensor
+        import torch
+        if values.dtype not in (torch.int64, torch.uint64) or not values.is_contiguous():
+            raise FheError(_capi.INVALID_ARGUMENT, "expected a contiguous int64 or uint64 tensor")
+        return values.data_ptr(), values.numel(), values.dtype == torch.int64, values
+    a = np.asarray(values)
+    if a.size == 0:
+        a = np.zeros(0, np.uint64)
+    if a.dtype.kind not in "iu" or a.ndim != 1:
+        raise FheError(_capi.INVALID_ARGUMENT, "expected a 1-D array of 64-bit integers")
+    a = np.ascontiguousarray(a, dtype=np.int64 if a.dtype.kind == "i" else np.uint64)
+    return a.ctypes.data, a.size, a.dtype.kind == "i", a
+
+
+class PlaintextVec:
+    """fhe::bfv::PlaintextVec (bfv/plaintext_vec.rs:20-103): `count` plaintexts of one encoding, their poly_ntt
+    resident on the device as a 1-part batch (`batch`, [count][1][limbs][N])."""
+
+    def __init__(self, batch: Ciphertext, encoding: Encoding):
+        self.batch, self.encoding, self.par = batch, encoding, batch.par
+
+    @classmethod
+    def try_encode(cls, values, encoding: Encoding, par: BfvParameters, stream: int = 0):
+        """PlaintextVec::try_encode (plaintext_vec.rs:37-103) on the device: values[k*N, (k+1)*N) become plaintext k.
+        `values`: a 1-D int64 / uint64 numpy array or sequence, or a contiguous torch tensor (pinned host or CUDA)."""
+        ptr, n, signed, keep = _values_source(values)
+        cls._check_count(n, par)
+        count = max(1, -(-n // par.degree()))
+        batch = Ciphertext(par, count, 1, encoding.level, NTT, stream)
+        check(_capi.lib().fhe_b200_encode(par.encoder(), encoding.kind, 1 if signed else 0, ptr if n else None, n,
+                                          batch._h, stream))
+        check(_capi.lib().fhe_b200_sync(stream))   # `values` may be a temporary: it has been read when this returns
+        del keep
+        return cls(batch, encoding)
+
+    @staticmethod
+    def _check_count(n: int, par: BfvParameters):
+        """a PlaintextVec takes any number of values (Plaintext overrides this)"""
+
+    def __len__(self):
+        return self.batch.count
+
+    @property
+    def level(self) -> int:
+        return self.batch.level
+
+    def poly_ntt(self) -> np.ndarray:
+        """the poly_ntt words of every plaintext, [count][limbs][N]"""
+        return self.batch.to_host()[:, 0]
+
+
+class Plaintext(PlaintextVec):
+    """fhe::bfv::Plaintext (bfv/plaintext.rs:20-27): one plaintext, at most N values (TooManyValues otherwise,
+    plaintext.rs:311-345)."""
+
+    @staticmethod
+    def _check_count(n: int, par: BfvParameters):
+        if n > par.degree():
+            raise FheError(_capi.INVALID_ARGUMENT, "TooManyValues: %d, maximum %d" % (n, par.degree()))
 
 
 def _unpack_rq(batch: "Ciphertext", rq_messages, want_rep: int) -> None:
@@ -736,7 +871,9 @@ def dot_product_scalar(cts: "Ciphertext", pts, n_terms: Optional[int] = None) ->
     `cts` is a batch of ciphertexts, `pts` a batch of NTT plaintext polynomials (a one-part `Ciphertext` batch, or
     u64 words [count][limbs][N] = Plaintext::poly_ntt).  With `n_terms` smaller than the batch, the call computes
     count / n_terms independent dot products at once; an operand holding exactly n_terms entries is shared by all of
-    them (the expanded PIR query of examples/mulpir.rs:153-181)."""
+    them (the expanded PIR query of examples/mulpir.rs:153-181).  A device `PlaintextVec` is used in place."""
+    if isinstance(pts, PlaintextVec):
+        pts = pts.batch
     if not isinstance(pts, Ciphertext):
         w = np.ascontiguousarray(pts, dtype=np.uint64)
         if w.ndim != 3:

@@ -32,6 +32,10 @@ struct LevelData {
   ScalerData ext, down;
   bool has_sd = false;
   SwitchDownDev sd;
+  // CipherPlainContext (parameters.rs:604-633): Q_level mod t (when t fits a Modulus) and delta = (-t)^-1 mod q_i
+  u64 q_mod_t = 0;
+  std::vector<u64> delta;
+  const u64 *d_delta = nullptr, *d_delta_s = nullptr;
 };
 
 // Device copy of one RnsScaler's tables (rns/scaler.rs:79-175).  `to_dev` uploads a vector and keeps ownership of the
@@ -81,6 +85,8 @@ struct fhe_b200_params {
   std::vector<u64> moduli, ext, primes, psi;
   std::vector<u32> moduli_sizes;
   BigUint t;
+  bool t_small = false;            // BfvParameters::plaintext.small(): t is a zq::Modulus (2 <= t < 2^62)
+  PlainMod t_mod{0, 0, 0};
   std::vector<NttTablesH> tables;  // host copies (kept for inspection / host-only handles)
   std::vector<LimbDev> h_limbs;
   LimbDev* d_limbs = nullptr;
@@ -165,6 +171,16 @@ struct fhe_b200_params {
       d->sd.inv = to_dev(inv);
       d->sd.inv_s = to_dev(inv_s);
     }
+    if (t_small) d->q_mod_t = from.product.mod_u64(t_mod.t);
+    std::vector<u64> delta_s;
+    for (u64 qi : ctx) {
+      u64 iv;
+      if (!invmod_h(qi - t.mod_u64(qi), qi, &iv)) throw FheError(FHE_B200_INVALID_MODULUS, "PlaintextModulusNotCoprime");
+      d->delta.push_back(iv);
+      delta_s.push_back(ModulusH(qi).shoup(iv));
+    }
+    d->d_delta = to_dev(d->delta);
+    d->d_delta_s = to_dev(delta_s);
     auto* raw = d.get();
     levels[lv] = std::move(d);
     return *raw;
@@ -236,6 +252,31 @@ struct fhe_b200_multiplicator {
   }
   void upload_scaler(ScalerData& sd, const std::vector<u64>& to_moduli) {
     upload_scaler_tables(sd, to_moduli, [&](const auto& v) { return to_dev(v); }, [&](u64 q) { return prime_index(q); });
+  }
+};
+
+// The plaintext side of BfvParameters: the NTT operator of t (parameters.rs:71-75, :598) and the SIMD slot map
+// (matrix_reps_index_map, :713-726).  Its limb table is the parameter set's followed by t, so the level RowIds of
+// the parameter set index it unchanged.
+struct fhe_b200_encoder {
+  const fhe_b200_params* par;
+  bool has_ntt = false;                 // NttOperator::new(t) is Some (ntt/native.rs:35-73)
+  u64 psi_t = 0;
+  NttTablesH tables;                    // of t, when has_ntt
+  std::vector<u32> index_map;           // slot i -> coefficient index
+  std::vector<LimbDev> h_limbs;
+  LimbDev* d_limbs = nullptr;
+  u32* d_inv_map = nullptr;             // coefficient index -> slot
+  RowIds t_ids;                         // one row per plaintext, all modulo t
+  std::vector<void*> d_allocs;
+  template <typename T>
+  T* to_dev(const std::vector<T>& v) {
+    if (par->device < 0 || v.empty()) return nullptr;
+    T* d = nullptr;
+    FHE_CUDA(cudaMalloc(&d, v.size() * sizeof(T)));
+    d_allocs.push_back(d);
+    FHE_CUDA(cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+    return d;
   }
 };
 
@@ -653,6 +694,11 @@ static int params_build(int device, uint32_t degree, const std::vector<u64>& mod
   p->moduli = moduli;
   p->t = BigUint::from_le_bytes(pt, pt_len);
   REQUIRE(!p->t.is_zero(), FHE_B200_INVALID_ARGUMENT, "plaintext modulus is zero");
+  if (p->t.bits() <= 62 && p->t.to_u64() >= 2) {
+    const ModulusH tm(p->t.to_u64());
+    p->t_small = true;
+    p->t_mod = PlainMod{tm.p, tm.bhi, tm.blo};
+  }
   // validate_moduli (parameters.rs:471-552)
   BigUint Q(1);
   for (size_t i = 0; i < moduli.size(); i++) {
@@ -1007,6 +1053,182 @@ int fhe_b200_dot_product_scalar(const fhe_b200_batch* cts, const fhe_b200_batch*
              cts->par->d_limbs, cts->par->logn, (cudaStream_t)stream);
   FHE_CUDA(cudaGetLastError());
   out->repr = FHE_B200_NTT;
+  API_END
+}
+
+// ---- plaintext encoding
+int fhe_b200_encoder_create(const fhe_b200_params* p, const uint64_t* psi_t, fhe_b200_encoder** out) {
+  API_BEGIN
+  REQUIRE(p && out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  ScopedDevice g(p->device);
+  std::unique_ptr<fhe_b200_encoder> e(new fhe_b200_encoder());
+  struct Cleanup {   // frees the device tables if construction throws
+    fhe_b200_encoder* e;
+    ~Cleanup() { if (e) { for (void* d : e->d_allocs) cudaFree(d); cudaGetLastError(); } }
+  } cleanup{e.get()};
+  e->par = p;
+  const u32 N = p->N;
+  // parameters.rs:713-726
+  e->index_map.resize(N);
+  auto brev = [&](u64 x) {
+    u32 r = 0;
+    for (u32 b = 0; b < p->logn; b++) r |= (u32)((x >> b) & 1) << (p->logn - 1 - b);
+    return r;
+  };
+  const u64 m = 2 * (u64)N;
+  u64 pos = 1;
+  for (u32 i = 0; i < N / 2; i++) {
+    e->index_map[i] = brev((pos - 1) >> 1);
+    e->index_map[N / 2 + i] = brev((m - pos - 1) >> 1);
+    pos = (pos * 3) & (m - 1);
+  }
+  std::vector<u32> inv(N);
+  for (u32 i = 0; i < N; i++) inv[e->index_map[i]] = i;
+  e->h_limbs = p->h_limbs;
+  std::memset(&e->t_ids, 0, sizeof(RowIds));
+  e->t_ids.limbs_per_poly = 1;
+  e->t_ids.ids[0] = (unsigned short)p->h_limbs.size();
+  // NttOperator::new (ntt/native.rs:35-73): t is a Modulus, prime, and 1 mod 2N
+  const u64 t = p->t_mod.t;
+  e->has_ntt = p->t_small && t % m == 1 && is_prime_u64(t);
+  if (e->has_ntt) {
+    e->psi_t = psi_t ? *psi_t : default_psi(t, N);
+    e->tables = make_ntt_tables(t, N, e->psi_t);
+    e->h_limbs.push_back(make_limb_dev(t, e->tables, [&](const std::vector<ulonglong2>& v) { return e->to_dev(v); }));
+  }
+  e->d_limbs = e->to_dev(e->h_limbs);
+  e->d_inv_map = e->to_dev(inv);
+  params_retain(p);
+  cleanup.e = nullptr;
+  *out = e.release();
+  API_END
+}
+
+int fhe_b200_encoder_free(fhe_b200_encoder* e) {
+  if (!e) return FHE_B200_OK;
+  if (e->par->device >= 0) {
+    ScopedDevice g(e->par->device);
+    for (void* d : e->d_allocs) cudaFree(d);
+    cudaGetLastError();
+  }
+  params_release(e->par);
+  delete e;
+  return FHE_B200_OK;
+}
+
+int fhe_b200_encode(const fhe_b200_encoder* e, int encoding, int is_signed, const void* values, size_t n_values,
+                    fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  REQUIRE(e, FHE_B200_INVALID_ARGUMENT, "null encoder");
+  const fhe_b200_params* par = e->par;
+  DeviceGuard g(par);
+  REQUIRE(out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  REQUIRE(encoding == FHE_B200_ENCODING_POLY || encoding == FHE_B200_ENCODING_SIMD, FHE_B200_INVALID_ARGUMENT,
+          "unknown encoding");
+  REQUIRE(par->t_small, FHE_B200_UNSUPPORTED, "the plaintext modulus does not fit a u64 Modulus");
+  const bool simd = encoding == FHE_B200_ENCODING_SIMD;
+  REQUIRE(!simd || e->has_ntt, FHE_B200_NTT_UNAVAILABLE, "EncodingError::SimdUnavailable");   // plaintext_vec.rs:47
+  REQUIRE(out->par == par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch");
+  REQUIRE(!out->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
+  const LevelData& lv = par->level(out->level);
+  REQUIRE(out->parts == 1, FHE_B200_BAD_POLY_COUNT, "a plaintext batch has one polynomial per entry");
+  const size_t N = par->N;
+  const size_t count = std::max<size_t>(1, (n_values + N - 1) / N);
+  REQUIRE(out->count == count, FHE_B200_INVALID_ARGUMENT, "batch must hold max(1, ceil(n_values / N)) plaintexts");
+  REQUIRE(values || !n_values, FHE_B200_INVALID_ARGUMENT, "null values");
+  const u32 L = lv.L, logn = par->logn;
+  const bool poly_u64 = !simd && !is_signed;
+  // forward butterflies take inputs below 4 q_j: Poly u64 words are arbitrary, the other words are below t
+  u64 qmin = ~0ull;
+  for (u32 j = 0; j < L; j++) qmin = std::min(qmin, par->moduli[j]);
+  const bool reduce = poly_u64 || par->t_mod.t > 4 * qmin - 1;
+  const char* src = (const char*)values;
+  ChunkRunner chunks(par, (u32)count, (cudaStream_t)stream);
+  chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace ws(par, st);
+    const size_t v0 = (size_t)c0 * N, vn = n_values > v0 ? std::min(n_values - v0, (size_t)n * N) : 0;
+    u64* staged = ws.words(std::max<size_t>(vn, 1));
+    if (vn) FHE_CUDA(cudaMemcpyAsync(staged, src + v0 * sizeof(u64), vn * sizeof(u64), cudaMemcpyDefault, st));
+    const u64* coeffs = staged;
+    if (!(poly_u64 && vn == (size_t)n * N)) {
+      u64* c = ws.words((size_t)n * N);
+      launch_encode_load(staged, c, n, vn, simd ? e->d_inv_map : nullptr, is_signed != 0, par->t_mod, logn, st);
+      if (simd) launch_ntt(c, c, n, e->t_ids, e->d_limbs, logn, true, 1, false, st);   // NttOperator::backward mod t
+      coeffs = c;
+    }
+    // try_convert_from + into_ntt: every limb of plaintext k transforms row k of `coeffs`
+    launch_ntt(coeffs, out->d + (size_t)c0 * L * N, n * L, lv.ctx_ids, e->d_limbs, logn, false, L, reduce, st);
+  });
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
+  API_END
+}
+
+// pts: 1-part NTT batch at a's level with 1 or a->count entries (the checks of plain_op plus the batch's shape)
+static void check_plain_batch(const fhe_b200_batch* a, const fhe_b200_batch* pts) {
+  REQUIRE(a && pts, FHE_B200_INVALID_ARGUMENT, "null argument");
+  check_same(a, pts);
+  REQUIRE(pts->count == 1 || pts->count == a->count, FHE_B200_INVALID_ARGUMENT, "plaintext count must be 1 or the batch size");
+  REQUIRE(a->parts >= 1 && pts->parts == 1, FHE_B200_BAD_POLY_COUNT, "plaintext batch must hold one polynomial per entry");
+  need_repr(a, FHE_B200_NTT);
+  need_repr(pts, FHE_B200_NTT);
+}
+
+int fhe_b200_mul_plain_batch(fhe_b200_batch* a, const fhe_b200_batch* pts, void* stream) {
+  API_BEGIN
+  check_plain_batch(a, pts);
+  DeviceGuard g(a->par);
+  launch_mul_plain(a->d, pts->d, a->count, a->parts, pts->count, ids_of(a), a->par->d_limbs, a->par->logn,
+                   (cudaStream_t)stream, 0);
+  FHE_CUDA(cudaGetLastError());
+  API_END
+}
+
+int fhe_b200_add_plain_batch(fhe_b200_batch* a, const fhe_b200_batch* pts, int subtract, void* stream) {
+  API_BEGIN
+  check_plain_batch(a, pts);
+  const fhe_b200_params* par = a->par;
+  REQUIRE(par->t_small && par->t_mod.t < par->moduli[0], FHE_B200_UNSUPPORTED,
+          "to_poly needs t below the first ciphertext modulus");
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(a->level);
+  const u32 L = lv.L, logn = par->logn;
+  const size_t N = par->N;
+  u64 qmin = ~0ull;
+  for (u32 j = 0; j < L; j++) qmin = std::min(qmin, par->moduli[j]);
+  const bool reduce = par->t_mod.t > 4 * qmin - 1;
+  RowIds q0_ids;
+  std::memset(&q0_ids, 0, sizeof(RowIds));
+  q0_ids.limbs_per_poly = 1;
+  // Plaintext::to_poly of plaintexts [p0, p0 + n) into m [n][L][N] (before the delta product)
+  auto to_poly = [&](u32 p0, u32 n, u64* m, Workspace& ws, cudaStream_t st) {
+    u64* x = ws.words((size_t)n * N);
+    FHE_CUDA(cudaMemcpy2DAsync(x, N * 8, pts->d + (size_t)p0 * L * N, L * N * 8, N * 8, n, cudaMemcpyDeviceToDevice, st));
+    launch_ntt(x, x, n, q0_ids, par->d_limbs, logn, true, 1, false, st);      // limb 0 of into_power_basis
+    launch_to_poly_load(x, (size_t)n * N, par->t_mod, lv.q_mod_t, st);
+    launch_ntt(x, m, n * L, lv.ctx_ids, par->d_limbs, logn, false, L, reduce, st);
+  };
+  cudaStream_t user = (cudaStream_t)stream;
+  Workspace shared_ws(par, user);
+  const bool shared = pts->count == 1;
+  u64* m_shared = nullptr;
+  if (shared) {   // built once, before the chunks' side streams fork from `user`
+    m_shared = shared_ws.words((size_t)L * N);
+    to_poly(0, 1, m_shared, shared_ws, user);
+  }
+  ChunkRunner chunks(par, a->count, user);
+  chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace ws(par, st);
+    const u64* m = m_shared;
+    if (!shared) {
+      u64* mc = ws.words((size_t)n * L * N);
+      to_poly(c0, n, mc, ws, st);
+      m = mc;
+    }
+    launch_add_scaled(a->d + (size_t)c0 * a->parts * L * N, m, n, a->parts, shared ? 1 : n, lv.d_delta, lv.d_delta_s,
+                      subtract != 0, lv.ctx_ids, par->d_limbs, logn, st);
+  });
+  FHE_CUDA(cudaGetLastError());
   API_END
 }
 
@@ -1547,6 +1769,26 @@ int fhe_b200_debug_ntt_tables(const fhe_b200_params* p, uint64_t q, uint64_t* om
   cp(zetas_inv, t.zi);
   cp(zetas_inv_shoup, t.zi_s);
   if (size_inv) *size_inv = t.ninv;
+  API_END
+}
+
+int fhe_b200_debug_encoder_tables(const fhe_b200_encoder* e, uint32_t level, uint32_t* index_map, uint64_t* omegas,
+                                  uint64_t* zetas_inv, uint64_t* q_mod_t, uint64_t* delta) {
+  API_BEGIN
+  REQUIRE(e, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* p = e->par;
+  const LevelData& lv = p->level(level);
+  if (index_map) std::copy(e->index_map.begin(), e->index_map.end(), index_map);
+  if (omegas || zetas_inv) {
+    REQUIRE(e->has_ntt, FHE_B200_NTT_UNAVAILABLE, "NttOperatorUnavailable: plaintext modulus");
+    if (omegas) std::copy(e->tables.om.begin(), e->tables.om.end(), omegas);
+    if (zetas_inv) std::copy(e->tables.zi.begin(), e->tables.zi.end(), zetas_inv);
+  }
+  if (q_mod_t) {
+    REQUIRE(p->t_small, FHE_B200_UNSUPPORTED, "the plaintext modulus does not fit a u64 Modulus");
+    *q_mod_t = lv.q_mod_t;
+  }
+  if (delta) std::copy(lv.delta.begin(), lv.delta.end(), delta);
   API_END
 }
 

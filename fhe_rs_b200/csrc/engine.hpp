@@ -133,6 +133,24 @@ struct SwitchDownDev {
 void launch_switch_down(const SwitchDownDev& S, const u64* in, u64* out, u32 polys, u32 L, const RowIds& ids,
                         const LimbDev* limbs, u32 logn, cudaStream_t st);
 
+// ---- plaintext encoding (plaintext_vec.rs:37-103, plaintext.rs:103-197)
+// constants of the plaintext modulus t (a zq::Modulus, t < 2^62)
+struct PlainMod {
+  u64 t, bhi, blo;
+};
+// coeffs [n_pt][N]: word c of plaintext k is value k*N + (inv_map ? inv_map[c] : c) of `staged` (the SIMD scatter
+// coeffs[map[i]] = v[i] written as a gather), or 0 past n_values; is_signed: the values are i64, reduced into [0, t)
+// (Modulus::reduce_vec_i64)
+void launch_encode_load(const u64* staged, u64* coeffs, u32 n_pt, size_t n_values, const u32* inv_map, bool is_signed,
+                        const PlainMod& T, u32 logn, cudaStream_t st);
+// Plaintext::to_poly from power-basis residues modulo q_0 (t < q_0, plaintext.rs:103-135, :172-181), in place:
+// x <- ((x mod t) * q_mod_t) mod t
+void launch_to_poly_load(u64* x, size_t n_words, const PlainMod& T, u64 q_mod_t, cudaStream_t st);
+// a[ct][0][j][:] +/-= m[ct % n_pt][j][:] * delta[j] mod q_j   (delta_s: Shoup companions; plaintext.rs:195 and
+// ops/mod.rs:88-97, :188-197)
+void launch_add_scaled(u64* a, const u64* m, u32 cts, u32 parts, u32 n_pt, const u64* delta, const u64* delta_s,
+                       bool subtract, const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st);
+
 // bit (un)packing of power-basis rows (fhe-util/src/lib.rs:71-146): row r of `rows` uses nbits[r % limbs] bits per
 // coefficient; packed row r starts at byte  (r / limbs) * poly_bytes + offs[r % limbs]
 struct PackDev {

@@ -973,11 +973,90 @@ __global__ void unpack_kernel(PackDev P, const unsigned char* bytes, u64* words,
   }
 }
 
+// ------------------------------------------------------------------ plaintext encoding
+// one thread per (plaintext, coefficient): reads are coalesced for Poly, writes always are
+__global__ void encode_load_kernel(const u64* staged, u64* coeffs, size_t n_words, size_t n_values, const u32* inv_map,
+                                   u32 is_signed, PlainMod T, u32 logn) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_words) return;
+  const u32 c = (u32)i & ((1u << logn) - 1);
+  const size_t v = inv_map ? ((i >> logn) << logn) + inv_map[c] : i;
+  u64 w = 0;
+  if (v < n_values) {
+    w = staged[v];
+    if (is_signed) {   // zq/mod.rs reduce_i64: the canonical residue of a signed word
+      const bool neg = (long long)w < 0;
+      const u64 r = barrett64(neg ? 0 - w : w, T.t, T.bhi, T.blo);
+      w = (neg && r) ? T.t - r : r;
+    }
+  }
+  coeffs[i] = w;
+}
+
+__global__ void to_poly_load_kernel(u64* x, size_t n_words, PlainMod T, u64 q_mod_t) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_words) return;
+  x[i] = mulmod(barrett64(x[i], T.t, T.bhi, T.blo), q_mod_t, T.t, T.bhi, T.blo);   // Modulus::scalar_mul_vec
+}
+
+struct AddScaledArgs {
+  u64* a;
+  const u64* m;
+  const u64 *delta, *delta_s;
+  u32 cts, parts, n_pt, logn, limbs_per_poly, subtract;
+  const LimbDev* limbs;
+  unsigned short ids[kMaxPos];
+};
+// delta is a constant in every NTT slot (parameters.rs:604-633), so m * delta is one Shoup product per word
+__global__ void add_scaled_kernel(AddScaledArgs A) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t total = ((size_t)A.cts * A.limbs_per_poly) << A.logn;
+  if (idx >= total) return;
+  const u32 c = (u32)idx & ((1u << A.logn) - 1);
+  const size_t row = idx >> A.logn;
+  const u32 j = (u32)(row % A.limbs_per_poly), ct = (u32)(row / A.limbs_per_poly);
+  const u64 p = A.limbs[A.ids[j]].p;
+  const u64 w = mul_shoup(A.m[((((size_t)(ct % A.n_pt)) * A.limbs_per_poly + j) << A.logn) + c], A.delta[j],
+                          A.delta_s[j], p);
+  u64* dst = A.a + ((((size_t)ct * A.parts) * A.limbs_per_poly + j) << A.logn) + c;
+  const u64 x = *dst;
+  *dst = A.subtract ? csub(x + p - w, p) : csub(x + w, p);
+}
+
 void copy_ids(unsigned short* dst, const RowIds& ids) {
   for (int i = 0; i < kMaxPos; i++) dst[i] = ids.ids[i];
 }
 
 }  // namespace
+
+void launch_encode_load(const u64* staged, u64* coeffs, u32 n_pt, size_t n_values, const u32* inv_map, bool is_signed,
+                        const PlainMod& T, u32 logn, cudaStream_t st) {
+  const size_t n_words = (size_t)n_pt << logn;
+  if (!n_words) return;
+  encode_load_kernel<<<(unsigned)((n_words + 255) / 256), 256, 0, st>>>(staged, coeffs, n_words, n_values, inv_map,
+                                                                         is_signed ? 1 : 0, T, logn);
+  g_launches++;
+}
+
+void launch_to_poly_load(u64* x, size_t n_words, const PlainMod& T, u64 q_mod_t, cudaStream_t st) {
+  if (!n_words) return;
+  to_poly_load_kernel<<<(unsigned)((n_words + 255) / 256), 256, 0, st>>>(x, n_words, T, q_mod_t);
+  g_launches++;
+}
+
+void launch_add_scaled(u64* a, const u64* m, u32 cts, u32 parts, u32 n_pt, const u64* delta, const u64* delta_s,
+                       bool subtract, const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st) {
+  AddScaledArgs A;
+  A.a = a; A.m = m; A.delta = delta; A.delta_s = delta_s;
+  A.cts = cts; A.parts = parts; A.n_pt = n_pt; A.logn = logn; A.limbs_per_poly = ids.limbs_per_poly;
+  A.subtract = subtract ? 1 : 0;
+  A.limbs = limbs;
+  copy_ids(A.ids, ids);
+  const size_t total = ((size_t)cts * ids.limbs_per_poly) << logn;
+  if (!total) return;
+  add_scaled_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(A);
+  g_launches++;
+}
 
 void launch_ew(EwOp op, u64* a, const u64* b, size_t n_rows, const RowIds& ids, const LimbDev* limbs, u32 logn,
                cudaStream_t st) {

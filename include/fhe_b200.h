@@ -69,6 +69,11 @@ typedef struct fhe_b200_batch fhe_b200_batch;   /* == Vec<Ciphertext> of one lev
 typedef struct fhe_b200_ksk fhe_b200_ksk;       /* == KeySwitchingKey (bfv/keys/key_switching_key.rs:22-45)     */
 typedef struct fhe_b200_multiplicator fhe_b200_multiplicator; /* == Multiplicator with a custom strategy
                                                    (bfv/ops/mul.rs:22-98)                                        */
+typedef struct fhe_b200_encoder fhe_b200_encoder; /* == the plaintext side of BfvParameters: the NTT operator of t
+                                                     and the SIMD slot map (parameters.rs:71-75, :713-726)      */
+
+/* Encoding (bfv/encoding.rs): the level comes from the output batch (Encoding::{poly,simd}_at_level). */
+typedef enum { FHE_B200_ENCODING_POLY = 0, FHE_B200_ENCODING_SIMD = 1 } fhe_b200_encoding;
 
 const char* fhe_b200_version(void);
 const char* fhe_b200_last_error(void);
@@ -161,6 +166,39 @@ int fhe_b200_add_plain(fhe_b200_batch* a, const uint64_t* host_polys, uint32_t n
  * CiphertextPolynomialCountMismatch -> BAD_POLY_COUNT, mixed levels -> INVALID_LEVEL. */
 int fhe_b200_dot_product_scalar(const fhe_b200_batch* cts, const fhe_b200_batch* pts, uint32_t n_terms,
                                 fhe_b200_batch* out, void* stream);
+
+/* ---- plaintexts on the device ---------------------------------------------------------------
+ * A device plaintext batch is an fhe_b200_batch with 1 part, in the NTT representation: entry k holds
+ * Plaintext::poly_ntt of one plaintext (plaintext.rs:20-27), at the level of its encoding.
+ * Encoder handle: psi_t (nullable) is the 2N-th root of unity for t, as `psi` of fhe_b200_params_create
+ * (a Rust host passes NttOperator::new(t).omegas[N/2], NULL selects the default rule).  Creation succeeds on every
+ * valid parameter set, host-only ones included; when t has no NTT operator (t not prime, or t != 1 mod 2N) SIMD
+ * encoding fails with FHE_B200_NTT_UNAVAILABLE (EncodingError::SimdUnavailable) and Poly encoding still works.
+ * The handle holds a reference on the parameter set. */
+int fhe_b200_encoder_create(const fhe_b200_params* p, const uint64_t* psi_t, fhe_b200_encoder** out);
+int fhe_b200_encoder_free(fhe_b200_encoder* e);
+/* PlaintextVec::try_encode (plaintext_vec.rs:37-103) of n_values u64 (is_signed == 0) or i64 (is_signed != 0) words
+ * into `out`, a 1-part batch of max(1, ceil(n_values / N)) entries at the encoding level; entry k encodes
+ * values[k*N, min(n_values, (k+1)*N)) and zero in its other slots; `out` becomes NTT.
+ *  - POLY, u64: the words are coefficients, not reduced mod t; each is reduced modulo every q_i (rq/convert.rs:160-183).
+ *  - SIMD, u64: slot i holds values[i]; the values must be below t (the reference's NTT assumes reduced input).
+ *  - i64 (either encoding): each word is first reduced into [0, t) (Modulus::reduce_vec_i64, plaintext.rs:347-372).
+ *  - At a level with a single modulus q_0 the reference keeps the N coefficient words unreduced (rq/convert.rs:150-159)
+ *    while the device reduces every word: the results agree for words below q_0 (SIMD words and reduced i64 words are
+ *    below t, so they differ only for t > q_0).
+ * values: pageable host, pinned host or device memory, copied with cudaMemcpyDefault and only enqueued, as for
+ * fhe_b200_batch_upload.  Errors: t beyond a u64 Modulus -> UNSUPPORTED; SIMD without an NTT for t -> NTT_UNAVAILABLE;
+ * parts != 1 -> BAD_POLY_COUNT; wrong count, NULL values with n_values > 0 -> INVALID_ARGUMENT; host-only
+ * parameters -> NO_DEVICE. */
+int fhe_b200_encode(const fhe_b200_encoder* e, int encoding, int is_signed, const void* values, size_t n_values,
+                    fhe_b200_batch* out, void* stream);
+/* fhe_b200_mul_plain with a device plaintext batch (ops/mod.rs:229-238): pts holds 1 (shared) or a.count entries at
+ * a's level.  Same checks and error codes, plus BAD_POLY_COUNT when pts has more than one part. */
+int fhe_b200_mul_plain_batch(fhe_b200_batch* a, const fhe_b200_batch* pts, void* stream);
+/* fhe_b200_add_plain with a device plaintext batch (ops/mod.rs:88-97, :188-197): Plaintext::to_poly is derived from
+ * poly_ntt on the device as the reference does (plaintext.rs:103-135, :172-197).  t >= q_0 -> UNSUPPORTED. */
+int fhe_b200_add_plain_batch(fhe_b200_batch* a, const fhe_b200_batch* pts, int subtract, void* stream);
+
 /* &Ciphertext * &Ciphertext (bfv/ops/mod.rs:259-358): n parts x m parts -> n + m - 1 parts (out3 must have that many;
  * 2 x 2 -> 3 is the fused path) */
 int fhe_b200_mul(const fhe_b200_batch* a, const fhe_b200_batch* b, fhe_b200_batch* out3, void* stream);
@@ -255,6 +293,10 @@ int fhe_b200_debug_scaler_tables(const fhe_b200_params* p, uint32_t level, int w
 /* NTT tables of prime q: any of omegas/zetas_inv (N words each) may be NULL. */
 int fhe_b200_debug_ntt_tables(const fhe_b200_params* p, uint64_t q, uint64_t* omegas, uint64_t* omegas_shoup,
                               uint64_t* zetas_inv, uint64_t* zetas_inv_shoup, uint64_t* size_inv);
+/* Encoder tables: matrix_reps_index_map (N words), the NTT tables of t (N words each; NTT_UNAVAILABLE when t has none),
+ * and for `level` q_mod_t (one word) and delta = (-t)^-1 mod q_i (one word per limb).  Any output may be NULL. */
+int fhe_b200_debug_encoder_tables(const fhe_b200_encoder* e, uint32_t level, uint32_t* index_map, uint64_t* omegas,
+                                  uint64_t* zetas_inv, uint64_t* q_mod_t, uint64_t* delta);
 
 #ifdef __cplusplus
 }

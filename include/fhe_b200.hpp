@@ -8,6 +8,7 @@
 //   bfv::RGSWCiphertext                         bfv/rgsw_ciphertext.rs:20 (external product = two key switches)
 //   bfv::GaloisKey / EvaluationKey              bfv/keys/galois_key.rs:18, evaluation_key.rs:110-170
 //   bfv::Multiplicator                          bfv/ops/mul.rs:22
+//   bfv::Encoding / Plaintext / PlaintextVec    bfv/encoding.rs, bfv/plaintext.rs:20, plaintext_vec.rs:20
 // Fallible reference calls return Result<_, fhe::Error>; here they throw fhe_b200::Error carrying
 // the fhe_b200_status code (same variants, see fhe_b200.h).
 #pragma once
@@ -15,6 +16,7 @@
 #include <map>
 #include <algorithm>
 #include <memory>
+#include <mutex>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -40,7 +42,6 @@ class BfvParameters {
  public:
   BfvParameters(const BfvParameters&) = delete;
   BfvParameters& operator=(const BfvParameters&) = delete;
-  ~BfvParameters() { fhe_b200_params_destroy(h_); }
   size_t degree() const { return fhe_b200_params_degree(h_); }
   std::vector<uint64_t> moduli() const {
     std::vector<uint64_t> m(fhe_b200_params_n_moduli(h_));
@@ -56,11 +57,26 @@ class BfvParameters {
     return m;
   }
   const fhe_b200_params* handle() const { return h_; }
+  // ntt_operator + matrix_reps_index_map of the plaintext modulus (parameters.rs:71-75, :713-726), built on first use
+  const fhe_b200_encoder* encoder() const {
+    std::call_once(enc_once_, [this] {
+      check(fhe_b200_encoder_create(h_, has_plaintext_psi_ ? &plaintext_psi_ : nullptr, &enc_));
+    });
+    return enc_;
+  }
 
  private:
   friend class BfvParametersBuilder;
-  explicit BfvParameters(fhe_b200_params* h) : h_(h) {}
+  BfvParameters(fhe_b200_params* h, bool has_psi_t, uint64_t psi_t)
+      : h_(h), has_plaintext_psi_(has_psi_t), plaintext_psi_(psi_t) {}
   fhe_b200_params* h_;
+  bool has_plaintext_psi_;
+  uint64_t plaintext_psi_;
+  mutable std::once_flag enc_once_;
+  mutable fhe_b200_encoder* enc_ = nullptr;
+
+ public:
+  ~BfvParameters() { fhe_b200_encoder_free(enc_); fhe_b200_params_destroy(h_); }
 };
 
 class BfvParametersBuilder {
@@ -71,6 +87,8 @@ class BfvParametersBuilder {
   BfvParametersBuilder& set_moduli_sizes(const std::vector<uint32_t>& s) { sizes_ = s; return *this; }
   BfvParametersBuilder& set_ntt_roots(const std::vector<uint64_t>& psi) { psi_ = psi; return *this; }
   BfvParametersBuilder& set_device(int device) { device_ = device; return *this; }
+  // 2N-th root for the plaintext modulus (the reference's NttOperator::new(t).omegas[N/2]); default rule otherwise
+  BfvParametersBuilder& set_plaintext_ntt_root(uint64_t psi_t) { psi_t_ = psi_t; has_psi_t_ = true; return *this; }
   // BfvParametersBuilder::build_arc (bfv/parameters.rs:555)
   std::shared_ptr<BfvParameters> build_arc() const {
     uint8_t pt[8];
@@ -83,12 +101,14 @@ class BfvParametersBuilder {
                                    psi_.empty() ? nullptr : psi_.data(), &h));
     else
       check(fhe_b200_params_create_from_sizes(device_, degree_, sizes_.data(), (uint32_t)sizes_.size(), pt, 8, &h));
-    return std::shared_ptr<BfvParameters>(new BfvParameters(h));
+    return std::shared_ptr<BfvParameters>(new BfvParameters(h, has_psi_t_, psi_t_));
   }
 
  private:
   uint32_t degree_ = 0;
   uint64_t plaintext_ = 0;
+  uint64_t psi_t_ = 0;
+  bool has_psi_t_ = false;
   std::vector<uint64_t> moduli_, psi_;
   std::vector<uint32_t> sizes_;
   int device_ = 0;
@@ -115,6 +135,8 @@ class PinnedWords {
   uint64_t* p_ = nullptr;
   size_t n_ = 0;
 };
+
+class PlaintextVec;
 
 class Ciphertext {
  public:
@@ -177,6 +199,9 @@ class Ciphertext {
     check(fhe_b200_mul_plain(h_, poly_ntt.data(), 1, stream_));
     return *this;
   }
+  // the same with device plaintexts (1 shared, or one per ciphertext); to_poly() is derived on the device
+  inline Ciphertext& mul_plain(const PlaintextVec& pts);
+  inline Ciphertext& add_plain(const PlaintextVec& pts, bool subtract = false);
   // Poly::into_ntt / into_power_basis on every polynomial (rq/mod.rs:535, :590)
   Ciphertext& into_ntt() { check(fhe_b200_ntt_forward(h_, stream_)); return *this; }
   Ciphertext& into_power_basis() { check(fhe_b200_ntt_backward(h_, stream_)); return *this; }
@@ -230,6 +255,73 @@ class Ciphertext {
   fhe_b200_batch* h_ = nullptr;
   void* stream_ = nullptr;
 };
+
+// fhe::bfv::Encoding (bfv/encoding.rs)
+struct Encoding {
+  int kind;
+  uint32_t level;
+  static Encoding poly() { return {FHE_B200_ENCODING_POLY, 0}; }
+  static Encoding simd() { return {FHE_B200_ENCODING_SIMD, 0}; }
+  static Encoding poly_at_level(uint32_t level) { return {FHE_B200_ENCODING_POLY, level}; }
+  static Encoding simd_at_level(uint32_t level) { return {FHE_B200_ENCODING_SIMD, level}; }
+};
+
+// fhe::bfv::PlaintextVec (bfv/plaintext_vec.rs:20-103): the poly_ntt of every plaintext in a 1-part device batch.
+// `values` of try_encode may be host (pageable or PinnedWords) or device memory; SIMD values must be below t.
+class PlaintextVec {
+ public:
+  static PlaintextVec try_encode(const uint64_t* values, size_t n, const Encoding& e,
+                                 const std::shared_ptr<BfvParameters>& par) {
+    return encode(values, n, false, e, par);
+  }
+  static PlaintextVec try_encode(const int64_t* values, size_t n, const Encoding& e,
+                                 const std::shared_ptr<BfvParameters>& par) {
+    return encode(values, n, true, e, par);
+  }
+  template <typename T>
+  static PlaintextVec try_encode(const std::vector<T>& values, const Encoding& e, const std::shared_ptr<BfvParameters>& par) {
+    return try_encode(values.data(), values.size(), e, par);
+  }
+  size_t len() const { return batch_.count(); }
+  const Encoding& encoding() const { return encoding_; }
+  const Ciphertext& batch() const { return batch_; }
+  std::vector<uint64_t> poly_ntt() const { return batch_.to_host(); }   // [count][limbs][N]
+
+ protected:
+  PlaintextVec(Ciphertext b, const Encoding& e) : batch_(std::move(b)), encoding_(e) {}
+  static PlaintextVec encode(const void* values, size_t n, bool is_signed, const Encoding& e,
+                             const std::shared_ptr<BfvParameters>& par) {
+    const size_t N = par->degree();
+    Ciphertext b(par, (uint32_t)std::max<size_t>(1, (n + N - 1) / N), 1, e.level, Representation::Ntt);
+    check(fhe_b200_encode(par->encoder(), e.kind, is_signed ? 1 : 0, values, n, b.handle(), b.stream()));
+    b.sync();   // `values` may be released by the caller once this returns
+    return PlaintextVec(std::move(b), e);
+  }
+  Ciphertext batch_;
+  Encoding encoding_;
+};
+
+// fhe::bfv::Plaintext (bfv/plaintext.rs:20-27): one plaintext of at most N values (TooManyValues, :311-345)
+class Plaintext : public PlaintextVec {
+ public:
+  template <typename T>
+  static Plaintext try_encode(const std::vector<T>& values, const Encoding& e, const std::shared_ptr<BfvParameters>& par) {
+    if (values.size() > par->degree()) throw Error(FHE_B200_INVALID_ARGUMENT, "TooManyValues");
+    return Plaintext(PlaintextVec::try_encode(values, e, par));
+  }
+
+ private:
+  explicit Plaintext(PlaintextVec&& v) : PlaintextVec(std::move(v)) {}
+};
+
+inline Ciphertext& Ciphertext::mul_plain(const PlaintextVec& pts) {
+  check(fhe_b200_mul_plain_batch(h_, pts.batch().handle(), stream_));
+  return *this;
+}
+inline Ciphertext& Ciphertext::add_plain(const PlaintextVec& pts, bool subtract) {
+  check(fhe_b200_add_plain_batch(h_, pts.batch().handle(), subtract ? 1 : 0, stream_));
+  return *this;
+}
 
 class KeySwitchingKey {
  public:
@@ -336,6 +428,9 @@ inline Ciphertext dot_product_scalar(const Ciphertext& cts, const Ciphertext& pt
   Ciphertext out(cts.par(), groups ? groups : 1, cts.len(), cts.level(), Representation::Ntt, cts.stream());
   check(fhe_b200_dot_product_scalar(cts.handle(), pts.handle(), n_terms, out.handle(), cts.stream()));
   return out;
+}
+inline Ciphertext dot_product_scalar(const Ciphertext& cts, const PlaintextVec& pts, uint32_t n_terms) {
+  return dot_product_scalar(cts, pts.batch(), n_terms);
 }
 
 // fhe_math::rns::ScalingFactor (rns/scaler.rs:20-58): numerator / denominator as little-endian byte strings

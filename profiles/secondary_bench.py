@@ -65,4 +65,28 @@ rd = B * (ct_bytes + ct_bytes // 2)
 out["dot_product_scalar"] = {"terms_per_s": B / s, "n_terms": n_terms, "gbs": rd / s / 1e9, "hbm_frac": rd / s / 1e9 / hbm}
 s = timed(lambda: A.to_packed(), reps=2, warm=1)
 out["wire_pack_to_host"] = {"ct_per_s": B / s, "note": "inverse NTT + 62-bit packing + download to pageable host memory"}
+
+# plaintexts: B SIMD plaintexts of N slot values (B*N u64) against the B*L*N poly_ntt words they encode to
+from fhe_rs_b200 import _capi  # noqa: E402
+lib = _capi.lib()
+n_vals = B * DEGREE
+slots = torch.from_numpy(rng.integers(0, PLAINTEXT, size=n_vals, dtype=np.int64))
+slots_pinned, slots_dev = slots.pin_memory(), slots.cuda()
+PT = F.Ciphertext(par, B, 1)
+enc = par.encoder()
+for name, src in (("encode_simd_pinned_host", slots_pinned), ("encode_simd_device", slots_dev)):
+    s = timed(lambda: _capi.check(lib.fhe_b200_encode(enc, _capi.ENCODING_SIMD, 1, src.data_ptr(), n_vals, PT._h, 0)))
+    out[name] = {"pt_per_s": B / s, "input_mb": n_vals * 8 / 1e6}
+words_pinned = torch.empty(B * N_MODULI * DEGREE, dtype=torch.int64).pin_memory()
+s = timed(lambda: _capi.check(lib.fhe_b200_batch_upload(PT._h, 0, B, words_pinned.data_ptr(), 0)))
+out["upload_host_encoded_poly_ntt_pinned"] = {"pt_per_s": B / s, "input_mb": B * N_MODULI * DEGREE * 8 / 1e6,
+                                              "note": "today's route without the CPU encode: poly_ntt words from pinned memory"}
+P = F.PlaintextVec(PT, F.Encoding.simd())
+s = timed(lambda: A.mul_plain(P))
+out["mul_plain_batch"] = {"ct_per_s": B / s, "plaintexts": B}
+s = timed(lambda: A.add_plain(P))
+out["add_plain_batch"] = {"ct_per_s": B / s, "plaintexts": B, "note": "to_poly derived from poly_ntt on the device"}
+import subprocess  # noqa: E402
+out["gpu"] = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                            capture_output=True, text=True).stdout.strip()
 print(json.dumps(out, indent=1))
