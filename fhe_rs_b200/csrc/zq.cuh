@@ -274,12 +274,13 @@ __device__ __forceinline__ u64 fold94_solinas(u64 lo, u64 hi, u32 c) {
   const u32 x = (u32)((lo >> 62) | (hi << 2));
   return (u64)c * x + (lo & ((1ull << 62) - 1));         // < 2^60 + 2^62 < 2p
 }
-// Reduction of a lazy sum V = hi*2^128 + mid*2^64 + lo, hi < 2^16, modulo p = 2^62 - c to [0,2p):
-// 192 -> <2^111 -> <2^78 -> <2^62 + 2^44 bits.
+// Reduction of a lazy sum V = hi*2^128 + mid*2^64 + lo, hi < 2^32 (every sum an Acc192 holds, up to 2^160), modulo
+// p = 2^62 - c to [0,2p): top*c < 2^34 * 2^28 keeps the first fold's high word below 2^62, so
+// 192 -> <2^126 -> <2^93 -> <2^62 + 2^59 bits (tests/test_gpu_zq_probe.py checks hi = 2^32 - 1).
 __device__ __forceinline__ u64 fold192_solinas(u64 lo, u64 mid, u64 hi, u32 c) {
-  u64 top = (mid >> 62) | (hi << 2);                     // quotient bits 126.. (< 2^18)
-  fold_step_solinas(lo, mid, top, c);                    // < 2^111
-  fold_step_solinas(lo, mid, 0, c);                      // < 2^78
+  u64 top = (mid >> 62) | (hi << 2);                     // quotient bits 126.. (< 2^34)
+  fold_step_solinas(lo, mid, top, c);                    // < 2^126
+  fold_step_solinas(lo, mid, 0, c);                      // < 2^93
   return fold94_solinas(lo, mid, c);
 }
 

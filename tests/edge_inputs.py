@@ -1,0 +1,128 @@
+"""Crafted inputs for the arithmetic's decision points and range limits.
+
+Each coefficient of a polynomial is one independent scaler input, so the values are built as big integers and then
+projected onto the limbs of a basis.  Uniform random residues land on these points with probability around 2^-60:
+  * the exact scaler's rounding ties: num * x / den a hair away from a half-integer;
+  * its sign boundary: x next to F/2, where F is the product of the source basis;
+  * the extender (factor one) around (Q - 1)/2;
+  * switch_down around the ties of round(x / q_last).
+`residue_rows` gives rows that drive lazy sums to their extremes instead (all q - 1 and friends).
+"""
+from __future__ import annotations
+
+from typing import Dict, List, Sequence
+
+import numpy as np
+
+D_RANGE = range(-3, 4)
+
+# 62-bit primes at the edges of the device's limb modes, all == 1 mod 2^16 (NTT-friendly for any N <= 2^15).  A limb
+# p = 2^62 - c takes the Solinas path when c < 2^28.
+BOUNDARY_PRIMES = {
+    "solinas_max_c": 0x3ffffffff00a0001,     # c = 0xff5ffff: the thinnest [0, 2p) margin of the Solinas folds
+    "non_solinas_min": 0x3fffffffeff50001,   # c = 0x100affff: the largest 62-bit prime that is a Barrett limb
+    "above_2_61": 0x20000000000b0001,        # a Barrett limb just above 2^61
+}
+
+
+def product(moduli: Sequence[int]) -> int:
+    out = 1
+    for q in moduli:
+        out *= int(q)
+    return out
+
+
+def scaler_near_ties(F: int, num: int, den: int, rng: np.random.Generator, n_m: int = 4) -> List[int]:
+    """x = floor((2m + 1) * den / (2 num)) + d, d in [-3, 3], for random m with x in both halves of [0, F):
+    num * x / den is within a few num / den of m + 1/2."""
+    m_max = num * F // den          # num * x / den < m_max for x < F
+    out = []
+    for half in (0, 1):
+        lo, hi = (0, m_max // 2) if half == 0 else (m_max // 2, m_max)
+        for _ in range(n_m):
+            m = lo + int(rng.integers(0, 1 << 62)) * (hi - lo) // (1 << 62)
+            base = (2 * m + 1) * den // (2 * num)
+            out += [(base + d) % F for d in D_RANGE]
+    return out
+
+
+def sign_boundary(F: int) -> List[int]:
+    """F/2 + d with d in [-3, 3], plus 0, 1 and F - 1"""
+    return [(F // 2 + d) % F for d in D_RANGE] + [0, 1, F - 1]
+
+
+def extender_edges(Q: int) -> List[int]:
+    """(Q - 1)/2, (Q + 1)/2, (Q - 3)/2, 0 and Q - 1 (Q odd)"""
+    return [(Q - 1) // 2, (Q + 1) // 2, (Q - 3) // 2, 0, Q - 1]
+
+
+def switch_down_ties(Q: int, q_last: int, rng: np.random.Generator, n: int = 8) -> List[int]:
+    """x with x mod q_last in {(q_last - 1)/2, (q_last + 1)/2, 0, q_last - 1} and a random quotient"""
+    out = []
+    for r in ((q_last - 1) // 2, (q_last + 1) // 2, 0, q_last - 1):
+        for _ in range(n):
+            k = int(rng.integers(0, 1 << 62)) * (Q // q_last) // (1 << 62)
+            out.append(k * q_last + r)
+    return out + [(q_last - 1) // 2, (q_last + 1) // 2, Q - 1 - (q_last - 1) // 2]
+
+
+def wide_w_sums(sc, moduli: Sequence[int], rng: np.random.Generator, count: int, tries: int = 4000) -> List[List[int]]:
+    """Residue vectors whose theta_omega sum (rns/scaler.rs:278-302) has a magnitude in [2^190, 2^191): bits 190 and
+    191 of the U256 differ there, so only these inputs tell the sign test at bit 191 from one a bit lower.  The search
+    gives the terms of one sign residues in [15q/16, q) and the others zero.  The sum reaches the range only with
+    enough source limbs (29 at 62 bits do); with fewer, the search returns fewer vectors or none."""
+    import scaler_reference
+    signs = [int(s) for s in sc.theta_omega_sign]
+    out = []
+    for k in range(tries):
+        neg = k % 2 == 1
+        r = [int(q) - 1 - int(rng.integers(0, q >> 4)) if signs[i] == neg else 0 for i, q in enumerate(moduli)]
+        _, so = scaler_reference.v_and_w_sum(sc, r)
+        if ((so >> 190) & 1) != ((so >> 191) & 1) and so >> 192 in (0, (1 << 64) - 1):
+            out.append(r)
+            if len(out) == count:
+                break
+    return out
+
+
+def polys_from_residues(cols: Sequence[Sequence[int]], degree: int) -> np.ndarray:
+    """[count][limbs][N] with the given residue vectors as coefficients (repeated to fill the last polynomial)"""
+    count = -(-len(cols) // degree)
+    reps = -(-count * degree // len(cols))
+    a = np.array([[int(v) for v in c] for c in cols], dtype=np.uint64)
+    a = np.tile(a, (reps, 1))[: count * degree]
+    return np.ascontiguousarray(a.reshape(count, degree, -1).transpose(0, 2, 1))
+
+
+def polys_from_values(values: Sequence[int], moduli: Sequence[int], degree: int) -> np.ndarray:
+    """[count][limbs][N] residues of the values, N per polynomial; the last polynomial is filled by repeating them"""
+    vals = [int(v) for v in values]
+    count = -(-len(vals) // degree)
+    vals = (vals * (-(-count * degree // len(vals))))[: count * degree]
+    out = np.zeros((count, len(moduli), degree), np.uint64)
+    for i, q in enumerate(moduli):
+        out[:, i, :] = np.array([v % int(q) for v in vals], dtype=np.uint64).reshape(count, degree)
+    return out
+
+
+def residue_rows(moduli: Sequence[int], degree: int) -> Dict[str, np.ndarray]:
+    """[limbs][N] rows at the extremes: all 0, all q - 1, alternating 0 / q - 1, constant (q -/+ 1)/2, a single 1 at
+    coefficient 0 or at N - 1"""
+    L = len(moduli)
+    q = np.array([int(x) for x in moduli], dtype=np.uint64)[:, None]
+    one = np.ones((L, degree), np.uint64)
+    alt = np.zeros((L, degree), np.uint64)
+    alt[:, 1::2] = (q - np.uint64(1))[:, :1].repeat(degree // 2, axis=1)
+    first = np.zeros((L, degree), np.uint64)
+    first[:, 0] = 1
+    last = np.zeros((L, degree), np.uint64)
+    last[:, -1] = 1
+    return {
+        "zero": np.zeros((L, degree), np.uint64),
+        "max": one * (q - np.uint64(1)),
+        "alternating": alt,
+        "half_down": one * ((q - np.uint64(1)) // np.uint64(2)),
+        "half_up": one * ((q + np.uint64(1)) // np.uint64(2)),
+        "one_first": first,
+        "one_last": last,
+    }

@@ -195,6 +195,116 @@ def test_scaler_multiplication_bases(oracle):
         assert got == exp
 
 
+def test_boundary_primes(oracle):
+    """the boundary primes of tests/edge_inputs.py are primes == 1 mod 2^16, on the stated side of the Solinas rule
+    (p = 2^62 - c, c < 2^28), and not reachable from 2^62 by the prime generator within a few steps"""
+    import edge_inputs as E
+    for name, p in E.BOUNDARY_PRIMES.items():
+        assert oracle.is_prime(p) and p % (1 << 16) == 1 and p.bit_length() == 62, name
+        c = (1 << 62) - p
+        assert (c < (1 << 28)) == (name == "solinas_max_c"), name
+    gen, ub = [], 1 << 62
+    for _ in range(64):
+        ub = oracle.generate_prime(62, 1 << 16, ub)
+        gen.append(ub)
+    assert not set(gen) & set(E.BOUNDARY_PRIMES.values())
+
+
+# multiplication bases of the edge tests: name -> (degree, t, moduli sizes); the comments give the down scaler's
+# theta_garner_shift
+SCALER_BASES = {
+    "set_a": (1 << 12, 1032193, [62] * 2),       # down 5 -> 2, shift 126
+    "set_c": (1 << 15, 786433, [62] * 14),       # extension 14 -> 15, down 29 -> 14, shift 124
+    "l31": (1 << 13, 786433, [62] * 31),         # down 63 -> 31: shift 123, the lowest the device kernels accept
+    "small": (16, 1153, [40, 30]),               # extender 2 -> 3 with a small modulus: shift 127
+}
+_EPS = 2.0 ** -40
+
+
+def _scale_branch(x, F, n, d, Qto, negative):
+    """_expected_scale with the sign branch forced"""
+    if negative:
+        x = F - x
+        r = (x * n + ((d >> 1) - 1 if d % 2 == 0 else d >> 1)) // d
+        return (Qto - r % Qto) % Qto
+    return ((x * n + (d >> 1)) // d) % Qto
+
+
+def _windows(x, F, n, d):
+    """(near a rounding tie of n x / d, near the sign boundary F / 2)"""
+    from fractions import Fraction
+    frac = Fraction(x * n % d, d)
+    return abs(frac - Fraction(1, 2)) < _EPS, abs(Fraction(x, F) - Fraction(1, 2)) < _EPS
+
+
+def _scaler_cases(oracle, name):
+    """(scaler, from context, to context, factor, start, n_out, inputs) for the extender and the down scaler"""
+    import edge_inputs as E
+    degree, t, sizes = SCALER_BASES[name]
+    par = oracle.BfvParameters(degree, t, moduli_sizes=sizes)
+    mp = par.level(0).mul_params
+    frm, to = mp.frm.rns, mp.to.rns
+    L, K = len(frm.moduli), len(to.moduli)
+    Q, F = frm.product, to.product
+    rng = np.random.default_rng(len(sizes))
+    rnd = [int(rng.integers(0, 1 << 62)) * F // (1 << 62) for _ in range(16)]
+    down = E.scaler_near_ties(F, t, Q, rng) + E.sign_boundary(F) + rnd
+    ext = E.extender_edges(Q) + E.sign_boundary(Q) + E.scaler_near_ties(Q, 1, 1, rng)[:7] + [x % Q for x in rnd]
+    return [(mp.extender.scaler, frm, to, 1, 1, L, K - L, ext), (mp.down_scaler.scaler, to, frm, t, Q, 0, L, down)]
+
+
+@pytest.mark.parametrize("name", sorted(SCALER_BASES))
+def test_scaler_transcription_matches_oracle(oracle, name):
+    """tests/scaler_reference.py (a plain-integer restatement of rns/scaler.rs:249-352) equals the oracle's C scaler on
+    every crafted input: rounding ties, the sign boundary and the extender's edges."""
+    import scaler_reference
+    for sc, frm, to, n, d, start, n_out, xs in _scaler_cases(oracle, name):
+        assert sc.theta_garner_shift == {"set_a": (127, 126), "set_c": (125, 124), "l31": (124, 123),
+                                         "small": (127, 126)}[name][0 if n == 1 else 1]
+        for x in xs:
+            r = frm.project(x)
+            assert scaler_reference.scale(sc, r, n_out, start) == sc.scale_one(r, n_out, start), (name, x)
+    # residue vectors whose w sum sits between 2^190 and 2^191, where only bit 191 decides the sign of w (whether the
+    # sum can get there depends on the basis; the 63 source limbs of l31 reach it)
+    import edge_inputs as E
+    sc, frm = _scaler_cases(oracle, name)[1][:2]
+    wide = E.wide_w_sums(sc, frm.moduli_u64, np.random.default_rng(1), 32)
+    if name == "l31":
+        assert len(wide) == 32
+    for r in wide:
+        assert scaler_reference.scale(sc, r, len(sc.to.moduli)) == sc.scale_one(r, len(sc.to.moduli)), (name, r)
+
+
+@pytest.mark.parametrize("name", sorted(SCALER_BASES))
+def test_scaler_rounding_envelope(oracle, name):
+    """The reference's fixed-point scaler is exact centered rounding (_expected_scale) except inside two windows: num x
+    / den within 2^-40 of a half-integer, where it may round up by one, and x within 2^-40 F of F / 2, where it may
+    take the other sign branch (again possibly plus one).  This pins where the reference -- and so every device
+    kernel -- departs from exact rounding; any widening of these windows fails here."""
+    seen = {"tie_plus_one": 0, "other_branch": 0}
+    for sc, frm, to, n, d, start, n_out, xs in _scaler_cases(oracle, name):
+        Qto = to.product
+
+        def limbs(v):   # the limbs this scaler writes (the extender copies the first `start` ones)
+            return to.project(v % Qto)[start:start + n_out]
+        for x in xs:
+            got = sc.scale_one(frm.project(x), n_out, start)
+            exp = _expected_scale(x, frm.product, n, d, Qto)
+            if got == limbs(exp):
+                continue
+            near_tie, near_sign = _windows(x, frm.product, n, d)
+            if near_tie and got == limbs(exp + 1):
+                seen["tie_plus_one"] += 1
+                continue
+            other = _scale_branch(x, frm.product, n, d, Qto, x < frm.product // 2)
+            assert near_sign and got in (limbs(other), limbs(other + 1)), (name, x, near_tie, near_sign)
+            seen["other_branch"] += 1
+    # the crafted inputs do reach the departures (otherwise this test would check nothing)
+    assert seen["other_branch"] > 0, seen
+    if name != "small":
+        assert seen["tie_plus_one"] > 0, seen
+
+
 def test_poly_scaler_and_switch_down(oracle):
     """rq/scaler.rs:153-204 and rq/mod.rs:1040-1066: poly-level scale == per-coefficient BigUint rule;
     switch_down == round(x / q_last) with the reference's rounding."""
