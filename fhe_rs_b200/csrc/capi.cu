@@ -47,7 +47,7 @@ void upload_scaler_tables(ScalerData& s, const std::vector<u64>& to_moduli, ToDe
   d.n_from = s.h.n_from; d.n_to = s.h.n_to; d.is_one = s.h.is_one; d.shift = s.h.shift;
   d.tg_lo = s.h.theta_gamma_lo; d.tg_hi = s.h.theta_gamma_hi; d.tg_sign = s.h.theta_gamma_sign;
   for (size_t j = 0; j < to_moduli.size(); j++) d.to_ids[j] = (unsigned short)index_of(to_moduli[j]);
-  d.all_solinas = getenv("FHE_B200_NO_SOLINAS") ? 0 : 1;
+  d.all_solinas = switches().no_solinas ? 0 : 1;
   for (u64 q : to_moduli)
     if ((q >> 61) != 1 || ((1ull << 62) - q) >= (1ull << 28)) d.all_solinas = 0;
   d.gamma = to_dev(s.h.gamma);
@@ -316,10 +316,10 @@ LimbDev make_limb_dev(u64 q, const NttTablesH& t, ToDev&& to_dev) {
   d.ninv = t.ninv; d.zn = t.zn;
   // limb mode: p = 2^62 - c with c < 2^28 takes the Solinas constant-multiplication form
   const u64 cc = (1ull << 62) - q;
-  const bool sol = (q >> 61) == 1 && cc < (1ull << 28) && !getenv("FHE_B200_NO_SOLINAS");
+  const bool sol = (q >> 61) == 1 && cc < (1ull << 28) && !switches().no_solinas;
   // NTT butterflies: Shoup pairs by default (no Solinas instruction selection timed in bench_micro/bf_bench.cu beat
   // them); FHE_B200_SOLINAS_NTT=1 selects the (w, w*2^32 mod p) pairs instead
-  const bool sol_ntt = getenv("FHE_B200_SOLINAS_NTT") != nullptr;
+  const bool sol_ntt = switches().solinas_ntt;
   auto pairs = [&](const std::vector<u64>& v, const std::vector<u64>& shoup) {
     std::vector<ulonglong2> o(v.size());
     for (size_t k = 0; k < v.size(); k++) {
@@ -393,15 +393,7 @@ struct Workspace {
   }
 };
 
-u32 chunk_size() {
-  static u32 c = [] {
-    const char* e = getenv("FHE_B200_CHUNK");
-    int v = e ? atoi(e) : 256;   // ~28 GB of scratch per in-flight chunk at set C (108 MB per ciphertext); larger chunks
-                                 // mean fewer kernel boundaries per ciphertext
-    return (u32)(v < 1 ? 1 : v);
-  }();
-  return c;
-}
+u32 chunk_size() { return switches().chunk; }
 
 // A batched call works through its ciphertexts chunk by chunk.  On ONE stream every kernel boundary costs the tail of
 // one persistent grid plus the ring fill and table staging of the next, 18 boundaries per chunk.
@@ -416,14 +408,7 @@ struct ChunkRunner {
   cudaStream_t user;
   u32 count, chunk, ns;
   cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  static u32 streams() {
-    static const u32 n = [] {
-      const char* e = getenv("FHE_B200_STREAMS");
-      const int v = e ? atoi(e) : 2;
-      return (u32)(v < 1 ? 1 : v > 4 ? 4 : v);
-    }();
-    return n;
-  }
+  static u32 streams() { return switches().streams; }
   ChunkRunner(const fhe_b200_params* p, u32 n, cudaStream_t st) : par(p), user(st), count(n), chunk(chunk_size()), ns(1) {
     if (streams() < 2 || count <= chunk || chunk < streams()) return;
     ns = streams();
@@ -502,11 +487,7 @@ void key_switch_core(const fhe_b200_params* par, const fhe_b200_ksk* k, const u6
   // default: the rows pass of the digit transforms and the inner product run as one kernel, so the transformed digits
   // never go through HBM.  FHE_B200_KSMAC=tma keeps the unfused TMA chain (rows pass, then ksmac_tma_kernel),
   // =classic the per-thread inner product.
-  static const bool fused = [] {
-    const char* e = getenv("FHE_B200_KSMAC");
-    return !e || (strcmp(e, "tma") && strcmp(e, "classic"));
-  }();
-  if (adjacent && fused &&
+  if (adjacent && switches().ksmac == Switches::KSMAC_FUSED &&
       launch_key_switch_tma(c2, inter, k->k0, k->k1, base0, base1, out0, out1, cts, L, Lk, out_ct_rows, kl.ctx_ids,
                             par->d_limbs, par->logn, reduce, st))
     return;

@@ -1,6 +1,7 @@
 // Internal launch interfaces shared by ntt.cu / kernels.cu / capi.cu.
 #pragma once
 #include <atomic>
+#include <cuda.h>
 #include <cuda_runtime.h>
 
 #include "ntt.cuh"
@@ -8,6 +9,41 @@
 namespace fhe_b200 {
 
 extern std::atomic<unsigned long long> g_launches;
+
+// The FHE_B200_* environment switches (DESIGN.md, appendix), read once per process by switches() (ntt.cu).  Every
+// value the appendix lists is set by a bit-for-bit rerun test.
+struct Switches {
+  enum Ntt { NTT_FAST, NTT_AUTO, NTT_TMA };
+  enum Ksmac { KSMAC_FUSED, KSMAC_TMA, KSMAC_CLASSIC };
+  u32 chunk;              // FHE_B200_CHUNK: ciphertexts per chunk of a batched call (>= 1, default 256)
+  u32 streams;            // FHE_B200_STREAMS: side streams the chunks are dealt over (1..4, default 2)
+  Ntt ntt;                // FHE_B200_NTT = fast | tma (default auto)
+  bool generic_ntt;       // FHE_B200_GENERIC_NTT
+  bool solinas_ntt;       // FHE_B200_SOLINAS_NTT: Solinas twiddle pairs (generic tile kernels only)
+  bool no_solinas;        // FHE_B200_NO_SOLINAS: Barrett instead of the 2^62 = c folds everywhere
+  bool no_tensor_fusion;  // FHE_B200_NO_TENSOR_FUSION
+  bool classic_scaler;    // FHE_B200_SCALER=classic
+  Ksmac ksmac;            // FHE_B200_KSMAC = tma | classic (default fused)
+  int tma_cols;           // FHE_B200_TMA_COLS: 2 = ring depth 2 of the TMA cols pass (default 3)
+  int scale_unroll;       // FHE_B200_SCALE_UNROLL: 4 = unroll 4 of the TMA scaler's multiply loop (default 2)
+  u32 ks_stages;          // FHE_B200_KS_STAGES: digit ring depth of the key-switch kernels (2..4, default 2)
+  // every NTT of N > 4096 runs on the generic tile kernels
+  bool generic_tiles() const { return generic_ntt || solinas_ntt; }
+  // the TMA-fed NTT kernels may serve a launch
+  bool tma_allowed() const { return ntt != NTT_FAST && !generic_tiles(); }
+};
+const Switches& switches();
+
+// cuTensorMapEncodeTiled, fetched through the runtime so the library does not link against libcuda; null when the
+// driver lacks it
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+EncodeTiledFn tensor_map_encoder();
+// the buffer [rows][N] u64 as {box_cols, box_rows} boxes, no swizzle; false when the encoder is missing or refuses
+bool box_map(CUtensorMap* m, const u64* base, u64 rows, u32 logn, u32 box_cols, u32 box_rows);
+// multiprocessors of the current device (cached per device)
+int sm_count();
 
 struct CudaFail {
   cudaError_t err;

@@ -5,9 +5,6 @@
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
-#include <map>
-#include <mutex>
-#include <vector>
 
 #include "engine.hpp"
 #include "ntt_tma.cuh"
@@ -1128,55 +1125,16 @@ void launch_tensor_nm(const u64* a, const u64* b, const u64* xa, const u64* xb, 
   g_launches++;
 }
 
-namespace {
-typedef CUresult (*ScaleEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-ScaleEncodeFn scale_encoder() {
-  static ScaleEncodeFn fn = [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-      p = nullptr;
-    cudaGetLastError();
-    return (ScaleEncodeFn)p;
-  }();
-  return fn;
-}
-int scale_sm_count() {
-  static std::mutex mu;
-  static std::map<int, int> cache;
-  int dev = 0;
-  FHE_CUDA(cudaGetDevice(&dev));
-  std::lock_guard<std::mutex> g(mu);
-  auto it = cache.find(dev);
-  if (it != cache.end()) return it->second;
-  int n = 0;
-  FHE_CUDA(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
-  return cache[dev] = n;
-}
-}  // namespace
-
 // The persistent TMA-fed kernel serves N >= 128 when every output limb is a Solinas prime (all 62-bit primes the
 // reference's parameter builder generates are); FHE_B200_SCALER=classic keeps the per-tile kernel.
-static bool launch_scale_tma(const ScalerDev& S, const LimbDev* limbs, const std::vector<u64>* sol_c_of_out, const u64* in,
-                             u64* out0, u64* out1, u32 polys, u32 out_rows_per_poly, u32 start, u32 n_out, int split3,
-                             u32 logn, cudaStream_t st) {
-  (void)sol_c_of_out;
-  static const bool classic = [] { const char* e = getenv("FHE_B200_SCALER"); return e && !strcmp(e, "classic"); }();
-  if (classic || !scale_encoder() || logn < 7 || (reinterpret_cast<uintptr_t>(in) & 127)) return false;
+static bool launch_scale_tma(const ScalerDev& S, const LimbDev* limbs, const u64* in, u64* out0, u64* out1, u32 polys,
+                             u32 out_rows_per_poly, u32 start, u32 n_out, int split3, u32 logn, cudaStream_t st) {
+  if (switches().classic_scaler || !tensor_map_encoder() || logn < 7 || (reinterpret_cast<uintptr_t>(in) & 127))
+    return false;
   const u32 N = 1u << logn, nf = S.n_from;
   if (nf > 64 || (u64)polys * nf >= (1ull << 31)) return false;
   CUtensorMap tm;
-  const cuuint64_t gdim[2] = {N, (cuuint64_t)polys * nf};
-  const cuuint64_t gstride[1] = {(cuuint64_t)8 << logn};
-  const cuuint32_t box[2] = {(cuuint32_t)kScaleTC, nf};
-  const cuuint32_t es[2] = {1, 1};
-  if (scale_encoder()(&tm, CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, (void*)in, gdim, gstride, box, es,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-    return false;
+  if (!box_map(&tm, in, (u64)polys * nf, logn, kScaleTC, nf)) return false;
   ScaleTmaArgs A;
   A.S = S; A.limbs = limbs; A.out0 = out0; A.out1 = out1;
   A.polys = polys; A.out_rows_per_poly = out_rows_per_poly; A.start = start; A.n_out = n_out;
@@ -1189,10 +1147,9 @@ static bool launch_scale_tma(const ScalerDev& S, const LimbDev* limbs, const std
     ensure_dynamic_smem(k, smem);
     int per_sm = 0;
     FHE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, kScaleTC, smem));
-    return (u32)std::min<u64>(A.tiles_total, (u64)scale_sm_count() * std::max(per_sm, 1));
+    return (u32)std::min<u64>(A.tiles_total, (u64)sm_count() * std::max(per_sm, 1));
   };
-  static const int unr = [] { const char* e = getenv("FHE_B200_SCALE_UNROLL"); return e ? atoi(e) : 2; }();
-  if (unr == 4) {
+  if (switches().scale_unroll == 4) {
     if (S.is_one) scale_tma_kernel<true, 4><<<resident((const void*)scale_tma_kernel<true, 4>), kScaleTC, smem, st>>>(tm, A);
     else scale_tma_kernel<false, 4><<<resident((const void*)scale_tma_kernel<false, 4>), kScaleTC, smem, st>>>(tm, A);
   } else {
@@ -1206,8 +1163,8 @@ static bool launch_scale_tma(const ScalerDev& S, const LimbDev* limbs, const std
 void launch_scale(const ScalerDev& S, const LimbDev* limbs, const u64* in, u64* out0, u64* out1, u32 polys,
                   u32 out_rows_per_poly, u32 start, u32 n_out, int split3, u32 logn, cudaStream_t st) {
   if (!polys || !n_out) return;
-  if (S.all_solinas && launch_scale_tma(S, limbs, nullptr, in, out0, out1, polys, out_rows_per_poly, start, n_out, split3,
-                                        logn, st))
+  if (S.all_solinas &&
+      launch_scale_tma(S, limbs, in, out0, out1, polys, out_rows_per_poly, start, n_out, split3, logn, st))
     return;
   ScaleArgs A;
   A.S = S; A.limbs = limbs; A.in = in; A.out0 = out0; A.out1 = out1;
@@ -1232,25 +1189,17 @@ void launch_ksmac(const u64* inter, const u64* k0, const u64* k1, const u64* bas
                   u32 logn, cudaStream_t st, bool adjacent) {
   size_t total = ((size_t)cts * Lk) << logn;
   if (!total) return;
-  static const bool classic = [] { const char* e = getenv("FHE_B200_KSMAC"); return e && !strcmp(e, "classic"); }();
+  const bool classic = switches().ksmac == Switches::KSMAC_CLASSIC;
   // ring depth: 2 buffers -> 4 resident CTAs per SM at set C: the kernel needs warps more than prefetch depth.
   // FHE_B200_KS_STAGES = 2 | 3 | 4.
-  static const int stages = [] { const char* e = getenv("FHE_B200_KS_STAGES"); int v = e ? atoi(e) : 2; return v < 2 ? 2 : v > 4 ? 4 : v; }();
+  const int stages = (int)switches().ks_stages;
   const size_t smem_tma = ((size_t)(2 + stages) * n_dig * kKsTC + stages + 1) * sizeof(u64);
-  if (adjacent && !classic && scale_encoder() && logn >= 7 && n_dig <= 256 && smem_tma <= 200 * 1024 &&
+  if (adjacent && !classic && tensor_map_encoder() && logn >= 7 && n_dig <= 256 && smem_tma <= 200 * 1024 &&
       !((reinterpret_cast<uintptr_t>(inter) | reinterpret_cast<uintptr_t>(k0) | reinterpret_cast<uintptr_t>(k1)) & 127) &&
       (u64)cts * Lk * n_dig < (1ull << 31)) {
-    auto map = [&](const u64* base, u64 rows, CUtensorMap* m) {
-      const cuuint64_t gdim[2] = {(cuuint64_t)1 << logn, rows};
-      const cuuint64_t gstride[1] = {(cuuint64_t)8 << logn};
-      const cuuint32_t box[2] = {(cuuint32_t)kKsTC, n_dig};
-      const cuuint32_t es[2] = {1, 1};
-      return scale_encoder()(m, CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, (void*)base, gdim, gstride, box, es,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                             CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-    };
     CUtensorMap mt, m0, m1;
-    if (map(inter, (u64)cts * Lk * n_dig, &mt) && map(k0, (u64)Lk * n_dig, &m0) && map(k1, (u64)Lk * n_dig, &m1)) {
+    if (box_map(&mt, inter, (u64)cts * Lk * n_dig, logn, kKsTC, n_dig) &&
+        box_map(&m0, k0, (u64)Lk * n_dig, logn, kKsTC, n_dig) && box_map(&m1, k1, (u64)Lk * n_dig, logn, kKsTC, n_dig)) {
       KsTmaArgs T;
       T.base0 = base0; T.base1 = base1; T.out0 = out0; T.out1 = out1;
       T.cts = cts; T.n_dig = n_dig; T.Lk = Lk; T.out_ct_rows = out_ct_rows; T.logn = logn;
@@ -1261,7 +1210,7 @@ void launch_ksmac(const u64* inter, const u64* k0, const u64* k1, const u64* bas
         ensure_dynamic_smem((const void*)kern, smem_tma);
         int per_sm = 0;
         FHE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)kern, kKsTC, smem_tma));
-        const u32 grid = (u32)std::min<u64>(T.items_total, (u64)scale_sm_count() * std::max(per_sm, 1));
+        const u32 grid = (u32)std::min<u64>(T.items_total, (u64)sm_count() * std::max(per_sm, 1));
         kern<<<grid, kKsTC, smem_tma, st>>>(mt, m0, m1, T);
       };
       if (stages == 2) go(ksmac_tma_kernel<2>);

@@ -1,6 +1,7 @@
 // NTT launcher: picks the (N1, N2) split and tile shapes for a given N and instantiates
 // the tile kernels of ntt.cuh.
 #include <algorithm>
+#include <climits>
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
@@ -15,6 +16,81 @@
 namespace fhe_b200 {
 
 std::atomic<unsigned long long> g_launches{0};
+
+const Switches& switches() {
+  static const Switches s = [] {
+    auto set = [](const char* name) { return getenv(name) != nullptr; };
+    auto is = [](const char* name, const char* value) {
+      const char* e = getenv(name);
+      return e && !strcmp(e, value);
+    };
+    auto number = [](const char* name, int dflt) {
+      const char* e = getenv(name);
+      return e ? atoi(e) : dflt;
+    };
+    auto clamped = [&](const char* name, int dflt, int lo, int hi) {
+      const int v = number(name, dflt);
+      return (u32)(v < lo ? lo : v > hi ? hi : v);
+    };
+    Switches w;
+    // ~28 GB of scratch per in-flight chunk at set C (108 MB per ciphertext); larger chunks mean fewer kernel
+    // boundaries per ciphertext
+    w.chunk = clamped("FHE_B200_CHUNK", 256, 1, INT_MAX);
+    w.streams = clamped("FHE_B200_STREAMS", 2, 1, 4);
+    w.ntt = is("FHE_B200_NTT", "fast") ? Switches::NTT_FAST : is("FHE_B200_NTT", "tma") ? Switches::NTT_TMA
+                                                                                         : Switches::NTT_AUTO;
+    w.generic_ntt = set("FHE_B200_GENERIC_NTT");
+    w.solinas_ntt = set("FHE_B200_SOLINAS_NTT");
+    w.no_solinas = set("FHE_B200_NO_SOLINAS");
+    w.no_tensor_fusion = set("FHE_B200_NO_TENSOR_FUSION");
+    w.classic_scaler = is("FHE_B200_SCALER", "classic");
+    w.ksmac = is("FHE_B200_KSMAC", "tma")       ? Switches::KSMAC_TMA
+              : is("FHE_B200_KSMAC", "classic") ? Switches::KSMAC_CLASSIC
+                                                : Switches::KSMAC_FUSED;
+    w.tma_cols = number("FHE_B200_TMA_COLS", 3);
+    w.scale_unroll = number("FHE_B200_SCALE_UNROLL", 2);
+    w.ks_stages = clamped("FHE_B200_KS_STAGES", 2, 2, 4);
+    return w;
+  }();
+  return s;
+}
+
+EncodeTiledFn tensor_map_encoder() {
+  static EncodeTiledFn fn = [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess)
+      p = nullptr;
+    cudaGetLastError();
+    return (EncodeTiledFn)p;
+  }();
+  return fn;
+}
+
+bool box_map(CUtensorMap* m, const u64* base, u64 rows, u32 logn, u32 box_cols, u32 box_rows) {
+  const cuuint64_t gdim[2] = {(cuuint64_t)1 << logn, rows};
+  const cuuint64_t gstride[1] = {(cuuint64_t)8 << logn};
+  const cuuint32_t box[2] = {box_cols, box_rows};
+  const cuuint32_t es[2] = {1, 1};
+  return tensor_map_encoder() &&
+         tensor_map_encoder()(m, CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, (void*)base, gdim, gstride, box, es,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                              CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+int sm_count() {
+  static std::mutex mu;
+  static std::map<int, int> cache;
+  int dev = 0;
+  FHE_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> g(mu);
+  auto it = cache.find(dev);
+  if (it != cache.end()) return it->second;
+  int n = 0;
+  FHE_CUDA(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
+  return cache[dev] = n;
+}
 
 void ensure_dynamic_smem(const void* kernel, size_t bytes) {
   if (bytes <= 48 * 1024) return;   // the default limit needs no opt-in
@@ -51,22 +127,23 @@ void run_cols(const NttArgs& a, cudaStream_t st) {
   g_launches++;
 }
 
-template <int LOGP, bool COLS, bool INV, int TLOG = 12>
+template <int LOGP, bool COLS, bool INV, int TLOG>
 void run_fast(const NttArgs& a, cudaStream_t st) {
-  constexpr size_t smem = 2 * FastTile<LOGP, COLS, INV, false, TLOG>::TW * sizeof(u64);
+  constexpr size_t smem = 2 * FastTile<LOGP, COLS, INV, TLOG>::TW * sizeof(u64);
   ensure_dynamic_smem((const void*)ntt_fast_kernel<LOGP, COLS, INV, TLOG>, smem);
   constexpr int LOGB = TLOG - LOGP;
   const u32 tiles = COLS ? ((1u << (a.logn - LOGP)) >> LOGB) : ((1u << a.logn1) >> LOGB);
   ntt_fast_kernel<LOGP, COLS, INV, TLOG><<<a.n_rows * tiles, 1 << (TLOG - 3), smem, st>>>(a);
   g_launches++;
 }
-template <bool INV, int TLOG = 12>
+// 2048-word cols tiles; N = 2^16 keeps 4096 words (a 2048-word tile would be two columns wide there)
+template <bool INV>
 void run_fast_cols_for(const NttArgs& a, cudaStream_t st) {
   switch (a.logn1) {
-    case 7: run_fast<7, true, INV, TLOG>(a, st); break;
-    case 8: run_fast<8, true, INV, TLOG>(a, st); break;
-    case 9: run_fast<9, true, INV, TLOG>(a, st); break;
-    case 10: run_fast<10, true, INV, TLOG>(a, st); break;
+    case 7: run_fast<7, true, INV, 11>(a, st); break;
+    case 8: run_fast<8, true, INV, 11>(a, st); break;
+    case 9: run_fast<9, true, INV, 11>(a, st); break;
+    case 10: run_fast<10, true, INV, 12>(a, st); break;
     default: break;
   }
 }
@@ -99,22 +176,6 @@ void run_cols_for(const NttArgs& a, cudaStream_t st) {
 }
 
 // ---- TMA-fed persistent kernels (ntt_tma.cuh)
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn tensor_map_encoder() {
-  // the driver entry point is fetched through the runtime, so the library does not link against libcuda
-  static EncodeTiledFn fn = [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-      p = nullptr;
-    cudaGetLastError();
-    return (EncodeTiledFn)p;
-  }();
-  return fn;
-}
 struct TmaFail {};
 // the buffer [rows][N] u64 as 128-byte box rows: dims {16, rows*N/16}, box {16, box_rows}, 128-byte swizzle
 CUtensorMap rows_map(const u64* base, u64 rows, u32 logn, u32 box_rows) {
@@ -144,29 +205,11 @@ CUtensorMap cols_map(const u64* base, u64 rows, u32 logn, u32 box_rows) {
   return m;
 }
 
-int sm_count() {
-  static std::mutex mu;
-  static std::map<int, int> cache;
-  int dev = 0;
-  FHE_CUDA(cudaGetDevice(&dev));
-  std::lock_guard<std::mutex> g(mu);
-  auto it = cache.find(dev);
-  if (it != cache.end()) return it->second;
-  int n = 0;
-  FHE_CUDA(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
-  return cache[dev] = n;
-}
-
 constexpr int kRowsRlog = 4;
 
-// shared-memory ring depth x resident CTAs per SM of the rows / cols kernels (FHE_B200_TMA_ROWS / _COLS = "SxB")
-int tma_variant(const char* env, int dflt) {
-  const char* e = getenv(env);
-  return e ? atoi(e) : dflt;
-}
-
+// one tile per CTA iteration
 template <bool INV, int STAGES, int MINB>
-void run_tma_rows_v(const u64* in, u64 in_rows, u64* out, u64 out_rows, NttTmaArgs A, cudaStream_t st) {
+void run_tma_rows_one(const u64* in, u64 in_rows, u64* out, u64 out_rows, NttTmaArgs A, cudaStream_t st) {
   using Cfg = RowsCfg<kRowsRlog, STAGES>;
   const CUtensorMap mi = rows_map(in, in_rows, A.logn, 4 * Cfg::R), mo = rows_map(out, out_rows, A.logn, 4 * Cfg::R);
   A.tiles_per_row = (1u << (A.logn - 6)) / Cfg::R;
@@ -207,18 +250,15 @@ void run_tma_rows_pair(const u64* in, u64 in_rows, u64* out, u64 out_rows, NttTm
 
 template <bool INV>
 void run_tma_rows(const u64* in, u64 in_rows, u64* out, u64 out_rows, const NttTmaArgs& A, cudaStream_t st) {
-  // default: two polynomials per CTA iteration; FHE_B200_TMA_ROWS = 44 | 26 select the one-tile kernel with that ring
-  // depth x CTAs per SM
-  static const int v = tma_variant("FHE_B200_TMA_ROWS", 2);
-  if (v == 2 && A.n_polys % 2 == 0 && !(A.digit_adjacent && A.n_dig % 2)) {
+  // two polynomials per CTA iteration (ring depth 3 x 3 CTAs per SM) wherever the polynomials pair up; the one-tile
+  // kernel (4 x 4) serves an odd polynomial count, or a digit-adjacent launch with an odd digit count
+  if (A.n_polys % 2 == 0 && !(A.digit_adjacent && A.n_dig % 2))
     run_tma_rows_pair<INV, 3, 3>(in, in_rows, out, out_rows, A, st);
-    return;
-  }
-  if (v == 26) run_tma_rows_v<INV, 2, 6>(in, in_rows, out, out_rows, A, st);
-  else run_tma_rows_v<INV, 4, 4>(in, in_rows, out, out_rows, A, st);
+  else
+    run_tma_rows_one<INV, 4, 4>(in, in_rows, out, out_rows, A, st);
 }
 template <int LOGP, bool INV, int STAGES, int MINB>
-void run_tma_cols_v(const u64* in, u64 in_rows, u64* out, u64 out_rows, NttTmaArgs A, cudaStream_t st) {
+void run_tma_cols(const u64* in, u64 in_rows, u64* out, u64 out_rows, NttTmaArgs A, cudaStream_t st) {
   using Cfg = ColsCfg<LOGP, STAGES>;
   const CUtensorMap mi = cols_map(in, in_rows, A.logn, Cfg::BOX_ROWS), mo = cols_map(out, out_rows, A.logn, Cfg::BOX_ROWS);
   A.tiles_per_row = 4;
@@ -235,38 +275,25 @@ void run_tma_cols_v(const u64* in, u64 in_rows, u64* out, u64 out_rows, NttTmaAr
   }
   g_launches++;
 }
-template <int LOGP, bool INV>
-void run_tma_cols(const u64* in, u64 in_rows, u64* out, u64 out_rows, const NttTmaArgs& A, cudaStream_t st) {
-  static const int v = tma_variant("FHE_B200_TMA_COLS", 3);
-  if (LOGP == 9) {
-    if (v == 2) run_tma_cols_v<9, INV, 2, 1>(in, in_rows, out, out_rows, A, st);
-    else run_tma_cols_v<9, INV, 3, 1>(in, in_rows, out, out_rows, A, st);
-  } else if (LOGP == 8) {
-    if (v == 2) run_tma_cols_v<8, INV, 2, 3>(in, in_rows, out, out_rows, A, st);
-    else run_tma_cols_v<8, INV, 3, 2>(in, in_rows, out, out_rows, A, st);
-  } else {
-    if (v == 2) run_tma_cols_v<7, INV, 2, 6>(in, in_rows, out, out_rows, A, st);
-    else run_tma_cols_v<7, INV, 3, 4>(in, in_rows, out, out_rows, A, st);
-  }
-}
+// ring depth 3 (FHE_B200_TMA_COLS=2: 2); resident CTAs per SM by tile height
 template <bool INV>
 void run_tma_cols_for(const u64* in, u64 in_rows, u64* out, u64 out_rows, const NttTmaArgs& A, cudaStream_t st) {
+  const bool d2 = switches().tma_cols == 2;
   switch (A.logn - 6) {
-    case 7: run_tma_cols<7, INV>(in, in_rows, out, out_rows, A, st); break;
-    case 8: run_tma_cols<8, INV>(in, in_rows, out, out_rows, A, st); break;
-    case 9: run_tma_cols<9, INV>(in, in_rows, out, out_rows, A, st); break;
+    case 7:
+      if (d2) run_tma_cols<7, INV, 2, 6>(in, in_rows, out, out_rows, A, st);
+      else run_tma_cols<7, INV, 3, 4>(in, in_rows, out, out_rows, A, st);
+      break;
+    case 8:
+      if (d2) run_tma_cols<8, INV, 2, 3>(in, in_rows, out, out_rows, A, st);
+      else run_tma_cols<8, INV, 3, 2>(in, in_rows, out, out_rows, A, st);
+      break;
+    case 9:
+      if (d2) run_tma_cols<9, INV, 2, 1>(in, in_rows, out, out_rows, A, st);
+      else run_tma_cols<9, INV, 3, 1>(in, in_rows, out, out_rows, A, st);
+      break;
     default: throw TmaFail{};
   }
-}
-
-// digit-broadcast cols passes walk their tiles limb-innermost (cols_tile, ntt_tma.cuh): each source tile leaves DRAM
-// once instead of once per limb.  FHE_B200_BCAST_WALK=limb_major keeps the limb-major walk.
-bool bcast_limb_inner() {
-  static const bool v = [] {
-    const char* e = getenv("FHE_B200_BCAST_WALK");
-    return !(e && !strcmp(e, "limb_major"));
-  }();
-  return v;
 }
 
 // Both passes through the TMA kernels.  Returns false when the shape is outside their domain (the caller then uses
@@ -290,8 +317,7 @@ bool launch_ntt_tma(const u64* in, u64* out, u32 n_rows, const RowIds& ids, cons
   const u64 in_rows = in_div == 1 ? n_rows : n_rows / lpp;
   try {
     NttTmaArgs first = A, second = A;
-    first.in_bcast = in_div != 1;
-    first.limb_inner = first.in_bcast && bcast_limb_inner();
+    first.in_bcast = first.limb_inner = in_div != 1;
     if (!inverse) {
       first.reduce_on_load = reduce_on_load;
       second.lazy_out = lazy_out;
@@ -335,10 +361,7 @@ bool launch_tensor_intt_tma(const u64* a, const u64* b, const u64* xa, const u64
     A.tiles_per_row = (1u << (logn - 6)) / R;
     A.items_total = K * A.tiles_per_row * cts;
     for (int i = 0; i < kMaxPos; i++) A.ids[i] = mul_ids.ids[i];
-    static const int v = tma_variant("FHE_B200_TENSOR_V", 22);   // ring depth x CTAs per SM
-    if (v == 13) run_tensor_rows<1, 3>(ma, mb, mxa, mxb, mo, A, st);
-    else if (v == 14) run_tensor_rows<1, 4>(ma, mb, mxa, mxb, mo, A, st);
-    else run_tensor_rows<2, 2>(ma, mb, mxa, mxb, mo, A, st);
+    run_tensor_rows<2, 2>(ma, mb, mxa, mxb, mo, A, st);   // ring depth 2 x 2 CTAs per SM
     // second pass of the inverse transform of the 3K product rows, in place
     NttTmaArgs C;
     std::memset(&C, 0, sizeof(C));
@@ -365,48 +388,23 @@ void run_ks_rows_mac(const CUtensorMap& mi, const CUtensorMap& m0, const CUtenso
   g_launches++;
 }
 
-// a key [Lk][n_dig][N] as {128-coefficient, n_dig-row} boxes, no swizzle
-CUtensorMap key_map(const u64* base, u64 rows, u32 logn, u32 box_cols, u32 box_rows) {
-  CUtensorMap m;
-  const cuuint64_t gdim[2] = {(cuuint64_t)1 << logn, rows};
-  const cuuint64_t gstride[1] = {(cuuint64_t)8 << logn};
-  const cuuint32_t box[2] = {box_cols, box_rows};
-  const cuuint32_t es[2] = {1, 1};
-  if (tensor_map_encoder()(&m, CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, (void*)base, gdim, gstride, box, es,
-                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-    throw TmaFail{};
-  return m;
-}
-
-int tma_mode() {
-  static const int mode = [] {
-    const char* e = getenv("FHE_B200_NTT");
-    if (getenv("FHE_B200_GENERIC_NTT") || getenv("FHE_B200_SOLINAS_NTT")) return 0;
-    if (e && !strcmp(e, "fast")) return 0;
-    if (e && !strcmp(e, "tma")) return 2;
-    return 1;
-  }();
-  return mode;
-}
-
 }  // namespace
 
 // TMA-fed persistent kernels: the default whenever a launch carries enough polynomials per limb to amortise the
 // per-(limb, tile position) twiddle staging; FHE_B200_NTT=fast keeps the register-resident kernels, =tma forces the
 // TMA ones for any batch size (tests)
 bool ntt_uses_tma(u32 n_rows, const RowIds& ids, u32 logn, u32 in_div, const u64* in, const u64* out) {
+  const Switches& sw = switches();
   const u32 lpp = ids.limbs_per_poly;
-  if (!tma_mode() || logn < 13 || logn > 15 || !tensor_map_encoder()) return false;
+  if (!sw.tma_allowed() || logn < 13 || logn > 15 || !tensor_map_encoder()) return false;
   if (n_rows % lpp != 0 || (in_div != 1 && in_div != lpp)) return false;
   if ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) & 127) return false;
-  return tma_mode() == 2 || n_rows / lpp >= 8;
+  return sw.ntt == Switches::NTT_TMA || n_rows / lpp >= 8;
 }
 
 bool launch_tensor_inverse_ntt(const u64* a, const u64* b, const u64* xa, const u64* xb, u64* T, u32 cts, u32 L, u32 K,
                                const RowIds& mul_ids, const LimbDev* limbs, u32 logn, cudaStream_t st) {
-  static const bool off = getenv("FHE_B200_NO_TENSOR_FUSION") != nullptr;
-  if (off || K <= L || !ntt_uses_tma(cts * 3 * K, mul_ids, logn, 1, T, T)) return false;
+  if (switches().no_tensor_fusion || K <= L || !ntt_uses_tma(cts * 3 * K, mul_ids, logn, 1, T, T)) return false;
   if ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(xa) |
        reinterpret_cast<uintptr_t>(xb)) & 127)
     return false;
@@ -417,7 +415,7 @@ bool launch_key_switch_tma(const u64* c2, u64* inter, const u64* k0, const u64* 
                            const u64* base1, u64* out0, u64* out1, u32 cts, u32 n_dig, u32 Lk, u32 out_ct_rows,
                            const RowIds& ids, const LimbDev* limbs, u32 logn, bool reduce, cudaStream_t st) {
   // ring depth of the digit tiles: 2 (default) or 3 (FHE_B200_KS_STAGES >= 3); both keep 3 CTAs per SM at n_dig = 14
-  static const int stages = tma_variant("FHE_B200_KS_STAGES", 2) >= 3 ? 3 : 2;
+  const int stages = switches().ks_stages >= 3 ? 3 : 2;
   using Cfg = KsRowsCfg<2>;
   const u32 n_rows = cts * n_dig * Lk;
   if (logn < 13 || logn > 15 || !tensor_map_encoder() || ids.limbs_per_poly != Lk || n_dig == 0 || n_dig > 256)
@@ -426,11 +424,13 @@ bool launch_key_switch_tma(const u64* c2, u64* inter, const u64* k0, const u64* 
        reinterpret_cast<uintptr_t>(k1)) & 127)
     return false;
   if ((stages == 3 ? KsRowsCfg<3>::smem(n_dig) : Cfg::smem(n_dig)) > 227 * 1024) return false;
+  // every tensor map first: a shape the TMA cannot describe launches nothing.  The keys [Lk][n_dig][N] are read as
+  // {128-coefficient, n_dig-row} boxes.
+  CUtensorMap m0, m1;
+  if (!box_map(&m0, k0, (u64)Lk * n_dig, logn, Cfg::TC, n_dig) || !box_map(&m1, k1, (u64)Lk * n_dig, logn, Cfg::TC, n_dig))
+    return false;
   try {
-    // every tensor map first: a shape the TMA cannot describe launches nothing
     const CUtensorMap mi = rows_map(inter, n_rows, logn, 4 * Cfg::R);
-    const CUtensorMap m0 = key_map(k0, (u64)Lk * n_dig, logn, Cfg::TC, n_dig);
-    const CUtensorMap m1 = key_map(k1, (u64)Lk * n_dig, logn, Cfg::TC, n_dig);
     // digit broadcast + large-stride stages: inter [ct][j][d][N] (in_bcast: the source row of polynomial (ct, d) is
     // row ct*n_dig + d of c2 for every limb j)
     NttTmaArgs C;
@@ -438,8 +438,7 @@ bool launch_key_switch_tma(const u64* c2, u64* inter, const u64* k0, const u64* 
     C.limbs = limbs;
     C.n_polys = cts * n_dig;
     C.lpp = Lk;
-    C.in_bcast = 1;
-    C.limb_inner = bcast_limb_inner();
+    C.in_bcast = C.limb_inner = 1;
     C.digit_adjacent = 1;
     C.n_dig = n_dig;
     C.reduce_on_load = reduce ? 1 : 0;
@@ -495,8 +494,7 @@ void launch_ntt(const u64* in, u64* out, u32 n_rows, const RowIds& ids, const Li
   if (digit_adjacent) throw CudaFail{cudaErrorNotSupported, "digit-adjacent NTT output needs the TMA kernels"};
   // the register-resident kernels carry the Shoup butterflies only (the Solinas form measured no faster and doubled
   // their code size); FHE_B200_SOLINAS_NTT therefore selects the generic tile kernels, which keep both
-  static const bool generic = getenv("FHE_B200_GENERIC_NTT") != nullptr || getenv("FHE_B200_SOLINAS_NTT") != nullptr;
-  if (generic) {
+  if (switches().generic_tiles()) {
     if (!inverse) {
       run_cols_for<false>(a, st);
       run_rows<6, 6, false>(second, st);
@@ -506,27 +504,16 @@ void launch_ntt(const u64* in, u64* out, u32 n_rows, const RowIds& ids, const Li
     }
     return;
   }
-  // Tile sizes.  Smaller CTAs (same 8 words and <= 64 registers per thread, so the same number of resident warps)
-  // put more independent CTAs on an SM; their load / butterfly / exchange phases interleave and the multiplier
-  // pipe idles less (1024-word cols tiles would mean 16-byte column segments at N = 2^15).
-  // FHE_B200_ROWS_TLOG / FHE_B200_COLS_TLOG = 12 select the 4096-word tiles.
-  static const int rows_tlog = getenv("FHE_B200_ROWS_TLOG") ? atoi(getenv("FHE_B200_ROWS_TLOG")) : 10;
-  static const int cols_tlog = getenv("FHE_B200_COLS_TLOG") ? atoi(getenv("FHE_B200_COLS_TLOG")) : 11;
-  auto rows = [&](const NttArgs& x, bool inv) {
-    if (rows_tlog == 10) { if (inv) run_fast<6, false, true, 10>(x, st); else run_fast<6, false, false, 10>(x, st); }
-    else { if (inv) run_fast<6, false, true>(x, st); else run_fast<6, false, false>(x, st); }
-  };
-  auto cols = [&](const NttArgs& x, bool inv) {
-    // (N = 2^16 would leave a 2048-word tile two columns wide: keep the 4096-word tile there)
-    if (cols_tlog == 11 && x.logn1 <= 9) { if (inv) run_fast_cols_for<true, 11>(x, st); else run_fast_cols_for<false, 11>(x, st); }
-    else { if (inv) run_fast_cols_for<true>(x, st); else run_fast_cols_for<false>(x, st); }
-  };
+  // Tile sizes: 1024-word rows tiles, 2048-word cols tiles.  Smaller CTAs (same 8 words and <= 64 registers per
+  // thread, so the same number of resident warps) put more independent CTAs on an SM; their load / butterfly /
+  // exchange phases interleave and the multiplier pipe idles less (1024-word cols tiles would mean 16-byte column
+  // segments at N = 2^15).
   if (!inverse) {
-    cols(a, false);
-    rows(second, false);
+    run_fast_cols_for<false>(a, st);
+    run_fast<6, false, false, 10>(second, st);
   } else {
-    rows(a, true);
-    cols(second, true);
+    run_fast<6, false, true, 10>(a, st);
+    run_fast_cols_for<true>(second, st);
   }
 }
 

@@ -1,5 +1,5 @@
 // Register-resident variant of the two tile kernels of ntt.cuh for N >= 2^13 (2^TLOG-word tiles,
-// 2^(TLOG-3) threads, 8 words per thread; TLOG = 10 for the rows pass, 11 for the cols pass, see ntt.cu).  Same transform, same tables, same outputs; what changes is
+// 2^(TLOG-3) threads, 8 words per thread; TLOG = 10 for the rows pass, 11 for the cols pass (12 at N = 2^16), see ntt.cu).  Same transform, same tables, same outputs; what changes is
 // the data movement, tuned to the issue limits (the ALU pipe -- address arithmetic, selects, carries --
 // not HBM, bounds the NTT):
 //   * the first round reads its 8 words straight from global memory into registers and the last
@@ -18,7 +18,7 @@ __host__ __device__ constexpr u32 pad_delta(u32 je, u32 S) { return je * S + ((j
 
 // LOGP: log2 points of the in-tile transform; TLOG: log2 words per tile (8 words per thread, 2^(TLOG-3) threads);
 // LOGB = TLOG - LOGP batch lanes; COLS layout as in ntt.cuh.
-template <int LOGP, bool COLS, bool INV, bool SOL, int TLOG = 12>
+template <int LOGP, bool COLS, bool INV, int TLOG>
 struct FastTile {
   static constexpr int LOGB = TLOG - LOGP;
   static constexpr u32 NT = 1u << (TLOG - 3);
@@ -75,7 +75,6 @@ struct FastTile {
                                                  u32 logn, u32 row0, bool first_pass) {
     constexpr int R = 1 << NS;
     const u64 p = L.p, p2 = L.p2;
-    const u32 c = (u32)L.sol_c;
 #pragma unroll
     for (int q = 0; q < (8 >> NS); q++) {
       const u32 root0 = COLS ? 0u : (row0 + g.b[q]);
@@ -100,13 +99,13 @@ struct FastTile {
 #pragma unroll
             for (int e = 0; e < half; e++) {
               const int jj = m * 2 * half + e;
-              bf_fwd<SOL>(v[jj], v[jj + half], w.x, w.y, p, p2, c);
+              bf_fwd<false>(v[jj], v[jj + half], w.x, w.y, p, p2, 0);
             }
           }
         }
         if (s_base + t + NS == (int)logn) {
 #pragma unroll
-          for (int j = 0; j < R; j++) v[j] = fwd_final<SOL>(v[j], p, p2, c);
+          for (int j = 0; j < R; j++) v[j] = fwd_final<false>(v[j], p, p2, 0);
         }
       } else {
         // twiddles of the round up front as in the forward branch
@@ -130,8 +129,8 @@ struct FastTile {
 #pragma unroll
             for (int e = 0; e < half; e++) {
               u64 a = v[e], b2 = v[e + half];
-              v[e] = csub(mul_const_lazy<SOL>(a + b2, L.ninv, L.ninv_s, p, c), p);
-              v[e + half] = csub(mul_const_lazy<SOL>(p2 + a - b2, L.zn, L.zn_s, p, c), p);
+              v[e] = csub(mul_const_lazy<false>(a + b2, L.ninv, L.ninv_s, p, 0), p);
+              v[e + half] = csub(mul_const_lazy<false>(p2 + a - b2, L.zn, L.zn_s, p, 0), p);
             }
           } else {
             const ulonglong2* tp = L.zi + ((1u << logn) - (2u << s) + (root0 << tl) + (g.a_hi[q] << u));
@@ -141,7 +140,7 @@ struct FastTile {
 #pragma unroll
               for (int e = 0; e < half; e++) {
                 const int jj = m * 2 * half + e;
-                bf_inv<SOL>(v[jj], v[jj + half], z.x, z.y, p, p2, c);
+                bf_inv<false>(v[jj], v[jj + half], z.x, z.y, p, p2, 0);
               }
             }
           }
@@ -295,8 +294,8 @@ __global__ void __launch_bounds__(1 << (TLOG - 3), 2 << (12 - TLOG)) ntt_fast_ke
   const LimbDev& L = A.limbs[A.ids[row % A.limbs_per_poly]];
   const bool first_pass = COLS || A.logn1 == 0;
   // (a lazy forward transform never meets the `stage == logn` test that selects the fully reducing last stage)
-  FastTile<LOGP, COLS, INV, false, TLOG>::run(src, dst, gstride_a, sm, A.reduce_on_load != 0, L, s_base,
-                                        (!INV && A.lazy_out) ? 0xffu : A.logn, row0, first_pass);
+  FastTile<LOGP, COLS, INV, TLOG>::run(src, dst, gstride_a, sm, A.reduce_on_load != 0, L, s_base,
+                                 (!INV && A.lazy_out) ? 0xffu : A.logn, row0, first_pass);
 }
 
 }  // namespace fhe_b200

@@ -38,7 +38,7 @@ struct NttTmaArgs {
   u32 logn;
   u32 tiles_per_row;
   u32 tiles_total;     // lpp * tiles_per_row * n_polys; tile index = (j*tiles_per_row + tau)*n_polys + p
-  u32 limb_inner;      // cols pass only: tile index = (tau*n_polys + p)*lpp + j instead (see ntt_tma_cols_kernel)
+  u32 limb_inner;      // = in_bcast (cols pass): tile index = (tau*n_polys + p)*lpp + j instead (see cols_tile)
   unsigned short ids[kMaxPos];
 };
 
@@ -1125,7 +1125,7 @@ __device__ __forceinline__ void cols_round(u32 buf, u32 tw_base, u64 p, u64 p2, 
 }
 
 // tile index -> (limb j, tile position tau, polynomial p).  Limb-major by default: consecutive tiles of a CTA share
-// the limb's twiddles.  A.limb_inner puts the limb innermost, for the digit broadcast (in_bcast): there the Lk tiles
+// the limb's twiddles.  A.limb_inner (set with in_bcast) puts the limb innermost, for the digit broadcast: there the Lk tiles
 // (tau, p, j = 0 .. Lk-1) read the SAME source tile, so back to back only the first read reaches DRAM and the rest
 // hit L2 (limb-major, one limb's pass over a chunk's c2 is far larger than L2 and every limb refetches it), for the
 // price of restaging the 2^LOGP twiddle pairs per tile.

@@ -188,3 +188,38 @@ def test_wide_golden_fixture_matches_oracle(oracle):
     assert (dec(g["switch_to_2"][0], 2) == ma).all()
     assert (dec(g["strategy2"][0]) == (ma * mb) % t).all() and (dec(g["strategy2_relin"][0]) == (ma * mb) % t).all()
     assert (dec(g["mul_3x2"][0]) == (ma * mb * mb) % t).all()
+
+
+def test_environment_switches_are_documented_and_tested():
+    """The engine reads its FHE_B200_* switches in one place (switches(), ntt.cu): no other source under csrc/ calls
+    getenv, the names it reads are exactly the ones the appendix of DESIGN.md lists, and every one of them is set by at
+    least one test's environment parametrization, so every variant they select is parity-tested."""
+    csrc = os.path.join(ROOT, "fhe_rs_b200", "csrc")
+    callers, body = [], None
+    for d, _, files in os.walk(csrc):
+        for f in files:
+            src = open(os.path.join(d, f)).read()
+            if "getenv" in src:
+                callers.append(os.path.relpath(os.path.join(d, f), csrc))
+            m = re.search(r"^const Switches& switches\(\) \{\n(.*?)^\}\n", src, flags=re.S | re.M)
+            if m:
+                body = m.group(1)
+                assert src.count("getenv") == body.count("getenv"), "getenv outside switches() in " + f
+    assert callers == ["ntt.cu"], callers
+    assert body is not None and "getenv" in body
+    read = set(re.findall(r'"(FHE_B200_[A-Z_]+)"', body))
+    design = open(os.path.join(ROOT, "DESIGN.md")).read()
+    table = design.split("## Appendix — environment switches", 1)[1]
+    documented = set()
+    for line in table.splitlines()[1:]:
+        if line.startswith("## "):
+            break
+        if line.startswith("| `"):
+            documented |= set(re.findall(r"FHE_B200_[A-Z_]+", line.split("|")[1]))
+    documented.discard("FHE_B200_LIB")   # read by the Python loader, not by the engine
+    assert read == documented, read ^ documented
+    tested = set()
+    for f in os.listdir(os.path.join(ROOT, "tests")):
+        if f.endswith(".py"):
+            tested |= set(re.findall(r'"(FHE_B200_[A-Z_]+)"\s*:', open(os.path.join(ROOT, "tests", f)).read()))
+    assert read <= tested, read - tested

@@ -1,6 +1,8 @@
 """The three key-switch code paths must produce the same words: the default (the digit transforms' rows pass fused
 with the inner product), FHE_B200_KSMAC=tma (rows pass, then the TMA inner-product kernel) and FHE_B200_KSMAC=classic
-(per-thread inner product), plus the default with one-ciphertext chunks.  Each path runs this file as a script in a
+(per-thread inner product), plus the default with one-ciphertext chunks and the TMA inner product at digit ring
+depths 3 and 4 (FHE_B200_KS_STAGES; the depth-3 run also takes the ring-depth-2 cols pass, FHE_B200_TMA_COLS=2, which
+the mixed-size case enters with reduction on load).  Each path runs this file as a script in a
 subprocess (the switch is read once per process) and the outputs are compared word for word.  The oracle checks of
 test_gpu_parity.py pin the default path to the reference; this test pins the alternatives to it.
 
@@ -18,7 +20,9 @@ pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PATHS = {"fused": {}, "tma": {"FHE_B200_KSMAC": "tma"}, "classic": {"FHE_B200_KSMAC": "classic"},
-         "fused_chunk1": {"FHE_B200_CHUNK": "1"}}
+         "fused_chunk1": {"FHE_B200_CHUNK": "1"},
+         "tma_stages3": {"FHE_B200_KSMAC": "tma", "FHE_B200_KS_STAGES": "3", "FHE_B200_TMA_COLS": "2"},
+         "tma_stages4": {"FHE_B200_KSMAC": "tma", "FHE_B200_KS_STAGES": "4"}}
 
 
 def _rows(rng, moduli, prefix, degree):

@@ -51,6 +51,11 @@ def test_ntt_forward_backward(oracle, F, logn, nmod):
     assert (got == exp).all()
     back = ct.into_power_basis().to_host()
     assert (back == x).all()
+    # an odd number of polynomials per limb (three 1-part polynomials): the TMA rows pass cannot pair them and takes
+    # its one-tile kernel (under FHE_B200_NTT=tma at 2^13 <= N <= 2^15)
+    odd = F.Ciphertext.from_host(gpar, x[:, :1], repr=F.POWER_BASIS)
+    assert (odd.into_ntt().to_host() == exp[:, :1]).all()
+    assert (odd.into_power_basis().to_host() == x[:, :1]).all()
     # backward on arbitrary (reduced) NTT-domain input
     ct2 = F.Ciphertext.from_host(gpar, x, repr=F.NTT)
     got = ct2.into_power_basis().to_host()
@@ -438,12 +443,14 @@ def test_wide_golden_fixture(F):
 
 
 @pytest.mark.parametrize("env", [{"FHE_B200_SOLINAS_NTT": "1"}, {"FHE_B200_NO_SOLINAS": "1"}, {"FHE_B200_GENERIC_NTT": "1"},
-                                 {"FHE_B200_CHUNK": "1"}, {"FHE_B200_ROWS_TLOG": "12", "FHE_B200_COLS_TLOG": "12"},
-                                 {"FHE_B200_NTT": "tma"}, {"FHE_B200_NTT": "fast"},
-                                 {"FHE_B200_NTT": "tma", "FHE_B200_CHUNK": "1"}, {"FHE_B200_SCALER": "classic"}, {"FHE_B200_KSMAC": "classic"}, {"FHE_B200_NO_TENSOR_FUSION": "1"}, {"FHE_B200_NTT": "tma", "FHE_B200_TMA_ROWS": "44"}])
+                                 {"FHE_B200_CHUNK": "1"}, {"FHE_B200_NTT": "tma"}, {"FHE_B200_NTT": "fast"},
+                                 {"FHE_B200_NTT": "tma", "FHE_B200_CHUNK": "1"}, {"FHE_B200_SCALER": "classic"}, {"FHE_B200_KSMAC": "classic"}, {"FHE_B200_NO_TENSOR_FUSION": "1"},
+                                 {"FHE_B200_NTT": "tma", "FHE_B200_TMA_COLS": "2", "FHE_B200_SCALE_UNROLL": "4",
+                                  "FHE_B200_KS_STAGES": "3"}])
 def test_alternate_code_paths(F, env):
     """the optional arithmetic / kernel variants (Solinas twiddle pairs, Barrett-only folds, generic tile NTT,
-    one-ciphertext chunks, 4096-word NTT tiles) must be bit-identical too: rerun the set-A multiply + the 2^13 NTT test under each switch"""
+    one-ciphertext chunks, the TMA kernels' ring depth and unroll alternatives) must be bit-identical too: rerun the
+    set-A multiply + the 2^13 NTT test under each switch"""
     import os
     import subprocess
     import sys
