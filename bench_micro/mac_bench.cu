@@ -1,9 +1,12 @@
 // Throughput of the 64x64 multiply-accumulate forms on one SM sub-partition (clk per MAC per warp):
 //  V0: four plain IMAD.WIDE (no carries; lower bound)   V1: even/odd carry chains (Acc192 in zq.cuh)
 //  V2: 128-bit product then 192-bit add (the r1a form)
+//  V3: three products per term, operands < 2^62 split at bit 31 (AccKara in zq.cuh), at the scaler loop's shape: the
+//      split of r is shared by the NACC outputs, the omega halves and their sums are precomputed
 #include <cstdio>
 #include <cuda_runtime.h>
 #include "device.cuh"
+#include "../fhe_rs_b200/csrc/zq.cuh"
 typedef unsigned long long u64;
 typedef unsigned int u32;
 
@@ -11,7 +14,9 @@ template <int V>
 struct Acc {
   u32 e0, e1, e2, e3, e4, o1, o2, o3;
   u64 lo, mid, hi;
-  __device__ __forceinline__ void clear() { e0 = e1 = e2 = e3 = e4 = o1 = o2 = o3 = 0; lo = mid = hi = 0; }
+  fhe_b200::AccKara kara;
+  __device__ __forceinline__ void clear() { e0 = e1 = e2 = e3 = e4 = o1 = o2 = o3 = 0; lo = mid = hi = 0; kara.clear(); }
+  __device__ __forceinline__ void mac(const fhe_b200::Split31& r, const fhe_b200::Split31& w) { kara.mac(r, w); }
   __device__ __forceinline__ void mac(u64 a, u64 b) {
     if (V == 0) {
       asm volatile("{\n\t.reg .u32 a0,a1,b0,b1;\n\tmov.b64 {a0,a1}, %3;\n\tmov.b64 {b0,b1}, %4;\n\t"
@@ -34,23 +39,38 @@ struct Acc {
       asm volatile("add.cc.u64 %0, %0, %3;\n\taddc.cc.u64 %1, %1, %4;\n\taddc.u64 %2, %2, 0;" : "+l"(lo), "+l"(mid), "+l"(hi) : "l"(pl), "l"(ph));
     }
   }
-  __device__ __forceinline__ u64 fin() const { return lo ^ mid ^ hi ^ e0 ^ e1 ^ e2 ^ e3 ^ e4 ^ o1 ^ o2 ^ o3; }
+  __device__ __forceinline__ u64 fin() const {
+    u64 a, b;
+    u32 c;
+    kara.merged(a, b, c);
+    return lo ^ mid ^ hi ^ e0 ^ e1 ^ e2 ^ e3 ^ e4 ^ o1 ^ o2 ^ o3 ^ (V == 3 ? a ^ b ^ c : 0);
+  }
 };
 
 template <int V, int NACC>
 __global__ void k(u64* out, u64 seed, int iters) {
   Acc<V> acc[NACC];
   u64 w[8];
+  fhe_b200::Split31 ws[8];
 #pragma unroll
   for (int i = 0; i < NACC; i++) acc[i].clear();
 #pragma unroll
-  for (int i = 0; i < 8; i++) w[i] = (seed * (threadIdx.x + 17 + i)) & 0x3fffffffffffffffull;
-  u64 r = seed ^ threadIdx.x;
+  for (int i = 0; i < 8; i++) {
+    w[i] = (seed * (threadIdx.x + 17 + i)) & 0x3fffffffffffffffull;
+    ws[i] = fhe_b200::split31(w[i]);
+  }
+  u64 r = (seed ^ threadIdx.x) & 0x3fffffffffffffffull;
   for (int it = 0; it < iters; it++) {
 #pragma unroll
     for (int u = 0; u < 8 / NACC * 1; u++) {
+      if (V == 3) {
+        const fhe_b200::Split31 rs = fhe_b200::split31(r);
 #pragma unroll
-      for (int a = 0; a < NACC; a++) acc[a].mac(r, w[(u * NACC + a) & 7]);
+        for (int a = 0; a < NACC; a++) acc[a].mac(rs, ws[(u * NACC + a) & 7]);
+      } else {
+#pragma unroll
+        for (int a = 0; a < NACC; a++) acc[a].mac(r, w[(u * NACC + a) & 7]);
+      }
       r = (r + 0x9e3779b97f4a7c15ull) & 0x3fffffffffffffffull;
     }
   }
@@ -81,7 +101,7 @@ void run(int warps_per_smsp) {
 }
 int main() {
   for (int w : {1, 2, 4, 6, 12}) {
-    run<0, 4>(w); run<1, 4>(w); run<2, 4>(w);
+    run<0, 4>(w); run<1, 4>(w); run<2, 4>(w); run<3, 4>(w);
   }
   run<1, 1>(6); run<1, 2>(6); run<1, 8>(6); run<2, 2>(6); run<2, 1>(6);
   return 0;

@@ -264,21 +264,37 @@ __device__ __forceinline__ U256 u256_mul_128(u128 v, u64 tlo, u64 thi) {
 // chain lacks; the register-resident one-limb-at-a-time form was latency-bound on that chain).
 constexpr int kScaleTC = 128;
 
-// sum_i r_i * omega_{j0+k, i} for the G (<= 4) output limbs of one group
+// The omega table in shared memory: omega_ji (< q_j < 2^62) split at bit 31 into three u32 planes per source row i,
+// [i][w0, w1, w0 + w1][n_out4], so the four output limbs of a group take three 128-bit loads per term.
+__device__ __forceinline__ void stage_omega_split(u32* s_om, const ScalerDev& S, u32 start, u32 n_out, u32 n_out4) {
+  const u32 nf = S.n_from;
+  for (u32 idx = threadIdx.x; idx < nf * n_out4; idx += blockDim.x) {
+    const u32 ii = idx / n_out4, jj = idx - ii * n_out4;
+    const Split31 w = split31(jj < n_out ? S.omega[(size_t)(start + jj) * nf + ii] : 0);
+    u32* row = s_om + (size_t)ii * 3 * n_out4 + jj;
+    row[0] = w.lo;
+    row[n_out4] = w.hi;
+    row[2 * n_out4] = w.sum;
+  }
+}
+
+// sum_i r_i * omega_{j0+k, i} for the G (<= 4) output limbs of one group, three products per term (AccKara: every
+// r_i is a canonical residue and every omega_ji is reduced, both < 2^62).  The unroll stays bounded: fully unrolled,
+// ptxas keeps carry predicates alive across terms and parks them in registers.
 template <int G, int UNR = 2>
-__device__ __forceinline__ void scale_mac_group(Acc192 (&acc)[4], const u64* r_col, const ulonglong2* om, u32 nf,
-                                                u32 om_stride) {
+__device__ __forceinline__ void scale_mac_group(AccKara (&acc)[4], const u64* r_col, const u32* om, u32 nf,
+                                                u32 n_out4) {
 #pragma unroll UNR
   for (u32 i = 0; i < nf; i++) {
-    const u64 r = r_col[i * kScaleTC];
-    const ulonglong2 o0 = om[(size_t)i * om_stride];
-    acc[0].mac(r, o0.x);
-    if (G > 1) acc[1].mac(r, o0.y);
-    if (G > 2) {
-      const ulonglong2 o1 = om[(size_t)i * om_stride + 1];
-      acc[2].mac(r, o1.x);
-      if (G > 3) acc[3].mac(r, o1.y);
-    }
+    const Split31 r = split31(r_col[i * kScaleTC]);
+    const u32* row = om + (size_t)i * 3 * n_out4;
+    const uint4 w0 = *reinterpret_cast<const uint4*>(row);
+    const uint4 w1 = *reinterpret_cast<const uint4*>(row + n_out4);
+    const uint4 ws = *reinterpret_cast<const uint4*>(row + 2 * n_out4);
+    acc[0].mac(r.lo, r.hi, r.sum, w0.x, w1.x, ws.x);
+    if (G > 1) acc[1].mac(r.lo, r.hi, r.sum, w0.y, w1.y, ws.y);
+    if (G > 2) acc[2].mac(r.lo, r.hi, r.sum, w0.z, w1.z, ws.z);
+    if (G > 3) acc[3].mac(r.lo, r.hi, r.sum, w0.w, w1.w, ws.w);
   }
 }
 
@@ -289,8 +305,8 @@ __global__ void __launch_bounds__(kScaleTC) scale_kernel(ScaleArgs A) {
   const u32 n_out4 = (n_out + 3) & ~3u;
   constexpr u32 TC = kScaleTC;
   u64* s_r = smem;                                // [n_from][TC]
-  u64* s_omega = s_r + (size_t)nf * TC;           // [n_from][n_out4]  (transposed)
-  u64* s_gamma = s_omega + (size_t)nf * n_out4;   // [n_out4]
+  u32* s_omega = reinterpret_cast<u32*>(s_r + (size_t)nf * TC);   // [n_from][3][n_out4]  (stage_omega_split)
+  u64* s_gamma = reinterpret_cast<u64*>(s_omega + (size_t)nf * 3 * n_out4);   // [n_out4]
   u64* s_tgl = s_gamma + n_out4;                  // theta tables [n_from]
   u64* s_tgh = s_tgl + nf;
   u64* s_tol = s_tgh + nf;
@@ -317,10 +333,7 @@ __global__ void __launch_bounds__(kScaleTC) scale_kernel(ScaleArgs A) {
     asm volatile("cp.async.commit_group;" ::: "memory");
   }
   // the (L2-resident) tables, spread over the whole CTA
-  for (u32 idx = cc; idx < nf * n_out4; idx += TC) {
-    const u32 ii = idx / n_out4, jj = idx - ii * n_out4;
-    s_omega[idx] = jj < n_out ? S.omega[(size_t)(A.start + jj) * nf + ii] : 0;
-  }
+  stage_omega_split(s_omega, S, A.start, n_out, n_out4);
   for (u32 i = cc; i < n_out4; i += TC) s_gamma[i] = i < n_out ? S.gamma[A.start + i] : 0;
   for (u32 i = cc; i < nf; i += TC) {
     s_tgl[i] = S.tgar_lo[i];
@@ -386,17 +399,17 @@ __global__ void __launch_bounds__(kScaleTC) scale_kernel(ScaleArgs A) {
 
   // outputs (:316-351): y_j = (-(v mod q_j) * gamma_j +/- w + sum_i r_i * omega_ji) mod q_j, four limbs at a time
   for (u32 j0 = 0; j0 < n_out; j0 += 4) {
-    Acc192 acc[4];
+    AccKara acc[4];
 #pragma unroll
     for (int k = 0; k < 4; k++) acc[k].clear();
-    const ulonglong2* om = reinterpret_cast<const ulonglong2*>(s_omega + j0);
+    const u32* om = s_omega + j0;
     // the multiplier pipe bounds this loop (bench_micro/mac_bench.cu), so the last group only multiplies for the
     // limbs it really has (14 outputs = 4+4+4+2, not 16)
     switch (min(4u, n_out - j0)) {
-      case 4: scale_mac_group<4>(acc, s_r + cc, om, nf, n_out4 / 2); break;
-      case 3: scale_mac_group<3>(acc, s_r + cc, om, nf, n_out4 / 2); break;
-      case 2: scale_mac_group<2>(acc, s_r + cc, om, nf, n_out4 / 2); break;
-      default: scale_mac_group<1>(acc, s_r + cc, om, nf, n_out4 / 2); break;
+      case 4: scale_mac_group<4>(acc, s_r + cc, om, nf, n_out4); break;
+      case 3: scale_mac_group<3>(acc, s_r + cc, om, nf, n_out4); break;
+      case 2: scale_mac_group<2>(acc, s_r + cc, om, nf, n_out4); break;
+      default: scale_mac_group<1>(acc, s_r + cc, om, nf, n_out4); break;
     }
 #pragma unroll
     for (int k = 0; k < 4; k++) {
@@ -404,7 +417,7 @@ __global__ void __launch_bounds__(kScaleTC) scale_kernel(ScaleArgs A) {
       if (jj >= n_out) break;
       const LimbDev& M = A.limbs[S.to_ids[A.start + jj]];
       u64 vr = reduce94_limb((u64)v, (u64)(v >> 64), M);   // v < n_from * 2^63
-      acc[k].mac(vr ? M.p - vr : 0, s_gamma[jj]);
+      acc[k].mac(split31(vr ? M.p - vr : 0), split31(s_gamma[jj]));
       if (!S.is_one) {
         u64 wr = reduce94_limb((u64)w, (u64)(w >> 64), M); // w < 2^70
         acc[k].add64(w_sign ? (wr ? M.p - wr : 0) : wr);
@@ -454,8 +467,8 @@ __global__ void __launch_bounds__(kScaleTC) scale_tma_kernel(const __grid_consta
   const u32 n_out4 = (n_out + 3) & ~3u;
   constexpr u32 TC = kScaleTC;
   u64* s_r = smem;                                // [n_from][TC]   (TMA destination, 128-byte aligned)
-  u64* s_omega = s_r + (size_t)nf * TC;           // [n_from][n_out4]  (transposed)
-  u64* s_gamma = s_omega + (size_t)nf * n_out4;   // [n_out4]
+  u32* s_omega = reinterpret_cast<u32*>(s_r + (size_t)nf * TC);   // [n_from][3][n_out4]  (stage_omega_split)
+  u64* s_gamma = reinterpret_cast<u64*>(s_omega + (size_t)nf * 3 * n_out4);   // [n_out4]
   u64* s_p2 = s_gamma + n_out4;                   // [n_out4]  2 q_j
   u64* s_c = s_p2 + n_out4;                       // [n_out4]  c_j = 2^62 - q_j
   u64* s_tgl = s_c + n_out4;                      // theta_garner [n_from]
@@ -467,10 +480,7 @@ __global__ void __launch_bounds__(kScaleTC) scale_tma_kernel(const __grid_consta
   const u32 bar = smem_u32(s_bar);
   const u32 cc = threadIdx.x;
 
-  for (u32 idx = cc; idx < nf * n_out4; idx += TC) {
-    const u32 ii = idx / n_out4, jj = idx - ii * n_out4;
-    s_omega[idx] = jj < n_out ? S.omega[(size_t)(A.start + jj) * nf + ii] : 0;
-  }
+  stage_omega_split(s_omega, S, A.start, n_out, n_out4);
   for (u32 i = cc; i < n_out4; i += TC) {
     const bool live = i < n_out;
     const LimbDev& M = A.limbs[S.to_ids[A.start + (live ? i : 0)]];
@@ -571,16 +581,16 @@ __global__ void __launch_bounds__(kScaleTC) scale_tma_kernel(const __grid_consta
 
     // outputs (:316-351): y_j = (-(v mod q_j) * gamma_j +/- w + sum_i r_i * omega_ji) mod q_j, four limbs at a time
     for (u32 j0 = 0; j0 < n_out; j0 += 4) {
-      Acc192 acc[4];
+      AccKara acc[4];
 #pragma unroll
       for (int k = 0; k < 4; k++) acc[k].clear();
-      const ulonglong2* om = reinterpret_cast<const ulonglong2*>(s_omega + j0);
+      const u32* om = s_omega + j0;
       const u32 g = min(4u, n_out - j0);
       switch (g) {
-        case 4: scale_mac_group<4, UNR>(acc, s_r + cc, om, nf, n_out4 / 2); break;
-        case 3: scale_mac_group<3, UNR>(acc, s_r + cc, om, nf, n_out4 / 2); break;
-        case 2: scale_mac_group<2, UNR>(acc, s_r + cc, om, nf, n_out4 / 2); break;
-        default: scale_mac_group<1, UNR>(acc, s_r + cc, om, nf, n_out4 / 2); break;
+        case 4: scale_mac_group<4, UNR>(acc, s_r + cc, om, nf, n_out4); break;
+        case 3: scale_mac_group<3, UNR>(acc, s_r + cc, om, nf, n_out4); break;
+        case 2: scale_mac_group<2, UNR>(acc, s_r + cc, om, nf, n_out4); break;
+        default: scale_mac_group<1, UNR>(acc, s_r + cc, om, nf, n_out4); break;
       }
       if (j0 + 4 >= n_out) {
         // the tile has been read for the last time: fetch the next one while the last epilogue runs
@@ -597,7 +607,8 @@ __global__ void __launch_bounds__(kScaleTC) scale_tma_kernel(const __grid_consta
         if (jj >= n_out) break;
         const u64 p2 = s_p2[jj];
         const u32 c = (u32)s_c[jj];
-        acc[k].mac(p2 - ((u64)vh * c + vl), s_gamma[jj]);      // -(v mod q) * gamma, as a positive multiple
+        // -(v mod q) * gamma as a positive multiple: 2q - v' is in (0, 2q], brought to [0, q] for the split
+        acc[k].mac(split31(csub(p2 - ((u64)vh * c + vl), p2 >> 1)), split31(s_gamma[jj]));
         if (!IS_ONE) {
           const u64 wr = (u64)wh * c + wl;                     // w mod q in [0, 2q)
           acc[k].add64(w_sign ? p2 - wr : wr);
@@ -1141,7 +1152,8 @@ static bool launch_scale_tma(const ScalerDev& S, const LimbDev* limbs, const u64
   A.split3 = split3; A.logn = logn;
   A.tiles_total = polys * (N / kScaleTC);
   const size_t n_out4 = (n_out + 3) & ~(size_t)3;
-  const size_t smem = (nf * kScaleTC + nf * n_out4 + 3 * n_out4 + 4 * nf) * sizeof(u64) + ((nf + 1) & ~(size_t)1) * 4 + 16;
+  const size_t smem = (nf * kScaleTC + 3 * n_out4 + 4 * nf) * sizeof(u64) + nf * 3 * n_out4 * sizeof(u32) +
+                      ((nf + 1) & ~(size_t)1) * 4 + 16;
   // persistent grid = exactly the CTAs that are resident at once (registers and shared memory both limit it)
   auto resident = [&](const void* k) {
     ensure_dynamic_smem(k, smem);
@@ -1178,7 +1190,7 @@ void launch_scale(const ScalerDev& S, const LimbDev* limbs, const u64* in, u64* 
     return;
   }
   const size_t n_out4 = (n_out + 3) & ~(size_t)3, nf = S.n_from;
-  const size_t smem = (nf * kScaleTC + nf * n_out4 + n_out4 + 5 * nf) * sizeof(u64);
+  const size_t smem = (nf * kScaleTC + n_out4 + 5 * nf) * sizeof(u64) + nf * 3 * n_out4 * sizeof(u32);
   ensure_dynamic_smem((const void*)scale_kernel, smem);
   scale_kernel<<<polys * (N / kScaleTC), kScaleTC, smem, st>>>(A);
   g_launches++;

@@ -283,14 +283,23 @@ __device__ __forceinline__ u64 fold192_solinas(u64 lo, u64 mid, u64 hi, u32 c) {
   fold_step_solinas(lo, mid, 0, c);                      // < 2^93
   return fold94_solinas(lo, mid, c);
 }
+// residue in [0,2p) of a lazy sum hi*2^128 + mid*2^64 + lo < 2^160 in the limb's mode (Solinas fold or Barrett)
+__device__ __forceinline__ u64 reduce160_lazy(u64 lo, u64 mid, u64 hi, const LimbDev& m) {
+  if (m.sol_c) return fold192_solinas(lo, mid, hi, (u32)m.sol_c);
+  u64 r1 = barrett128_lazy(lo, mid, m.p, m.bhi, m.blo);  // [0,2p)
+  u64 hl = hi * m.c128, hh = __umul64hi(hi, m.c128);
+  u64 r2 = barrett128_lazy(hl, hh, m.p, m.bhi, m.blo);   // [0,2p)
+  return csub(r1 + r2, m.p2);
+}
 
 // Lazy multiply-accumulate register: sum of 64x64-bit products, exact up to 2^160, reduced once at the end
-// (used by the RNS scaler and the key-switch inner product; replaces the reference's per-term Shoup
+// (used by the key-switch inner product, the tensor and the scaler of rings below one tile; replaces the reference's per-term Shoup
 // reduction, rns/scaler.rs:340-347 and rq/ops.rs:208).
 // The four 32x32 partial products of a term go to two column sets that are never added to each other inside the
 // loop: the even one (e0..e4, products aligned at words 0 and 2) and the odd one (o1..o3, aligned at word 1).
 // Each mad.lo.cc/madc.hi.cc pair is ONE IMAD.WIDE.U32 with carry-out (and carry-in for the second of a chain), so
-// a term costs 4 IMAD.WIDE + 2 IADD3.X -- the FMA-pipe minimum -- instead of 4 IMAD.WIDE + 9 carry-chain adds of
+// a term costs 4 IMAD.WIDE + 2 IADD3.X -- the minimum of the schoolbook product (AccKara below takes three products
+// when both operands are < 2^62) -- instead of 4 IMAD.WIDE + 9 carry-chain adds of
 // the 128-bit-product-then-192-bit-add form, whose carry-chain adds load the ALU pipe more than its multiplies do.
 struct Acc192 {
   u32 e0, e1, e2, e3, e4, o1, o2, o3;
@@ -343,26 +352,108 @@ struct Acc192 {
   // residue in [0,2p) of the accumulated value (which must be < 2^160)
   __device__ __forceinline__ u64 reduce_lazy(const LimbDev& m) const {
     u64 lo, mid;
-    u32 hi32;
-    merged(lo, mid, hi32);
-    const u64 hi = hi32;
-    if (m.sol_c) return fold192_solinas(lo, mid, hi, (u32)m.sol_c);
-    u64 r1 = barrett128_lazy(lo, mid, m.p, m.bhi, m.blo);  // [0,2p)
-    u64 hl = hi * m.c128, hh = __umul64hi(hi, m.c128);
-    u64 r2 = barrett128_lazy(hl, hh, m.p, m.bhi, m.blo);   // [0,2p)
-    return csub(r1 + r2, m.p2);
+    u32 hi;
+    merged(lo, mid, hi);
+    return reduce160_lazy(lo, mid, hi, m);
   }
   // canonical residue of the accumulated value (which must be < 2^160)
   __device__ __forceinline__ u64 reduce(const LimbDev& m) const {
     u64 lo, mid;
-    u32 hi32;
-    merged(lo, mid, hi32);
-    const u64 hi = hi32;
-    if (m.sol_c) return csub(fold192_solinas(lo, mid, hi, (u32)m.sol_c), m.p);
-    u64 r1 = barrett128_lazy(lo, mid, m.p, m.bhi, m.blo);  // [0,2p)
-    u64 hl = hi * m.c128, hh = __umul64hi(hi, m.c128);
-    u64 r2 = barrett128_lazy(hl, hh, m.p, m.bhi, m.blo);   // [0,2p)
-    return csub(csub(r1 + r2, m.p2), m.p);
+    u32 hi;
+    merged(lo, mid, hi);
+    return csub(reduce160_lazy(lo, mid, hi, m), m.p);
+  }
+};
+
+// Lazy multiply-accumulate of terms r*w with BOTH operands < 2^62, three 32x32 products per term instead of four.
+// The caller splits each operand at bit 31 (split31: r = r1*2^31 + r0, halves < 2^31, half sum rs = r0 + r1 < 2^32),
+// and Karatsuba gives
+//   r*w = r0*w0 + 2^31*[(r0+r1)(w0+w1) - r0*w0 - r1*w1] + 2^62*r1*w1 .
+// The three products go to three 96-bit column sums L = sum r0*w0, M = sum rs*ws, H = sum r1*w1, each its own
+// mad.lo.cc/madc.hi.cc/addc chain (one IMAD.WIDE with carry + one IADD3.X), no carry crossing between them; merged()
+// combines them once.  Bounds for n terms and k add64 addends: r0*w0, r1*w1 < 2^62 and rs*ws < 2^64, so the sums are
+// exact while n + k < 2^32; M - L - H = sum (r0*w1 + r1*w0) >= 0 because add64 adds to L and M alike; the value
+// V = sum r*w + sum addends < n*2^124 + k*2^64 < 2^160, the contract of Acc192::merged (the scaler: n <= 65, k <= 1).
+// An operand of 2^62 or more breaks the split (r1 or rs no longer fits its word): such terms go through Acc192.
+struct Split31 {
+  u32 lo, hi, sum;
+};
+__device__ __forceinline__ Split31 split31(u64 x) {
+  const u32 lo = (u32)x & 0x7fffffffu, hi = (u32)(x >> 31);
+  return {lo, hi, lo + hi};
+}
+struct AccKara {
+  // the low two words of each sum are one 64-bit register, so the pair an IMAD.WIDE adds into stays in place
+  u64 l, m, h;
+  u32 l2, m2, h2;
+  __device__ __forceinline__ void clear() { l = m = h = 0; l2 = m2 = h2 = 0; }
+  __device__ __forceinline__ void mac(u32 r0, u32 r1, u32 rs, u32 w0, u32 w1, u32 ws) {
+    asm("{\n\t"
+        ".reg .u32 x0, x1, y0, y1, z0, z1;\n\t"
+        "mov.b64 {x0, x1}, %0;\n\t"
+        "mov.b64 {y0, y1}, %1;\n\t"
+        "mov.b64 {z0, z1}, %2;\n\t"
+        "mad.lo.cc.u32 x0, %6, %9, x0;\n\t"
+        "madc.hi.cc.u32 x1, %6, %9, x1;\n\t"
+        "addc.u32 %3, %3, 0;\n\t"
+        "mad.lo.cc.u32 y0, %8, %11, y0;\n\t"
+        "madc.hi.cc.u32 y1, %8, %11, y1;\n\t"
+        "addc.u32 %4, %4, 0;\n\t"
+        "mad.lo.cc.u32 z0, %7, %10, z0;\n\t"
+        "madc.hi.cc.u32 z1, %7, %10, z1;\n\t"
+        "addc.u32 %5, %5, 0;\n\t"
+        "mov.b64 %0, {x0, x1};\n\t"
+        "mov.b64 %1, {y0, y1};\n\t"
+        "mov.b64 %2, {z0, z1};\n\t"
+        "}"
+        : "+l"(l), "+l"(m), "+l"(h), "+r"(l2), "+r"(m2), "+r"(h2)
+        : "r"(r0), "r"(r1), "r"(rs), "r"(w0), "r"(w1), "r"(ws));
+  }
+  __device__ __forceinline__ void mac(const Split31& r, const Split31& w) { mac(r.lo, r.hi, r.sum, w.lo, w.hi, w.sum); }
+  __device__ __forceinline__ void add64(u64 v) {
+    asm("add.cc.u64 %0, %0, %4;\n\t"
+        "addc.u32 %1, %1, 0;\n\t"
+        "add.cc.u64 %2, %2, %4;\n\t"
+        "addc.u32 %3, %3, 0;"
+        : "+l"(l), "+r"(l2), "+l"(m), "+r"(m2)
+        : "l"(v));
+  }
+  // value = hi * 2^128 + mid * 2^64 + lo = L + 2^31 * (M - L - H) + 2^62 * H
+  __device__ __forceinline__ void merged(u64& lo, u64& mid, u32& hi) const {
+    const u32 l0 = (u32)l, l1 = (u32)(l >> 32), h0 = (u32)h, h1 = (u32)(h >> 32);
+    u32 d0, d1, d2;
+    asm("sub.cc.u32 %0, %3, %6;\n\t"
+        "subc.cc.u32 %1, %4, %7;\n\t"
+        "subc.u32 %2, %5, %8;\n\t"
+        "sub.cc.u32 %0, %0, %9;\n\t"
+        "subc.cc.u32 %1, %1, %10;\n\t"
+        "subc.u32 %2, %2, %11;"
+        : "=r"(d0), "=r"(d1), "=r"(d2)
+        : "r"((u32)m), "r"((u32)(m >> 32)), "r"(m2), "r"(l0), "r"(l1), "r"(l2), "r"(h0), "r"(h1), "r"(h2));
+    // D * 2^31 and H * 2^62 as five little-endian words (H * 2^62 has none at word 0)
+    const u32 a0 = d0 << 31, a1 = __funnelshift_l(d0, d1, 31), a2 = __funnelshift_l(d1, d2, 31), a3 = d2 >> 1;
+    const u32 b1 = h0 << 30, b2 = __funnelshift_l(h0, h1, 30), b3 = __funnelshift_l(h1, h2, 30), b4 = h2 >> 2;
+    u32 w0, w1, w2, w3;
+    asm("add.cc.u32 %0, %5, %8;\n\t"
+        "addc.cc.u32 %1, %6, %9;\n\t"
+        "addc.cc.u32 %2, %7, %10;\n\t"
+        "addc.cc.u32 %3, %11, 0;\n\t"
+        "addc.u32 %4, %15, 0;\n\t"
+        "add.cc.u32 %1, %1, %12;\n\t"
+        "addc.cc.u32 %2, %2, %13;\n\t"
+        "addc.cc.u32 %3, %3, %14;\n\t"
+        "addc.u32 %4, %4, 0;"
+        : "=r"(w0), "=r"(w1), "=r"(w2), "=r"(w3), "=r"(hi)
+        : "r"(l0), "r"(l1), "r"(l2), "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b1), "r"(b2), "r"(b3), "r"(b4));
+    lo = ((u64)w1 << 32) | w0;
+    mid = ((u64)w3 << 32) | w2;
+  }
+  // canonical residue of the accumulated value
+  __device__ __forceinline__ u64 reduce(const LimbDev& m) const {
+    u64 lo, mid;
+    u32 hi;
+    merged(lo, mid, hi);
+    return csub(reduce160_lazy(lo, mid, hi, m), m.p);
   }
 };
 
