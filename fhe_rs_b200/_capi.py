@@ -43,6 +43,7 @@ SYMBOLS = {
     "fhe_b200_batch_download": (_i, [_vp, _u32, _u32, _vp, _vp]),
     "fhe_b200_batch_download_async": (_i, [_vp, _u32, _u32, _vp, _vp]),
     "fhe_b200_batch_copy": (_i, [_vp, _vp, _vp]),
+    "fhe_b200_batch_copy_range": (_i, [_vp, _u32, _vp, _u32, _u32, _u32, _vp]),
     "fhe_b200_host_alloc": (_i, [C.c_size_t, _i, _pp]),
     "fhe_b200_host_free": (_i, [_vp]),
     "fhe_b200_batch_device_ptr": (_i, [_vp, _pp, C.POINTER(C.c_size_t)]),
@@ -69,6 +70,7 @@ SYMBOLS = {
     "fhe_b200_multiplicator_free": (_i, [_vp]),
     "fhe_b200_multiplicator_multiply": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp]),
     "fhe_b200_galois": (_i, [_vp, _u32, _vp, _vp, _vp]),
+    "fhe_b200_expand": (_i, [_vp, _u32, _pp, _u32, _vp, _vp]),
     "fhe_b200_substitute": (_i, [_vp, _u32, _vp, _vp]),
     "fhe_b200_switch_down": (_i, [_vp, _vp]),
     "fhe_b200_key_switch": (_i, [_vp, _u32, _vp, _vp, _vp]),
@@ -81,6 +83,7 @@ SYMBOLS = {
     "fhe_b200_launch_count": (_u64, []),
     "fhe_b200_debug_scaler_tables": (_i, [_vp, _u32, _i, _pu32, _pu32, _pu32] + [_vp] * 8),
     "fhe_b200_debug_ntt_tables": (_i, [_vp, _u64, _vp, _vp, _vp, _vp, _pu64]),
+    "fhe_b200_debug_expansion_monomial": (_i, [_vp, _u32, _u32, _vp]),
     "fhe_b200_debug_encoder_tables": (_i, [_vp, _u32, _vp, _vp, _vp, _pu64, _vp]),
 }
 

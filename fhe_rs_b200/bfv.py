@@ -380,6 +380,13 @@ class Ciphertext:
         check(_capi.lib().fhe_b200_batch_copy(out._h, self._h, self.stream))
         return out
 
+    def take(self, first: int, n: int, stride: int = 1) -> "Ciphertext":
+        """a new batch of the n ciphertexts first, first + stride, ..., first + (n-1)*stride (fhe_b200_batch_copy_range)"""
+        c, p, lv, _, r = self._info()
+        out = Ciphertext(self.par, n, p, lv, r, self.stream)
+        check(_capi.lib().fhe_b200_batch_copy_range(out._h, 0, self._h, first, stride, n, self.stream))
+        return out
+
     # -- representation (Poly::into_ntt / into_power_basis, rq/mod.rs:535, :590)
     def into_ntt(self) -> "Ciphertext":
         check(_capi.lib().fhe_b200_ntt_forward(self._h, self.stream))
@@ -827,30 +834,33 @@ class EvaluationKey:
         out += self.gk[2 * self.par.degree() - 1].relinearize(out)
         return out
 
-    def expands(self, ct: Ciphertext, size: int, monomials: Sequence[np.ndarray]):
-        """EvaluationKey::expands (evaluation_key.rs:192-256), oblivious expansion of eprint 2019/1483.
-        monomials[l]: NTT words [limbs][N] of -x^(N - 2^l) (evaluation_key.rs:465-474)."""
+    def supports_expansion(self, level: int) -> bool:  # evaluation_key.rs:175-189
         n = self.par.degree()
-        if size == 0 or size > n:
-            raise FheError(_capi.INVALID_ARGUMENT, "EvaluationKeyError: invalid expansion size")
-        level = (size - 1).bit_length()
-        out = [None] * (1 << level)
-        out[0] = ct.clone()
+        return level == 0 or (level <= n.bit_length() - 1 and all(((n >> l) + 1) in self.gk for l in range(level)))
+
+    def expands_batch(self, ct: Ciphertext, size: int) -> Ciphertext:
+        """EvaluationKey::expands (evaluation_key.rs:192-256) of every ciphertext of `ct` (Q queries) as one batch of
+        size * Q: entry i*Q + q is output i of query q (fhe_b200_expand)."""
+        n = self.par.degree()
+        level = max(0, (size - 1).bit_length())
+        keys = (C.c_void_p * max(1, level))()
         for l in range(level):
-            gk = self.gk.get((n >> l) + 1)
-            if gk is None or l >= len(monomials):
-                raise FheError(_capi.INVALID_ARGUMENT, "EvaluationKeyError: expansion not supported by this key")
-            step = 1 << l
-            for i in range(step):
-                sub = gk.relinearize(out[i])
-                j = step | i
-                if j < size:
-                    tgt = out[i].clone()
-                    tgt -= sub
-                    tgt.mul_plain(monomials[l])
-                    out[j] = tgt
-                out[i] += sub
-        return out[:size]
+            gk = self.gk.get((n >> l) + 1) if l < n.bit_length() - 1 else None
+            keys[l] = gk.ksk._h.value if gk is not None else None
+        # (an out-of-range size allocates a placeholder: fhe_b200_expand rejects the size before it looks at `out`)
+        out = Ciphertext(self.par, size * ct.count if 0 < size <= n else 1, 2, ct.level, NTT, ct.stream)
+        check(_capi.lib().fhe_b200_expand(ct._h, size, C.cast(keys, C.POINTER(C.c_void_p)), level, out._h, ct.stream))
+        return out
+
+    def expands(self, ct: Ciphertext, size: int, monomials: Optional[Sequence[np.ndarray]] = None):
+        """EvaluationKey::expands (evaluation_key.rs:192-256), oblivious expansion of eprint 2019/1483: a list of `size`
+        batches of ct.count ciphertexts, output i of every query.  `monomials` is accepted for older callers and
+        ignored: the monomials -x^(N - 2^l) (:465-474) are fixed by the parameters and built by the library."""
+        if size == 0 or size > self.par.degree():
+            raise FheError(_capi.INVALID_ARGUMENT, "EvaluationKeyError: invalid expansion size")
+        whole = self.expands_batch(ct, size)
+        q = ct.count
+        return [whole.take(i * q, q) for i in range(size)]
 
     def rotates_rows(self, ct: Ciphertext) -> Ciphertext:  # evaluation_key.rs:110-126
         e = 2 * self.par.degree() - 1

@@ -207,6 +207,51 @@ struct fhe_b200_params {
     perms[exponent] = d;
     return d;
   }
+
+  // The expansion monomial -x^(N - 2^l) of EvaluationKey (evaluation_key.rs:465-474) at level `lv`, NTT words [L][N].
+  // The forward NTT evaluates at psi^(2 bitrev(i) + 1) and psi^N = -1, so -z^(N - 2^l) = z^(-2^l) at every point z:
+  // word i of limb q is psi_q^(-(2^l) (2 bitrev(i) + 1) mod 2N).  l < log2 N.
+  std::vector<u64> expansion_monomial(u32 lv, u32 l) const {
+    const u32 L = level(lv).L;
+    const u64 m = 2 * (u64)N;
+    std::vector<u64> out((size_t)L * N), pw(m);
+    for (u32 j = 0; j < L; j++) {
+      const u64 q = moduli[j];
+      pw[0] = 1;
+      for (u64 k = 1; k < m; k++) pw[k] = mulmod_h(pw[k - 1], psi[j], q);
+      for (u32 i = 0; i < N; i++) {
+        u32 r = 0;
+        for (u32 b = 0; b < logn; b++) r |= ((i >> b) & 1) << (logn - 1 - b);
+        const u64 e = (((u64)(2 * r + 1)) << l) % m;
+        out[(size_t)j * N + i] = pw[(m - e) % m];
+      }
+    }
+    return out;
+  }
+  // the same as (value, Shoup companion) pairs on the device, built on first use per (level, l)
+  const ulonglong2* expansion_monomial_dev(u32 lv, u32 l) const {
+    {
+      std::lock_guard<std::mutex> g(mu);
+      auto it = monos.find({lv, l});
+      if (it != monos.end()) return it->second;
+    }
+    const std::vector<u64> w = expansion_monomial(lv, l);   // level() takes the mutex itself
+    std::lock_guard<std::mutex> g(mu);
+    auto it = monos.find({lv, l});
+    if (it != monos.end()) return it->second;
+    std::vector<ulonglong2> pairs(w.size());
+    for (size_t j = 0; j < w.size() / N; j++) {
+      const ModulusH mq(moduli[j]);
+      for (size_t k = j * N; k < (j + 1) * N; k++) {
+        pairs[k].x = w[k];
+        pairs[k].y = mq.shoup(w[k]);
+      }
+    }
+    const ulonglong2* d = to_dev(pairs);
+    monos[{lv, l}] = d;
+    return d;
+  }
+  mutable std::map<std::pair<u32, u32>, const ulonglong2*> monos;
 };
 
 struct fhe_b200_batch {
@@ -534,6 +579,22 @@ void key_switch_apply(const fhe_b200_params* par, const fhe_b200_ksk* k, const u
       launch_ew(EW_ADD, out, base, (size_t)cts * 2 * L, cl.ctx_ids, par->d_limbs, logn, st);
     }
   }
+}
+
+// GaloisKey::relinearize (galois_key.rs:63-86) of n 2-part NTT ciphertexts [n][2][L][N] at `src` into `dst` (same
+// layout), on one stream: the chunk body of fhe_b200_galois and of every level of fhe_b200_expand.
+void galois_range(const fhe_b200_params* par, const LevelData& lv, const int* perm, const fhe_b200_ksk* gk,
+                  const u64* src, u64* dst, u32 n, cudaStream_t st) {
+  const size_t row = (size_t)1 << par->logn, L = lv.L;
+  Workspace ws(par, st);
+  u64* s = ws.words((size_t)n * 2 * L * row);
+  u64* c2 = ws.words((size_t)n * L * row);
+  // galois_key.rs:66: substitute both parts; part 1 becomes the key-switch input
+  launch_gather(src, s, (size_t)n * 2 * L, perm, par->logn, st);
+  FHE_CUDA(cudaMemcpy2DAsync(c2, L * row * 8, s + L * row, 2 * L * row * 8, L * row * 8, n, cudaMemcpyDeviceToDevice, st));
+  launch_ntt(c2, c2, n * (u32)L, lv.ctx_ids, par->d_limbs, par->logn, true, 1, false, st);
+  // galois_key.rs:67 + :78: out0 = key_switch0 + substitute(ct[0]); out1 = key_switch1
+  key_switch_apply(par, gk, c2, n, dst, 2, s, ws, st);
 }
 
 // extend -> tensor -> scale down of bfv/ops/mul.rs:192-206 for `cts` ciphertext pairs.
@@ -878,6 +939,23 @@ int fhe_b200_batch_copy(fhe_b200_batch* dst, const fhe_b200_batch* src, void* st
   FHE_CUDA(cudaMemcpyAsync(dst->d, src->d, src->words_per_ct() * src->count * sizeof(u64), cudaMemcpyDeviceToDevice,
                            (cudaStream_t)stream));
   dst->repr = src->repr;
+  API_END
+}
+int fhe_b200_batch_copy_range(fhe_b200_batch* dst, uint32_t dst_first, const fhe_b200_batch* src, uint32_t src_first,
+                              uint32_t src_stride, uint32_t n, void* stream) {
+  API_BEGIN
+  REQUIRE(dst && src && dst != src, FHE_B200_INVALID_ARGUMENT, "null or aliased argument");
+  check_same(dst, src);
+  REQUIRE(dst->parts == src->parts, FHE_B200_BAD_POLY_COUNT, "shapes differ");
+  REQUIRE(dst->repr == src->repr, FHE_B200_INVALID_REPRESENTATION, "IncorrectRepresentation");
+  REQUIRE(n > 0 && src_stride > 0, FHE_B200_INVALID_ARGUMENT, "empty range or zero stride");
+  REQUIRE((uint64_t)dst_first + n <= dst->count &&
+              (uint64_t)src_first + (uint64_t)(n - 1) * src_stride < src->count,
+          FHE_B200_INVALID_ARGUMENT, "range exceeds batch");
+  DeviceGuard g(src->par);
+  const size_t w = src->words_per_ct() * sizeof(u64);
+  FHE_CUDA(cudaMemcpy2DAsync(dst->d + src->words_per_ct() * dst_first, w, src->d + src->words_per_ct() * src_first,
+                             w * src_stride, w, n, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   API_END
 }
 int fhe_b200_host_alloc(size_t bytes, int write_combined, void** out) {
@@ -1510,22 +1588,71 @@ int fhe_b200_galois(const fhe_b200_batch* ct, uint32_t exponent, const fhe_b200_
   REQUIRE(exponent & 1, FHE_B200_INVALID_EXPONENT, "InvalidSubstitutionExponent");
   DeviceGuard g(par);
   const LevelData& lv = par->level(ct->level);
-  const size_t row = (size_t)1 << par->logn, L = lv.L;
+  const size_t W = ct->words_per_ct();
   const int* perm = par->perm(exponent);
   ChunkRunner chunks(par, ct->count, (cudaStream_t)stream);
   chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
-    Workspace ws(par, st);
-    const u64* src = ct->d + (size_t)c0 * 2 * L * row;
-    u64* dst = out->d + (size_t)c0 * 2 * L * row;
-    u64* s = ws.words((size_t)n * 2 * L * row);
-    u64* c2 = ws.words((size_t)n * L * row);
-    // galois_key.rs:66: substitute both parts; part 1 becomes the key-switch input
-    launch_gather(src, s, (size_t)n * 2 * L, perm, par->logn, st);
-    FHE_CUDA(cudaMemcpy2DAsync(c2, L * row * 8, s + L * row, 2 * L * row * 8, L * row * 8, n, cudaMemcpyDeviceToDevice, st));
-    launch_ntt(c2, c2, n * (u32)L, lv.ctx_ids, par->d_limbs, par->logn, true, 1, false, st);
-    // galois_key.rs:67 + :78: out0 = key_switch0 + substitute(ct[0]); out1 = key_switch1
-    key_switch_apply(par, gk, c2, n, dst, 2, s, ws, st);
+    galois_range(par, lv, perm, gk, ct->d + c0 * W, out->d + c0 * W, n, st);
   });
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
+  API_END
+}
+
+int fhe_b200_expand(const fhe_b200_batch* ct, uint32_t size, const fhe_b200_ksk* const* gks, uint32_t n_gks,
+                    fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  REQUIRE(ct && out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = ct->par;
+  REQUIRE(size > 0 && size <= par->N, FHE_B200_INVALID_ARGUMENT,
+          "InvalidExpansionSize: " + std::to_string(size) + " for degree " + std::to_string(par->N));
+  REQUIRE(ct->parts == 2, FHE_B200_BAD_POLY_COUNT, "InvalidPolynomialCount: expected 2");
+  REQUIRE(!ct->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
+  need_repr(ct, FHE_B200_NTT);
+  const u32 Q = ct->count;
+  REQUIRE(out != ct && out->d != ct->d, FHE_B200_INVALID_ARGUMENT, "out must not alias ct");
+  REQUIRE(out->par == par && !out->mul_basis && out->level == ct->level && out->parts == 2 &&
+              (uint64_t)out->count == (uint64_t)size * Q,
+          FHE_B200_INVALID_ARGUMENT, "out must hold size * ct.count 2-part ciphertexts at ct's level");
+  // level = ceil(log2 size) (evaluation_key.rs:212); the key of level l is for element (N >> l) + 1 (:222-228)
+  u32 level = 0;
+  while ((1u << level) < size) level++;
+  REQUIRE(n_gks >= level && (level == 0 || gks), FHE_B200_INVALID_ARGUMENT,
+          "EvaluationKeyError: Missing GaloisKey: expansion level " + std::to_string(level) + " needs that many keys");
+  for (u32 l = 0; l < level; l++) {
+    REQUIRE(gks[l], FHE_B200_INVALID_ARGUMENT,
+            "EvaluationKeyError: Missing GaloisKey { element: " + std::to_string((par->N >> l) + 1) + " }");
+    check_ksk(gks[l], par, ct->level);
+  }
+  DeviceGuard g(par);
+  cudaStream_t user = (cudaStream_t)stream;
+  const LevelData& lv = par->level(ct->level);
+  const size_t W = ct->words_per_ct();
+  // tables first: building one allocates and uploads synchronously, which must not happen between enqueued levels
+  std::vector<const int*> perms(level);
+  std::vector<const ulonglong2*> monos(level);
+  for (u32 l = 0; l < level; l++) {
+    perms[l] = par->perm((par->N >> l) + 1);
+    monos[l] = par->expansion_monomial_dev(ct->level, l);
+  }
+  // index-major order: entry i*Q + q of `out` is output i of query q, so the outputs 0 .. step-1 of every query are
+  // the contiguous region [0, step*Q) and the ones a level adds, step .. 2*step-1, the region right after it
+  FHE_CUDA(cudaMemcpyAsync(out->d, ct->d, W * Q * sizeof(u64), cudaMemcpyDeviceToDevice, user));
+  // at a partial last level the Galois images of outputs i >= size - step have no slot in `out`: they only feed lo
+  Workspace spill_ws(par, user);
+  const u32 last_step = level ? 1u << (level - 1) : 0;
+  u64* spill = level && 2 * last_step > size ? spill_ws.words((size_t)(2 * last_step - size) * Q * W) : nullptr;
+  for (u32 l = 0; l < level; l++) {
+    const u32 step = 1u << l, pairs = step * Q, n_hi = (std::min(2 * step, size) - step) * Q;
+    u64* hi = out->d + (size_t)pairs * W;
+    ChunkRunner chunks(par, pairs, user);
+    chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+      const u32 e = c0 + n, mid = std::min(std::max(c0, n_hi), e);
+      if (mid > c0) galois_range(par, lv, perms[l], gks[l], out->d + c0 * W, hi + c0 * W, mid - c0, st);
+      if (e > mid) galois_range(par, lv, perms[l], gks[l], out->d + mid * W, spill + (mid - n_hi) * W, e - mid, st);
+    });
+    launch_expand_butterfly(out->d, hi, spill, pairs, n_hi, monos[l], lv.ctx_ids, par->d_limbs, par->logn, user);
+  }
   FHE_CUDA(cudaGetLastError());
   out->repr = FHE_B200_NTT;
   API_END
@@ -1750,6 +1877,15 @@ int fhe_b200_debug_ntt_tables(const fhe_b200_params* p, uint64_t q, uint64_t* om
   cp(zetas_inv, t.zi);
   cp(zetas_inv_shoup, t.zi_s);
   if (size_inv) *size_inv = t.ninv;
+  API_END
+}
+
+int fhe_b200_debug_expansion_monomial(const fhe_b200_params* p, uint32_t level, uint32_t l, uint64_t* out) {
+  API_BEGIN
+  REQUIRE(p && out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  REQUIRE(l < p->logn, FHE_B200_INVALID_ARGUMENT, "expansion level must be below log2 N");
+  const std::vector<u64> w = p->expansion_monomial(level, l);
+  std::copy(w.begin(), w.end(), out);
   API_END
 }
 

@@ -92,6 +92,12 @@ void launch_ew(EwOp op, u64* a, const u64* b, size_t n_rows, const RowIds& ids, 
 void launch_mul_plain(u64* a, const u64* pt, u32 cts, u32 parts, u32 n_pt, const RowIds& ids, const LimbDev* limbs,
                       u32 logn, cudaStream_t st, u32 op = 0);
 
+// one level of EvaluationKey::expands (evaluation_key.rs:229-241) over `pairs` 2-part ciphertexts, all NTT:
+// lo [pairs][2][L][N] += s;  hi [n_hi][2][L][N] = (lo - s) * mono (mono: [L][N] (value, Shoup) pairs).
+// s of pair k is hi[k] for k < n_hi (read, then overwritten) and spill[k - n_hi] otherwise.
+void launch_expand_butterfly(u64* lo, u64* hi, const u64* spill, u32 pairs, u32 n_hi, const ulonglong2* mono,
+                             const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st);
+
 // dot_product_scalar (bfv/ops/dot_product.rs:55-184): out[g] = sum_{i<n_terms} ct[(g*n+i) % ct_count] (.) pt[(g*n+i) % pt_count]
 // ct: [ct_count][parts][limbs][N], pt: [pt_count][limbs][N], out: [groups][parts][limbs][N], all NTT
 void launch_dot(const u64* ct, const u64* pt, u64* out, u32 groups, u32 n_terms, u32 parts, u32 ct_count,

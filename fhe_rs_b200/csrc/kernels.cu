@@ -75,6 +75,44 @@ __global__ void mul_plain_kernel(MulPlainArgs A) {
   }
 }
 
+// ------------------------------------------------------------------ oblivious expansion butterfly
+struct ExpandArgs {
+  u64* lo;              // [pairs][2][L][N], in place
+  u64* hi;              // [n_hi][2][L][N]: s of the first n_hi pairs, replaced by the monomial product
+  const u64* spill;     // [pairs - n_hi][2][L][N]: s of the pairs without a slot in `hi`
+  const ulonglong2* mono;   // [L][N] (value, Shoup companion)
+  size_t n_words, hi_words;
+  u32 logn, limbs_per_poly;
+  const LimbDev* limbs;
+  unsigned short ids[kMaxPos];
+};
+// One level of EvaluationKey::expands (evaluation_key.rs:229-241) for every (i, query) pair:
+// hi = (lo - s) * m_l, lo = lo + s.  Two 64-bit words per thread (128-bit accesses); s is read from hi (or the spill
+// buffer) before the same thread overwrites it.  All values canonical, so the result equals the reference's
+// sub / mul_shoup / add sequence bit for bit.
+__global__ void expand_butterfly_kernel(ExpandArgs A) {
+  const size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 2;
+  if (i >= A.n_words) return;
+  const u32 j = (u32)((i >> A.logn) % A.limbs_per_poly);
+  const u32 slot = (u32)i & ((1u << A.logn) - 1);
+  const u64 p = A.limbs[A.ids[j]].p;
+  const bool has_hi = i < A.hi_words;
+  const u64* sp = has_hi ? A.hi + i : A.spill + (i - A.hi_words);
+  const ulonglong2 s = *reinterpret_cast<const ulonglong2*>(sp);
+  ulonglong2 x = *reinterpret_cast<ulonglong2*>(A.lo + i);
+  if (has_hi) {
+    const ulonglong2 m0 = A.mono[((size_t)j << A.logn) + slot];
+    const ulonglong2 m1 = A.mono[((size_t)j << A.logn) + slot + 1];
+    ulonglong2 d;
+    d.x = mul_shoup(csub(x.x + p - s.x, p), m0.x, m0.y, p);
+    d.y = mul_shoup(csub(x.y + p - s.y, p), m1.x, m1.y, p);
+    *reinterpret_cast<ulonglong2*>(A.hi + i) = d;
+  }
+  x.x = csub(x.x + s.x, p);
+  x.y = csub(x.y + s.y, p);
+  *reinterpret_cast<ulonglong2*>(A.lo + i) = x;
+}
+
 // ------------------------------------------------------------------ dot_product_scalar
 struct DotArgs {
   const u64 *ct, *pt;
@@ -1094,6 +1132,21 @@ void launch_mul_plain(u64* a, const u64* pt, u32 cts, u32 parts, u32 n_pt, const
   size_t total = ((size_t)cts * parts * ids.limbs_per_poly) << logn;
   if (!total) return;
   mul_plain_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(A);
+  g_launches++;
+}
+
+void launch_expand_butterfly(u64* lo, u64* hi, const u64* spill, u32 pairs, u32 n_hi, const ulonglong2* mono,
+                             const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st) {
+  ExpandArgs A;
+  const size_t ct_words = ((size_t)2 * ids.limbs_per_poly) << logn;
+  A.lo = lo; A.hi = hi; A.spill = spill; A.mono = mono;
+  A.n_words = pairs * ct_words;
+  A.hi_words = n_hi * ct_words;
+  A.logn = logn; A.limbs_per_poly = ids.limbs_per_poly; A.limbs = limbs;
+  copy_ids(A.ids, ids);
+  if (!A.n_words) return;
+  const u32 threads = 256;
+  expand_butterfly_kernel<<<(unsigned)((A.n_words / 2 + threads - 1) / threads), threads, 0, st>>>(A);
   g_launches++;
 }
 

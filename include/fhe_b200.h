@@ -122,6 +122,11 @@ int fhe_b200_batch_download(const fhe_b200_batch* b, uint32_t first, uint32_t n,
 int fhe_b200_batch_download_async(const fhe_b200_batch* b, uint32_t first, uint32_t n, uint64_t* host, void* stream);
 /* Ciphertext::clone: dst <- src (same parameters, shape, level; representation is copied) */
 int fhe_b200_batch_copy(fhe_b200_batch* dst, const fhe_b200_batch* src, void* stream);
+/* dst[dst_first + k] = src[src_first + k*src_stride] for k < n: same parameters, parts, level and representation,
+ * dst != src, n > 0, src_stride > 0 (one cudaMemcpy2DAsync).  Splits or gathers the entries of a batch, e.g. the
+ * per-index batches of an fhe_b200_expand output. */
+int fhe_b200_batch_copy_range(fhe_b200_batch* dst, uint32_t dst_first, const fhe_b200_batch* src,
+                              uint32_t src_first, uint32_t src_stride, uint32_t n, void* stream);
 /* Page-locked host staging memory for asynchronous uploads / downloads (cudaHostAlloc, portable across devices).
  * write_combined != 0 asks for write-combining pages: faster for the device to read over PCIe and invisible to the
  * CPU caches, slow for the CPU to read -- meant for upload-only buffers the host fills once, front to back. */
@@ -231,6 +236,17 @@ int fhe_b200_multiplicator_multiply(const fhe_b200_multiplicator* m, const fhe_b
  * (column rotation by i <-> 3^i mod 2N, row swap <-> 2N-1; evaluation_key.rs:118, :278-286) */
 int fhe_b200_galois(const fhe_b200_batch* ct, uint32_t exponent, const fhe_b200_ksk* gk,
                     fhe_b200_batch* out, void* stream);
+/* EvaluationKey::expands (keys/evaluation_key.rs:192-256) of each of the Q = ct.count ciphertexts of `ct`
+ * (oblivious expansion, eprint 2019/1483).  out: size*Q ciphertexts, 2 parts, ct's level; entry i*Q + q is expansion
+ * output i of query q (for Q = 1 the reference's Vec order); out becomes NTT.  gks[l], l < ceil(log2 size), is the
+ * key-switching key of the GaloisKey for element (N >> l) + 1, for ct's level (its key level may be lower, as with
+ * EvaluationKeyBuilder::new_leveled); the caller vouches for the element, as for fhe_b200_galois.  The monomials
+ * -x^(N - 2^l) (:465-474) are fixed by the parameters and built by the library.  Each level is one batched Galois call
+ * over all step*Q inputs and one butterfly kernel; size == 1 is a copy.  Errors: size == 0 or size > N, n_gks too small,
+ * a NULL key -> INVALID_ARGUMENT; a key for another level or parameter set -> as fhe_b200_galois; ct.parts != 2 ->
+ * BAD_POLY_COUNT; power basis -> INVALID_REPRESENTATION; wrong out shape or out aliasing ct -> INVALID_ARGUMENT. */
+int fhe_b200_expand(const fhe_b200_batch* ct, uint32_t size, const fhe_b200_ksk* const* gks, uint32_t n_gks,
+                    fhe_b200_batch* out, void* stream);
 /* Poly::substitute on every row of a batch: the slot permutation of an NTT batch (rq/mod.rs:360-389) or the signed
  * coefficient permutation x^j -> x^(j*exponent) of a power-basis batch (rq/mod.rs:390-408); `out` takes `in`'s
  * representation.  Even exponents: FHE_B200_INVALID_EXPONENT. */
@@ -293,6 +309,9 @@ int fhe_b200_debug_scaler_tables(const fhe_b200_params* p, uint32_t level, int w
 /* NTT tables of prime q: any of omegas/zetas_inv (N words each) may be NULL. */
 int fhe_b200_debug_ntt_tables(const fhe_b200_params* p, uint64_t q, uint64_t* omegas, uint64_t* omegas_shoup,
                               uint64_t* zetas_inv, uint64_t* zetas_inv_shoup, uint64_t* size_inv);
+/* NTT words [limbs][N] at `level` of the expansion monomial -x^(N - 2^l), l < log2 N (evaluation_key.rs:465-474), as
+ * fhe_b200_expand uses them; works on host-only handles. */
+int fhe_b200_debug_expansion_monomial(const fhe_b200_params* p, uint32_t level, uint32_t l, uint64_t* out);
 /* Encoder tables: matrix_reps_index_map (N words), the NTT tables of t (N words each; NTT_UNAVAILABLE when t has none),
  * and for `level` q_mod_t (one word) and delta = (-t)^-1 mod q_i (one word per limb).  Any output may be NULL. */
 int fhe_b200_debug_encoder_tables(const fhe_b200_encoder* e, uint32_t level, uint32_t* index_map, uint64_t* omegas,

@@ -179,6 +179,12 @@ class Ciphertext {
     check(fhe_b200_batch_copy(c.h_, h_, stream_));
     return c;
   }
+  // a new batch of the n ciphertexts first, first + stride, ..., first + (n-1)*stride
+  Ciphertext take(uint32_t first, uint32_t n, uint32_t stride = 1) const {
+    Ciphertext c(par_, n, len(), level(), representation(), stream_);
+    check(fhe_b200_batch_copy_range(c.h_, 0, h_, first, stride, n, stream_));
+    return c;
+  }
   // bfv/ops/mod.rs:54, :148, :205
   Ciphertext& operator+=(const Ciphertext& rhs) { check(fhe_b200_add(h_, rhs.h_, stream_)); return *this; }
   Ciphertext& operator-=(const Ciphertext& rhs) { check(fhe_b200_sub(h_, rhs.h_, stream_)); return *this; }
@@ -403,13 +409,64 @@ class EvaluationKey {
   explicit EvaluationKey(std::shared_ptr<BfvParameters> par) : par_(std::move(par)) {}
   void add_galois_key(std::shared_ptr<GaloisKey> gk) { gk_[gk->exponent % (2 * (uint32_t)par_->degree())] = std::move(gk); }
   Ciphertext rotates_rows(const Ciphertext& ct) const { return at(2 * (uint32_t)par_->degree() - 1).relinearize(ct); }
-  Ciphertext rotates_columns_by(const Ciphertext& ct, uint32_t i) const {
-    uint64_t e = 1, m = 2 * par_->degree();
-    for (uint32_t k = 0; k < i; k++) e = e * 3 % m;  // evaluation_key.rs:278-286
-    return at((uint32_t)e).relinearize(ct);
+  Ciphertext rotates_columns_by(const Ciphertext& ct, uint32_t i) const { return at(column_exponent(i)).relinearize(ct); }
+  // evaluation_key.rs:40-53
+  bool supports_inner_sum() const {
+    const uint32_t n = (uint32_t)par_->degree();
+    bool ok = gk_.count(2 * n - 1) != 0;
+    for (uint32_t i = 1; i < n / 2; i *= 2) ok = ok && gk_.count(column_exponent(i)) != 0;
+    return ok;
+  }
+  // EvaluationKey::computes_inner_sum (evaluation_key.rs:56-100)
+  Ciphertext computes_inner_sum(const Ciphertext& ct) const {
+    if (!supports_inner_sum()) throw Error(FHE_B200_INVALID_ARGUMENT, "EvaluationKeyError: inner sum not supported by this key");
+    const uint32_t n = (uint32_t)par_->degree();
+    Ciphertext out = ct.clone();
+    for (uint32_t i = 1; i < n / 2; i *= 2) out += at(column_exponent(i)).relinearize(out);
+    out += at(2 * n - 1).relinearize(out);
+    return out;
+  }
+  // evaluation_key.rs:175-189
+  bool supports_expansion(uint32_t level) const {
+    const uint32_t n = (uint32_t)par_->degree();
+    if (level == 0) return true;
+    if ((1ull << level) > n) return false;
+    for (uint32_t l = 0; l < level; l++)
+      if (!gk_.count((n >> l) + 1)) return false;
+    return true;
+  }
+  // EvaluationKey::expands (evaluation_key.rs:192-256) of every ciphertext of `ct` (Q queries) as one batch of
+  // size * Q: entry i*Q + q is output i of query q (fhe_b200_expand)
+  Ciphertext expands_batch(const Ciphertext& ct, uint32_t size) const {
+    const uint32_t n = (uint32_t)par_->degree();
+    if (size == 0 || size > n) throw Error(FHE_B200_INVALID_ARGUMENT, "EvaluationKeyError: InvalidExpansionSize");
+    uint32_t level = 0;
+    while ((1u << level) < size) level++;
+    std::vector<const fhe_b200_ksk*> keys(level, nullptr);
+    for (uint32_t l = 0; l < level; l++) {
+      auto it = gk_.find((n >> l) + 1);
+      if (it != gk_.end()) keys[l] = it->second->ksk->handle();
+    }
+    Ciphertext out(ct.par(), size * ct.count(), 2, ct.level(), Representation::Ntt, ct.stream());
+    check(fhe_b200_expand(ct.handle(), size, keys.data(), level, out.handle(), ct.stream()));
+    return out;
+  }
+  // the reference's return shape: `size` batches of ct.count() ciphertexts, output i of every query
+  std::vector<Ciphertext> expands(const Ciphertext& ct, uint32_t size) const {
+    const Ciphertext whole = expands_batch(ct, size);
+    const uint32_t q = ct.count();
+    std::vector<Ciphertext> out;
+    out.reserve(size);
+    for (uint32_t i = 0; i < size; i++) out.push_back(whole.take(i * q, q));
+    return out;
   }
 
  private:
+  uint32_t column_exponent(uint32_t i) const {   // evaluation_key.rs:278-286
+    uint64_t e = 1, m = 2 * par_->degree();
+    for (uint32_t k = 0; k < i; k++) e = e * 3 % m;
+    return (uint32_t)e;
+  }
   const GaloisKey& at(uint32_t e) const {
     auto it = gk_.find(e);
     if (it == gk_.end()) throw Error(FHE_B200_INVALID_ARGUMENT, "EvaluationKeyError: rotation not supported by this key");
