@@ -62,6 +62,11 @@ SYMBOLS = {
     "fhe_b200_encode": (_i, [_vp, _i, _i, _vp, C.c_size_t, _vp, _vp]),
     "fhe_b200_mul_plain_batch": (_i, [_vp, _vp, _vp]),
     "fhe_b200_add_plain_batch": (_i, [_vp, _vp, _i, _vp]),
+    "fhe_b200_secret_key_create": (_i, [_vp, _vp, _pp]),
+    "fhe_b200_secret_key_free": (_i, [_vp]),
+    "fhe_b200_decrypt": (_i, [_vp, _vp, _vp, _vp]),
+    "fhe_b200_decode": (_i, [_vp, _i, _i, _vp, _vp, C.c_size_t, _vp]),
+    "fhe_b200_measure_noise": (_i, [_vp, _vp, _vp, _vp]),
     "fhe_b200_mul": (_i, [_vp, _vp, _vp, _vp]),
     "fhe_b200_relinearize": (_i, [_vp, _vp, _vp, _vp]),
     "fhe_b200_mul_relin": (_i, [_vp, _vp, _vp, _i, _vp, _vp]),

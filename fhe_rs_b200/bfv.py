@@ -22,7 +22,7 @@ from .wire import WireError
 
 __all__ = ["BfvParameters", "BfvParametersBuilder", "Ciphertext", "KeySwitchingKey", "RelinearizationKey", "RGSWCiphertext",
            "GaloisKey", "EvaluationKey", "Multiplicator", "ScalingFactor", "dot_product_scalar", "FheError", "WireError", "NTT", "POWER_BASIS",
-           "Encoding", "Plaintext", "PlaintextVec"]
+           "Encoding", "Plaintext", "PlaintextVec", "SecretKey"]
 
 
 def _release(free_name: str, handle) -> None:
@@ -566,6 +566,81 @@ class PlaintextVec:
     def poly_ntt(self) -> np.ndarray:
         """the poly_ntt words of every plaintext, [count][limbs][N]"""
         return self.batch.to_host()[:, 0]
+
+    def resolve_encoding(self, encoding: Optional[Encoding] = None) -> Encoding:
+        """Plaintext::resolve_encoding (plaintext.rs:137-153)"""
+        if self.encoding is None and encoding is None:
+            raise FheError(_capi.INVALID_ARGUMENT, "PlaintextError::MissingEncoding")
+        if self.encoding is not None and encoding is not None and self.encoding != encoding:
+            raise FheError(_capi.INVALID_ARGUMENT, "EncodingError::Mismatch: found %r, expected %r"
+                           % (encoding, self.encoding))
+        return self.encoding if self.encoding is not None else encoding
+
+    def try_decode(self, encoding: Optional[Encoding] = None, signed: bool = False, out=None):
+        """Vec<u64>::try_decode / Vec<i64>::try_decode (signed=True) (plaintext.rs:374-459) of every plaintext on the
+        device: values [count * N], plaintext k at [k*N, (k+1)*N).  `out` (optional): a contiguous numpy array or
+        torch tensor (host, pinned or CUDA) of count * N 64-bit words that receives them; otherwise a new numpy array
+        of uint64 (int64 when signed) is returned."""
+        enc = self.resolve_encoding(encoding)
+        n = self.batch.count * self.par.degree()
+        if out is None:
+            out = np.empty(n, np.int64 if signed else np.uint64)
+        if hasattr(out, "data_ptr") and hasattr(out, "is_cuda"):   # torch.Tensor
+            if out.element_size() != 8 or not out.is_contiguous() or out.numel() != n:
+                raise FheError(_capi.INVALID_ARGUMENT, "expected a contiguous 64-bit tensor of %d words" % n)
+            ptr = out.data_ptr()
+        else:
+            if out.dtype.itemsize != 8 or out.dtype.kind not in "iu" or not out.flags["C_CONTIGUOUS"] or out.size != n:
+                raise FheError(_capi.INVALID_ARGUMENT, "expected a contiguous 64-bit array of %d words" % n)
+            ptr = out.ctypes.data
+        st = self.batch.stream
+        check(_capi.lib().fhe_b200_decode(self.par.encoder(), enc.kind, 1 if signed else 0, self.batch._h, ptr, n, st))
+        check(_capi.lib().fhe_b200_sync(st))
+        return out
+
+
+class SecretKey:
+    """fhe::bfv::SecretKey (keys/secret_key.rs:25-53) on the device, from its N signed coefficients.  Decryption and
+    noise measurement run on the device; the device copy of s is erased when the key is released.  Key generation and
+    encryption stay with the client (their randomness cannot be reproduced here)."""
+
+    def __init__(self, par: BfvParameters, coeffs):
+        c = np.array(coeffs, dtype=np.int64)   # our own copy, kept for to_bytes (the reference keeps SecretKey.coeffs)
+        if c.ndim != 1 or c.size != par.degree():
+            raise FheError(_capi.INVALID_ARGUMENT, "a secret key has N = %d coefficients" % par.degree())
+        self._coeffs = c
+        h = C.c_void_p()
+        check(_capi.lib().fhe_b200_secret_key_create(par._h, _ptr(c), C.byref(h)))
+        self._h, self.par = h, par
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            _release("fhe_b200_secret_key_free", h)
+        c = getattr(self, "_coeffs", None)
+        if c is not None:
+            c[:] = 0
+
+    def to_bytes(self) -> bytes:   # secret_key.rs:142-148
+        return wire.encode_secret_key(self._coeffs.tolist())
+
+    @staticmethod
+    def from_bytes(par: BfvParameters, data: bytes) -> "SecretKey":   # secret_key.rs:151-175
+        return SecretKey(par, wire.decode_secret_key(data, par.degree()))
+
+    def try_decrypt(self, ct: Ciphertext) -> PlaintextVec:
+        """SecretKey::try_decrypt (secret_key.rs:198-260) of every ciphertext of the batch: plaintexts with no
+        encoding (decode them with try_decode(encoding))."""
+        out = Ciphertext(self.par, ct.count, 1, ct.level, NTT, ct.stream)
+        check(_capi.lib().fhe_b200_decrypt(self._h, ct._h, out._h, ct.stream))
+        return PlaintextVec(out, None)
+
+    def measure_noise(self, ct: Ciphertext) -> np.ndarray:
+        """SecretKey::measure_noise (secret_key.rs:55-98) of every ciphertext: uint32 [count]"""
+        out = np.zeros(ct.count, np.uint32)
+        check(_capi.lib().fhe_b200_measure_noise(self._h, ct._h, _ptr(out), ct.stream))
+        check(_capi.lib().fhe_b200_sync(ct.stream))
+        return out
 
 
 class Plaintext(PlaintextVec):

@@ -312,11 +312,37 @@ struct fhe_b200_encoder {
   std::vector<LimbDev> h_limbs;
   LimbDev* d_limbs = nullptr;
   u32* d_inv_map = nullptr;             // coefficient index -> slot
+  int* d_index_map = nullptr;           // index_map on the device (the decoders' gather)
   RowIds t_ids;                         // one row per plaintext, all modulo t
   std::vector<void*> d_allocs;
   template <typename T>
   T* to_dev(const std::vector<T>& v) {
     if (par->device < 0 || v.empty()) return nullptr;
+    T* d = nullptr;
+    FHE_CUDA(cudaMalloc(&d, v.size() * sizeof(T)));
+    d_allocs.push_back(d);
+    FHE_CUDA(cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+    return d;
+  }
+};
+
+// SecretKey (keys/secret_key.rs:25-53) on the device: s as NTT words modulo every modulus of the parameter set (the
+// context of level l is the prefix moduli[..L-l], so every level reads a prefix of the same rows), and per level the
+// tables decryption and noise measurement need.  The words of s are erased before they are freed.
+struct fhe_b200_secret_key {
+  const fhe_b200_params* par;
+  u64* s = nullptr;                     // [n_moduli][N]
+  struct Level {
+    ScalerData scaler;                  // cipher_plain_context.scaler: level basis -> plaintext context, t / Q_level
+    const u64* garner = nullptr;        // [L][L]: (i, j < i) = q_j^-1 mod q_i
+    const u64* q_words = nullptr;       // Q_level as little-endian 64-bit words
+    u32 W = 0;
+  };
+  std::vector<Level> levels;
+  std::vector<void*> d_allocs;
+  template <typename T>
+  T* to_dev(const std::vector<T>& v) {
+    if (v.empty()) return nullptr;
     T* d = nullptr;
     FHE_CUDA(cudaMalloc(&d, v.size() * sizeof(T)));
     d_allocs.push_back(d);
@@ -426,6 +452,7 @@ struct Workspace {
   cudaStream_t st;
   cudaMemPool_t pool;
   std::vector<void*> ptrs;
+  std::vector<std::pair<void*, size_t>> secret;
   Workspace(const fhe_b200_params* par, cudaStream_t s) : st(s), pool(par->pool) {}
   u64* words(size_t n) {
     void* p = nullptr;
@@ -433,7 +460,14 @@ struct Workspace {
     ptrs.push_back(p);
     return (u64*)p;
   }
+  // scratch that will hold values derived from a secret key: zeroed on the stream before it goes back to the pool
+  u64* secret_words(size_t n) {
+    u64* p = words(n);
+    secret.emplace_back(p, n * sizeof(u64));
+    return p;
+  }
   ~Workspace() {
+    for (auto& s : secret) cudaMemsetAsync(s.first, 0, s.second, st);
     for (void* p : ptrs) cudaFreeAsync(p, st);
   }
 };
@@ -1157,6 +1191,7 @@ int fhe_b200_encoder_create(const fhe_b200_params* p, const uint64_t* psi_t, fhe
   }
   e->d_limbs = e->to_dev(e->h_limbs);
   e->d_inv_map = e->to_dev(inv);
+  e->d_index_map = e->to_dev(std::vector<int>(e->index_map.begin(), e->index_map.end()));
   params_retain(p);
   cleanup.e = nullptr;
   *out = e.release();
@@ -1243,6 +1278,26 @@ int fhe_b200_mul_plain_batch(fhe_b200_batch* a, const fhe_b200_batch* pts, void*
   API_END
 }
 
+// RowIds of a single row modulo q_0
+static RowIds q0_row_ids() {
+  RowIds ids;
+  std::memset(&ids, 0, sizeof(RowIds));
+  ids.limbs_per_poly = 1;
+  return ids;
+}
+
+// Plaintext::to_poly (plaintext.rs:172-197) up to the delta product, from the plaintexts' coefficients (t < q_0):
+// x [n][N] power-basis words, in place ((x mod t) * q_mod_t) mod t, then lifted to every limb of the level and
+// transformed into m [n][L][N]
+static void to_poly_from_coefficients(const fhe_b200_params* par, const LevelData& lv, u64* x, u32 n, u64* m,
+                                      cudaStream_t st) {
+  u64 qmin = ~0ull;
+  for (u32 j = 0; j < lv.L; j++) qmin = std::min(qmin, par->moduli[j]);
+  const bool reduce = par->t_mod.t > 4 * qmin - 1;
+  launch_to_poly_load(x, (size_t)n << par->logn, par->t_mod, lv.q_mod_t, st);
+  launch_ntt(x, m, n * lv.L, lv.ctx_ids, par->d_limbs, par->logn, false, lv.L, reduce, st);
+}
+
 int fhe_b200_add_plain_batch(fhe_b200_batch* a, const fhe_b200_batch* pts, int subtract, void* stream) {
   API_BEGIN
   check_plain_batch(a, pts);
@@ -1253,19 +1308,13 @@ int fhe_b200_add_plain_batch(fhe_b200_batch* a, const fhe_b200_batch* pts, int s
   const LevelData& lv = par->level(a->level);
   const u32 L = lv.L, logn = par->logn;
   const size_t N = par->N;
-  u64 qmin = ~0ull;
-  for (u32 j = 0; j < L; j++) qmin = std::min(qmin, par->moduli[j]);
-  const bool reduce = par->t_mod.t > 4 * qmin - 1;
-  RowIds q0_ids;
-  std::memset(&q0_ids, 0, sizeof(RowIds));
-  q0_ids.limbs_per_poly = 1;
+  const RowIds q0_ids = q0_row_ids();
   // Plaintext::to_poly of plaintexts [p0, p0 + n) into m [n][L][N] (before the delta product)
   auto to_poly = [&](u32 p0, u32 n, u64* m, Workspace& ws, cudaStream_t st) {
     u64* x = ws.words((size_t)n * N);
     FHE_CUDA(cudaMemcpy2DAsync(x, N * 8, pts->d + (size_t)p0 * L * N, L * N * 8, N * 8, n, cudaMemcpyDeviceToDevice, st));
     launch_ntt(x, x, n, q0_ids, par->d_limbs, logn, true, 1, false, st);      // limb 0 of into_power_basis
-    launch_to_poly_load(x, (size_t)n * N, par->t_mod, lv.q_mod_t, st);
-    launch_ntt(x, m, n * L, lv.ctx_ids, par->d_limbs, logn, false, L, reduce, st);
+    to_poly_from_coefficients(par, lv, x, n, m, st);
   };
   cudaStream_t user = (cudaStream_t)stream;
   Workspace shared_ws(par, user);
@@ -1286,6 +1335,235 @@ int fhe_b200_add_plain_batch(fhe_b200_batch* a, const fhe_b200_batch* pts, int s
     }
     launch_add_scaled(a->d + (size_t)c0 * a->parts * L * N, m, n, a->parts, shared ? 1 : n, lv.d_delta, lv.d_delta_s,
                       subtract != 0, lv.ctx_ids, par->d_limbs, logn, st);
+  });
+  FHE_CUDA(cudaGetLastError());
+  API_END
+}
+
+// ---- decryption, decoding and noise measurement
+int fhe_b200_secret_key_create(const fhe_b200_params* p, const int64_t* coeffs, fhe_b200_secret_key** out) {
+  API_BEGIN
+  REQUIRE(p && coeffs && out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  REQUIRE(p->t_small, FHE_B200_UNSUPPORTED, "the plaintext modulus does not fit a u64 Modulus");
+  DeviceGuard g(p);
+  std::unique_ptr<fhe_b200_secret_key> sk(new fhe_b200_secret_key());
+  struct Cleanup {   // frees the device tables (and erases s) if construction throws
+    fhe_b200_secret_key* k;
+    size_t s_bytes;
+    ~Cleanup() {
+      if (!k) return;
+      if (k->s) cudaMemset(k->s, 0, s_bytes);
+      for (void* d : k->d_allocs) cudaFree(d);
+      cudaGetLastError();
+    }
+  } cleanup{sk.get(), ((size_t)p->Lmax * p->N) * sizeof(u64)};
+  sk->par = p;
+  const u32 N = p->N, Lmax = p->Lmax;
+  // Poly::try_convert_from(&[i64], ctx, false) (rq/convert.rs:194-230): the canonical residue of every signed word
+  std::vector<u64> res((size_t)Lmax * N);
+  for (u32 j = 0; j < Lmax; j++) {
+    const u64 q = p->moduli[j];
+    for (u32 i = 0; i < N; i++) {
+      const u64 w = (u64)coeffs[i], mag = coeffs[i] < 0 ? 0 - w : w, r = mag % q;
+      res[(size_t)j * N + i] = (coeffs[i] < 0 && r) ? q - r : r;
+    }
+  }
+  sk->s = sk->to_dev(res);
+  volatile u64* wipe = res.data();   // erase the host copy (volatile: the stores are not elided)
+  for (size_t i = 0; i < res.size(); i++) wipe[i] = 0;
+  const LevelData& l0 = p->level(0);
+  launch_ntt(sk->s, sk->s, Lmax, l0.ctx_ids, p->d_limbs, p->logn, false, 1, false, nullptr);   // into_ntt
+  FHE_CUDA(cudaGetLastError());
+  FHE_CUDA(cudaStreamSynchronize(nullptr));
+  // the plaintext context: the first moduli whose sizes add up to bits(t) + 60 (parameters.rs:579-595)
+  const size_t t_bits = p->t.bits();
+  u32 pc = 0, acc = 0;
+  for (u32 sz : p->moduli_sizes) {
+    acc += sz;
+    pc++;
+    if (acc >= t_bits + 60) break;
+  }
+  pc = std::min(std::max(pc, 1u), Lmax);
+  const std::vector<u64> plain(p->moduli.begin(), p->moduli.begin() + pc);
+  const RnsContextH to(plain);
+  sk->levels.resize(Lmax);
+  for (u32 lv = 0; lv < Lmax; lv++) {
+    const u32 L = Lmax - lv;
+    const std::vector<u64> ctx(p->moduli.begin(), p->moduli.begin() + L);
+    const RnsContextH from(ctx);
+    fhe_b200_secret_key::Level& d = sk->levels[lv];
+    d.scaler.h = make_scaler_tables(from, to, p->t, from.product);   // parameters.rs:638-643
+    upload_scaler_tables(d.scaler, plain, [&](const auto& v) { return sk->to_dev(v); },
+                         [&](u64 q) { return p->prime_index(q); });
+    std::vector<u64> garner((size_t)L * L, 0);
+    for (u32 i = 0; i < L; i++)
+      for (u32 j = 0; j < i; j++)
+        if (!invmod_h(ctx[j] % ctx[i], ctx[i], &garner[(size_t)i * L + j]))
+          throw FheError(FHE_B200_INVALID_MODULUS, "NonCoprimeModuli");
+    d.garner = sk->to_dev(garner);
+    std::vector<u64> qw;
+    const BigUint& Q = from.product;
+    for (size_t k = 0; k < Q.w.size(); k += 2)
+      qw.push_back((u64)Q.w[k] | (k + 1 < Q.w.size() ? (u64)Q.w[k + 1] << 32 : 0));
+    d.W = (u32)qw.size();
+    d.q_words = sk->to_dev(qw);
+  }
+  params_retain(p);
+  cleanup.k = nullptr;
+  *out = sk.release();
+  API_END
+}
+
+int fhe_b200_secret_key_free(fhe_b200_secret_key* sk) {
+  if (!sk) return FHE_B200_OK;
+  {
+    ScopedDevice g(sk->par->device);
+    // SecretKey's Zeroize (secret_key.rs:28-40): erase the words of s before the memory is released.  Work that reads
+    // s may still be queued on streams that do not order against the legacy stream the memset runs on (the chunk
+    // runner's side streams, a caller's non-blocking stream): wait for the device first, as cudaFree would, so that
+    // releasing the key right after an enqueue-only call is as safe as releasing any other handle.
+    cudaDeviceSynchronize();
+    if (sk->s) cudaMemset(sk->s, 0, ((size_t)sk->par->Lmax * sk->par->N) * sizeof(u64));
+    cudaDeviceSynchronize();
+    for (void* d : sk->d_allocs) cudaFree(d);
+    cudaGetLastError();
+  }
+  params_release(sk->par);
+  delete sk;
+  return FHE_B200_OK;
+}
+
+// the checks shared by decrypt and measure_noise
+static void check_secret_input(const fhe_b200_secret_key* sk, const fhe_b200_batch* ct) {
+  REQUIRE(sk && ct, FHE_B200_INVALID_ARGUMENT, "null argument");
+  REQUIRE(ct->par == sk->par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch");
+  REQUIRE(!ct->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
+  need_repr(ct, FHE_B200_NTT);
+}
+
+// try_decrypt (secret_key.rs:198-260) of ciphertexts [c0, c0 + n) of ct up to the scaled phase: w [n][N] receives
+// ((v + t) mod q_0) mod t, v = row 0 of phase.scale(cipher_plain_context.scaler).  When ph_ntt is not null it receives
+// the NTT-domain phase [n][L][N] (which measure_noise reuses); otherwise the phase is transformed in place in scratch.
+static void decrypt_range(const fhe_b200_secret_key* sk, const fhe_b200_batch* ct, u32 c0, u32 n, u64* w, u64* ph_ntt,
+                          Workspace& ws, cudaStream_t st) {
+  const fhe_b200_params* par = sk->par;
+  const LevelData& lv = par->level(ct->level);
+  const u32 L = lv.L, logn = par->logn;
+  const size_t rows = (size_t)n * L;
+  u64* ph = ph_ntt ? ph_ntt : ws.secret_words(rows << logn);
+  launch_phase(ct->d + (((size_t)c0 * ct->parts * L) << logn), sk->s, ph, n, ct->parts, lv.ctx_ids, par->d_limbs, logn,
+               st);
+  u64* pb = ph_ntt ? ws.secret_words(rows << logn) : ph;
+  launch_ntt(ph, pb, (u32)rows, lv.ctx_ids, par->d_limbs, logn, true, 1, false, st);
+  // only output row 0 (q_0): the reference keeps v[..degree], and every output limb of the scaler is independent
+  launch_scale(sk->levels[ct->level].scaler.dev, par->d_limbs, pb, w, nullptr, n, 1, 0, 1, 0, logn, st);
+  const LimbDev& q0 = par->h_limbs[0];
+  launch_decrypt_epilogue(w, (size_t)n << logn, PlainMod{q0.p, q0.bhi, q0.blo}, par->t_mod, st);
+}
+
+int fhe_b200_decrypt(const fhe_b200_secret_key* sk, const fhe_b200_batch* ct, fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  check_secret_input(sk, ct);
+  REQUIRE(out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  REQUIRE(out->par == sk->par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch");
+  REQUIRE(!out->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
+  REQUIRE(out->parts == 1 && out->count == ct->count && out->level == ct->level, FHE_B200_INVALID_ARGUMENT,
+          "out must be a 1-part batch of ct.count plaintexts at ct's level");
+  const fhe_b200_params* par = sk->par;
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(ct->level);
+  const u32 L = lv.L, logn = par->logn;
+  u64 qmin = ~0ull;
+  for (u32 j = 0; j < L; j++) qmin = std::min(qmin, par->moduli[j]);
+  const bool reduce = par->t_mod.t > 4 * qmin - 1;   // the lifted words are below t
+  ChunkRunner chunks(par, ct->count, (cudaStream_t)stream);
+  chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace ws(par, st);
+    u64* w = ws.secret_words((size_t)n << logn);
+    decrypt_range(sk, ct, c0, n, w, nullptr, ws, st);
+    // Poly::try_convert_from(w, ctx).into_ntt(): every limb of plaintext k transforms row k of w
+    launch_ntt(w, out->d + ((size_t)c0 * L << logn), n * L, lv.ctx_ids, par->d_limbs, logn, false, L, reduce, st);
+  });
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
+  API_END
+}
+
+int fhe_b200_measure_noise(const fhe_b200_secret_key* sk, const fhe_b200_batch* ct, uint32_t* noise_bits,
+                           void* stream) {
+  API_BEGIN
+  check_secret_input(sk, ct);
+  REQUIRE(noise_bits, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = sk->par;
+  REQUIRE(par->t_mod.t < par->moduli[0], FHE_B200_UNSUPPORTED, "to_poly needs t below the first ciphertext modulus");
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(ct->level);
+  const fhe_b200_secret_key::Level& kl = sk->levels[ct->level];
+  const u32 L = lv.L, logn = par->logn;
+  cudaStream_t user = (cudaStream_t)stream;
+  Workspace out_ws(par, user);   // the per-ciphertext maxima, filled by the chunks' atomics
+  u32* noise = (u32*)out_ws.words((ct->count + 1) / 2);
+  FHE_CUDA(cudaMemsetAsync(noise, 0, ct->count * sizeof(u32), user));
+  {
+    ChunkRunner chunks(par, ct->count, user);
+    chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+      Workspace ws(par, st);
+      const size_t words = ((size_t)n * L) << logn;
+      u64* ph = ws.secret_words(words);
+      u64* w = ws.secret_words((size_t)n << logn);
+      decrypt_range(sk, ct, c0, n, w, ph, ws, st);
+      // phase - to_poly(decrypt(ct)), back to the power basis (secret_key.rs:61-84)
+      u64* m = ws.secret_words(words);
+      to_poly_from_coefficients(par, lv, w, n, m, st);
+      launch_add_scaled(ph, m, n, 1, n, lv.d_delta, lv.d_delta_s, true, lv.ctx_ids, par->d_limbs, logn, st);
+      launch_ntt(ph, ph, n * L, lv.ctx_ids, par->d_limbs, logn, true, 1, false, st);
+      launch_noise(ph, noise + c0, n, L, kl.garner, kl.q_words, kl.W, par->d_limbs, logn, st);
+    });
+  }
+  FHE_CUDA(cudaMemcpyAsync(noise_bits, noise, ct->count * sizeof(u32), cudaMemcpyDefault, user));
+  FHE_CUDA(cudaGetLastError());
+  API_END
+}
+
+int fhe_b200_decode(const fhe_b200_encoder* e, int encoding, int is_signed, const fhe_b200_batch* pts, void* values,
+                    size_t n_values, void* stream) {
+  API_BEGIN
+  REQUIRE(e, FHE_B200_INVALID_ARGUMENT, "null encoder");
+  const fhe_b200_params* par = e->par;
+  REQUIRE(encoding == FHE_B200_ENCODING_POLY || encoding == FHE_B200_ENCODING_SIMD, FHE_B200_INVALID_ARGUMENT,
+          "unknown encoding");
+  // Plaintext::coefficients (plaintext.rs:103-135): with t >= q_0 the reference lifts every limb
+  REQUIRE(par->t_small && par->t_mod.t < par->moduli[0], FHE_B200_UNSUPPORTED,
+          "decoding needs t below the first ciphertext modulus");
+  DeviceGuard g(par);
+  const bool simd = encoding == FHE_B200_ENCODING_SIMD;
+  REQUIRE(!simd || e->has_ntt, FHE_B200_NTT_UNAVAILABLE, "EncodingError::SimdUnavailable");   // plaintext.rs:155-160
+  REQUIRE(pts, FHE_B200_INVALID_ARGUMENT, "null argument");
+  REQUIRE(pts->par == par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch");
+  REQUIRE(!pts->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
+  REQUIRE(pts->parts == 1, FHE_B200_BAD_POLY_COUNT, "a plaintext batch has one polynomial per entry");
+  need_repr(pts, FHE_B200_NTT);
+  const size_t N = par->N;
+  REQUIRE(values && n_values == (size_t)pts->count * N, FHE_B200_INVALID_ARGUMENT,
+          "values must hold pts.count * N words");
+  const u32 L = pts->limbs, logn = par->logn;
+  const RowIds q0_ids = q0_row_ids();
+  char* dst = (char*)values;
+  ChunkRunner chunks(par, pts->count, (cudaStream_t)stream);
+  chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace ws(par, st);
+    u64* x = ws.words((size_t)n * N);
+    FHE_CUDA(cudaMemcpy2DAsync(x, N * 8, pts->d + (size_t)c0 * L * N, L * N * 8, N * 8, n, cudaMemcpyDeviceToDevice, st));
+    launch_ntt(x, x, n, q0_ids, par->d_limbs, logn, true, 1, false, st);      // limb 0 of into_power_basis
+    launch_to_poly_load(x, (size_t)n * N, par->t_mod, 1, st);                 // reduce_vec mod t
+    if (simd) {   // decode_simd_u64 (plaintext.rs:155-170): NttOperator::forward mod t, then the slot gather
+      launch_ntt(x, x, n, e->t_ids, e->d_limbs, logn, false, 1, false, st);
+      u64* y = ws.words((size_t)n * N);
+      launch_gather(x, y, n, e->d_index_map, logn, st);
+      x = y;
+    }
+    if (is_signed) launch_center(x, (size_t)n * N, par->t_mod.t, st);       // center_vec (plaintext.rs:440-446)
+    FHE_CUDA(cudaMemcpyAsync(dst + (size_t)c0 * N * 8, x, (size_t)n * N * 8, cudaMemcpyDefault, st));
   });
   FHE_CUDA(cudaGetLastError());
   API_END

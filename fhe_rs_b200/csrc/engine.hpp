@@ -193,6 +193,20 @@ void launch_to_poly_load(u64* x, size_t n_words, const PlainMod& T, u64 q_mod_t,
 void launch_add_scaled(u64* a, const u64* m, u32 cts, u32 parts, u32 n_pt, const u64* delta, const u64* delta_s,
                        bool subtract, const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st);
 
+// ---- decryption (keys/secret_key.rs:55-98, :198-260)
+// out [cts][L][N] = c0 + c1*s + c2*s^2 + ... of ct [cts][parts][L][N] (NTT, canonical); s row j at s + j*N
+void launch_phase(const u64* ct, const u64* s, u64* out, u32 cts, u32 parts, const RowIds& ids, const LimbDev* limbs,
+                  u32 logn, cudaStream_t st);
+// in place: v <- ((v + t) mod q_0) mod t   (Q0 = {q_0, Barrett constants})
+void launch_decrypt_epilogue(u64* v, size_t n_words, const PlainMod& Q0, const PlainMod& T, cudaStream_t st);
+// in place: Modulus::center, a - t when a >= t >> 1 (the words are read back as i64)
+void launch_center(u64* x, size_t n_words, u64 t, cudaStream_t st);
+// out[ct] = max(out[ct], max over the N coefficients of min(bits(x), bits(Q - x))), x the CRT lift of the L residues of
+// x [cts][L][N] (power basis, canonical; limb j modulo limbs[j]).  garner [L][L]: (i, j < i) = q_j^-1 mod q_i;
+// q_words: Q as W little-endian words.  L <= 32.
+void launch_noise(const u64* x, u32* out, u32 cts, u32 L, const u64* garner, const u64* q_words, u32 W,
+                  const LimbDev* limbs, u32 logn, cudaStream_t st);
+
 // bit (un)packing of power-basis rows (fhe-util/src/lib.rs:71-146): row r of `rows` uses nbits[r % limbs] bits per
 // coefficient; packed row r starts at byte  (r / limbs) * poly_bytes + offs[r % limbs]
 struct PackDev {

@@ -1069,6 +1069,113 @@ __global__ void add_scaled_kernel(AddScaledArgs A) {
   *dst = A.subtract ? csub(x + p - w, p) : csub(x + w, p);
 }
 
+// ------------------------------------------------------------------ decryption (keys/secret_key.rs:55-98, :198-260)
+struct PhaseArgs {
+  const u64* ct;   // [cts][parts][L][N]
+  const u64* s;    // row j: s modulo the j-th limb
+  u64* out;        // [cts][L][N]
+  u32 cts, parts, logn, limbs_per_poly;
+  const LimbDev* limbs;
+  unsigned short ids[kMaxPos];
+};
+// c0 + c1 s + c2 s^2 + ... as a Horner sum, one coefficient per thread.  Every product and sum is reduced to the
+// canonical residue (the reference's sum of canonical terms gives the same word).  No branch depends on the data.
+__global__ void phase_kernel(PhaseArgs A) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t total = ((size_t)A.cts * A.limbs_per_poly) << A.logn;
+  if (idx >= total) return;
+  const u32 c = (u32)idx & ((1u << A.logn) - 1);
+  const size_t row = idx >> A.logn;
+  const u32 j = (u32)(row % A.limbs_per_poly), ct = (u32)(row / A.limbs_per_poly);
+  const LimbDev& M = A.limbs[A.ids[j]];
+  const u64 s = A.s[((size_t)j << A.logn) + c];
+  const size_t stride = (size_t)A.limbs_per_poly << A.logn;
+  const u64* src = A.ct + (size_t)ct * A.parts * stride + ((size_t)j << A.logn) + c;
+  u64 acc = src[(size_t)(A.parts - 1) * stride];
+  for (int p = (int)A.parts - 2; p >= 0; p--) acc = csub(mulmod_limb(acc, s, M) + src[(size_t)p * stride], M.p);
+  A.out[idx] = acc;
+}
+
+// w = ((v + t) mod q_0) mod t on row 0 of the scaled phase (secret_key.rs:228-236): two Barrett reductions, no branch
+__global__ void decrypt_epilogue_kernel(u64* v, size_t n_words, PlainMod Q0, PlainMod T) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_words) return;
+  v[i] = barrett64(barrett64(v[i] + T.t, Q0.t, Q0.bhi, Q0.blo), T.t, T.bhi, T.blo);
+}
+
+// Modulus::center (zq/mod.rs:448-457): a - t when a >= t >> 1, else a, as a select
+__global__ void center_kernel(u64* x, size_t n_words, u64 t) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_words) return;
+  const u64 a = x[i];
+  x[i] = a >= (t >> 1) ? a - t : a;
+}
+
+struct NoiseArgs {
+  const u64* x;         // [cts][L][N] power basis, canonical
+  u32* out;             // [cts]
+  const u64* garner;    // [L][L]: entry (i, j), j < i, is q_j^-1 mod q_i
+  const u64* q_words;   // Q, W little-endian 64-bit words
+  u32 L, W, logn;
+  const LimbDev* limbs;   // limb j of the context is limbs[j]
+};
+// the bit length of a W-word integer
+__device__ __forceinline__ u32 bits_of(const u64* a, u32 W) {
+  for (int w = (int)W - 1; w >= 0; w--)
+    if (a[w]) return 64u * (u32)w + 64u - (u32)__clzll((long long)a[w]);
+  return 0;
+}
+// measure_noise's per-coefficient term min(bits(x), bits(Q - x)) (secret_key.rs:85-95) for the CRT lift x in [0, Q):
+// Garner's mixed-radix digits y_i (x = y_0 + y_1 q_0 + y_2 q_0 q_1 + ...), then a Horner sum into W words.  Exact for
+// every x.  The maximum over a block goes to out[ct] with one atomic.  Variable time, as the reference's unsafe fn.
+__global__ void __launch_bounds__(256) noise_kernel(NoiseArgs A) {
+  constexpr int kMax = 32;   // limbs of a context (parameter sets have fewer than 32 moduli)
+  const u32 N = 1u << A.logn, ct = blockIdx.y;
+  const u32 c = blockIdx.x * blockDim.x + threadIdx.x;
+  u32 noise = 0;
+  if (c < N) {
+    const u64* src = A.x + (((size_t)ct * A.L) << A.logn) + c;
+    u64 y[kMax], X[kMax];
+    for (u32 i = 0; i < A.L; i++) {
+      const LimbDev& M = A.limbs[i];
+      u64 r = src[(size_t)i << A.logn];
+      for (u32 j = 0; j < i; j++) {
+        const u64 yj = barrett64(y[j], M.p, M.bhi, M.blo);
+        r = mulmod_limb(csub(r + M.p - yj, M.p), A.garner[(size_t)i * A.L + j], M);
+      }
+      y[i] = r;
+    }
+    for (u32 w = 0; w < A.W; w++) X[w] = 0;
+    for (int i = (int)A.L - 1; i >= 0; i--) {   // X = X * q_i + y_i
+      u64 carry = y[i];
+      const u64 q = A.limbs[i].p;
+      for (u32 w = 0; w < A.W; w++) {
+        const unsigned __int128 p = (unsigned __int128)X[w] * q + carry;
+        X[w] = (u64)p;
+        carry = (u64)(p >> 64);
+      }
+    }
+    const u32 bx = bits_of(X, A.W);
+    u64 borrow = 0;
+    for (u32 w = 0; w < A.W; w++) {   // X <- Q - X
+      const u64 a = A.q_words[w], b = X[w];
+      const u64 d = a - b - borrow;
+      borrow = (a < b) || (a - b < borrow);
+      X[w] = d;
+    }
+    noise = min(bx, bits_of(X, A.W));
+  }
+  noise = __reduce_max_sync(0xffffffffu, noise);
+  __shared__ u32 s_max[8];
+  if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = noise;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    u32 m = 0;
+    for (u32 w = 0; w < (blockDim.x + 31) / 32; w++) m = max(m, s_max[w]);
+    atomicMax(A.out + ct, m);
+  }
+}
+
 void copy_ids(unsigned short* dst, const RowIds& ids) {
   for (int i = 0; i < kMaxPos; i++) dst[i] = ids.ids[i];
 }
@@ -1101,6 +1208,40 @@ void launch_add_scaled(u64* a, const u64* m, u32 cts, u32 parts, u32 n_pt, const
   const size_t total = ((size_t)cts * ids.limbs_per_poly) << logn;
   if (!total) return;
   add_scaled_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(A);
+  g_launches++;
+}
+
+void launch_phase(const u64* ct, const u64* s, u64* out, u32 cts, u32 parts, const RowIds& ids, const LimbDev* limbs,
+                  u32 logn, cudaStream_t st) {
+  PhaseArgs A;
+  A.ct = ct; A.s = s; A.out = out; A.cts = cts; A.parts = parts; A.logn = logn;
+  A.limbs_per_poly = ids.limbs_per_poly; A.limbs = limbs;
+  copy_ids(A.ids, ids);
+  const size_t total = ((size_t)cts * ids.limbs_per_poly) << logn;
+  if (!total || !parts) return;
+  phase_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(A);
+  g_launches++;
+}
+
+void launch_decrypt_epilogue(u64* v, size_t n_words, const PlainMod& Q0, const PlainMod& T, cudaStream_t st) {
+  if (!n_words) return;
+  decrypt_epilogue_kernel<<<(unsigned)((n_words + 255) / 256), 256, 0, st>>>(v, n_words, Q0, T);
+  g_launches++;
+}
+
+void launch_center(u64* x, size_t n_words, u64 t, cudaStream_t st) {
+  if (!n_words) return;
+  center_kernel<<<(unsigned)((n_words + 255) / 256), 256, 0, st>>>(x, n_words, t);
+  g_launches++;
+}
+
+void launch_noise(const u64* x, u32* out, u32 cts, u32 L, const u64* garner, const u64* q_words, u32 W,
+                  const LimbDev* limbs, u32 logn, cudaStream_t st) {
+  if (!cts) return;
+  NoiseArgs A;
+  A.x = x; A.out = out; A.garner = garner; A.q_words = q_words; A.L = L; A.W = W; A.logn = logn; A.limbs = limbs;
+  const u32 N = 1u << logn;
+  noise_kernel<<<dim3((N + 255) / 256, cts), 256, 0, st>>>(A);
   g_launches++;
 }
 

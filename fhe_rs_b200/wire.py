@@ -6,6 +6,7 @@ The reference serialises polynomials, ciphertexts and key-switching keys with pr
     fhers.bfv.Ciphertext         fhe/src/proto/bfv.proto:5-9         (bfv/ciphertext.rs:230-257)
     fhers.bfv.KeySwitchingKey    bfv.proto:16-23                     (keys/key_switching_key.rs:365-385)
     fhers.bfv.RelinearizationKey bfv.proto:25-27, GaloisKey :29-32, RGSWCiphertext :11-14
+    fhers.bfv.SecretKey          bfv.proto:54-56                     (keys/secret_key.rs:142-175)
 
 The heavy part of every one of them -- `Rq.coefficients`, the bit-packed power-basis words -- is produced and consumed
 on the device (fhe_b200_batch_pack / fhe_b200_batch_unpack).  This module is the few bytes around it: a hand-written
@@ -312,3 +313,56 @@ def decode_rgsw(data: Bytes) -> Tuple[memoryview, memoryview]:  # rgsw_ciphertex
     if f[2] is None:
         raise WireError("MissingField", detail="RgswKeySwitchingKey1")
     return f[1], f[2]
+
+
+# ------------------------------------------------------------------------------------------ SecretKey
+def _zigzag(n: int) -> int:
+    return ((n << 1) ^ (n >> 63)) & 0xFFFFFFFFFFFFFFFF
+
+
+def _unzigzag(n: int) -> int:
+    return (n >> 1) ^ -(n & 1)
+
+
+def encode_secret_key(coeffs: Sequence[int]) -> bytes:   # secret_key.rs:142-148, bfv.proto:54-56
+    """`repeated sint64 coeffs = 1`: one packed field of zig-zag varints (absent when there are no coefficients)"""
+    out: List[Bytes] = []
+    if len(coeffs):
+        _put_len(out, 1, b"".join(_varint(_zigzag(int(c))) for c in coeffs))
+    return _join(out)
+
+
+def decode_secret_key(data: Bytes, degree: int) -> List[int]:   # secret_key.rs:151-175
+    """the coefficients of a SecretKey message; packed and unpacked encodings are both accepted (as prost does).
+    A count other than `degree` is InvalidSecretKeyCoefficientCount."""
+    coeffs: List[int] = []
+    for field, wt, v in _fields(data):
+        if field != 1:
+            continue
+        if wt == _VARINT:
+            coeffs.append(_unzigzag(v))
+        elif wt == _LEN:
+            coeffs.extend(_unzigzag(x) for x in _packed_varints(v))
+        else:
+            raise WireError("Decode", detail="wire type %d for a sint64 field" % wt)
+    if len(coeffs) != degree:
+        raise WireError("InvalidSecretKeyCoefficientCount", detail="%d coefficients, expected %d" % (len(coeffs), degree))
+    return coeffs
+
+
+def _packed_varints(buf: memoryview) -> Iterator[int]:
+    pos, end = 0, len(buf)
+    while pos < end:
+        shift = value = 0
+        while True:
+            if pos >= end:
+                raise WireError("Decode", detail="truncated varint")
+            b = buf[pos]
+            pos += 1
+            if shift == 63 and b > 1:
+                raise WireError("Decode", detail="varint overflows 64 bits")
+            value |= (b & 0x7F) << shift
+            if not b & 0x80:
+                break
+            shift += 7
+        yield value

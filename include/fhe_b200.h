@@ -71,6 +71,7 @@ typedef struct fhe_b200_multiplicator fhe_b200_multiplicator; /* == Multiplicato
                                                    (bfv/ops/mul.rs:22-98)                                        */
 typedef struct fhe_b200_encoder fhe_b200_encoder; /* == the plaintext side of BfvParameters: the NTT operator of t
                                                      and the SIMD slot map (parameters.rs:71-75, :713-726)      */
+typedef struct fhe_b200_secret_key fhe_b200_secret_key; /* == SecretKey (bfv/keys/secret_key.rs:25-53)               */
 
 /* Encoding (bfv/encoding.rs): the level comes from the output batch (Encoding::{poly,simd}_at_level). */
 typedef enum { FHE_B200_ENCODING_POLY = 0, FHE_B200_ENCODING_SIMD = 1 } fhe_b200_encoding;
@@ -203,6 +204,41 @@ int fhe_b200_mul_plain_batch(fhe_b200_batch* a, const fhe_b200_batch* pts, void*
 /* fhe_b200_add_plain with a device plaintext batch (ops/mod.rs:88-97, :188-197): Plaintext::to_poly is derived from
  * poly_ntt on the device as the reference does (plaintext.rs:103-135, :172-197).  t >= q_0 -> UNSUPPORTED. */
 int fhe_b200_add_plain_batch(fhe_b200_batch* a, const fhe_b200_batch* pts, int subtract, void* stream);
+
+/* ---- decryption, decoding and noise measurement ---------------------------------------------
+ * SecretKey (keys/secret_key.rs:25-53) from its N signed coefficients (SecretKey.coeffs, the `coeffs` of the bfv.proto
+ * SecretKey message, bfv.proto:54-56; a Rust host reads them from sk.to_bytes(), see INTEGRATION.md).  The key is
+ * uploaded once as NTT words modulo every modulus of the parameter set; it also holds, per level, the tables of the
+ * cipher -> plaintext scaler (cipher_plain_context.scaler, parameters.rs:638-643) and of the noise measurement.  It
+ * holds a reference on the parameter set.  fhe_b200_secret_key_free waits for the device (like every *_free, work
+ * still queued with the key may be in flight), then erases the device words of s before releasing them (SecretKey's
+ * Zeroize, secret_key.rs:28-40), and scratch holding s-dependent values is zeroed before it goes back
+ * to the pool.  The decryption kernels have no branch that depends on the data.  Errors: t beyond a u64 Modulus ->
+ * UNSUPPORTED (the large-t branch of try_decrypt is not implemented); host-only parameters -> NO_DEVICE. */
+int fhe_b200_secret_key_create(const fhe_b200_params* p, const int64_t* coeffs, fhe_b200_secret_key** out);
+int fhe_b200_secret_key_free(fhe_b200_secret_key* sk);
+/* SecretKey::try_decrypt (secret_key.rs:198-260) of every ciphertext of `ct` (NTT, any number of parts >= 1): out is
+ * a 1-part batch of ct.count entries at ct's level; entry k becomes Plaintext::poly_ntt of the decryption of ct[k]
+ * (encoding None), word for word, also when t >= q_0.  The phase c0 + c1 s + c2 s^2 + ... is taken to the power basis,
+ * scaled by t / Q into limb 0 of the plaintext context, and w = ((v + t) mod q_0) mod t is lifted and transformed.
+ * Errors: ct or out of another parameter set, or over the multiplication basis -> CONTEXT_MISMATCH; power-basis ct ->
+ * INVALID_REPRESENTATION; out not 1-part, ct.count entries at ct's level -> INVALID_ARGUMENT. */
+int fhe_b200_decrypt(const fhe_b200_secret_key* sk, const fhe_b200_batch* ct, fhe_b200_batch* out, void* stream);
+/* Vec<u64>::try_decode (is_signed == 0) / Vec<i64>::try_decode (is_signed != 0) (plaintext.rs:103-135, :155-170,
+ * :374-459) of every plaintext of pts, a 1-part NTT batch at any level: values receives pts.count * N words, plaintext
+ * k at values[k*N, (k+1)*N).  Signed words are centred as Modulus::center does (a - t when a >= t >> 1, zq/mod.rs:448-457).
+ * values: pageable host, pinned host or device memory; the copy is only enqueued (cudaMemcpyDefault), read it after
+ * fhe_b200_sync(stream).  The encoding is the caller's (a batch does not record it; resolve_encoding is host work).
+ * Errors: t beyond a u64 Modulus, or t >= q_0 (the reference then lifts every limb) -> UNSUPPORTED; SIMD without an
+ * NTT for t -> NTT_UNAVAILABLE; parts != 1 -> BAD_POLY_COUNT; power basis -> INVALID_REPRESENTATION; another parameter
+ * set -> CONTEXT_MISMATCH; n_values != pts.count * N or NULL values -> INVALID_ARGUMENT; host-only parameters -> NO_DEVICE. */
+int fhe_b200_decode(const fhe_b200_encoder* e, int encoding, int is_signed, const fhe_b200_batch* pts, void* values,
+                    size_t n_values, void* stream);
+/* SecretKey::measure_noise (secret_key.rs:55-98) of every ciphertext of ct: noise_bits[k] = max over the coefficients
+ * of min(bits(x), bits(Q - x)), x in [0, Q) the CRT lift of phase - to_poly(decrypt(ct[k])) at ct's level.  Exact
+ * for every x.  noise_bits: ct.count words in host or device memory, only enqueued as for fhe_b200_decode.  Variable
+ * time, as the reference's (unsafe) function.  Errors: as fhe_b200_decrypt; t >= q_0 -> UNSUPPORTED. */
+int fhe_b200_measure_noise(const fhe_b200_secret_key* sk, const fhe_b200_batch* ct, uint32_t* noise_bits, void* stream);
 
 /* &Ciphertext * &Ciphertext (bfv/ops/mod.rs:259-358): n parts x m parts -> n + m - 1 parts (out3 must have that many;
  * 2 x 2 -> 3 is the fused path) */

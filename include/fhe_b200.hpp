@@ -9,6 +9,7 @@
 //   bfv::GaloisKey / EvaluationKey              bfv/keys/galois_key.rs:18, evaluation_key.rs:110-170
 //   bfv::Multiplicator                          bfv/ops/mul.rs:22
 //   bfv::Encoding / Plaintext / PlaintextVec    bfv/encoding.rs, bfv/plaintext.rs:20, plaintext_vec.rs:20
+//   bfv::SecretKey (decryption, measure_noise)  bfv/keys/secret_key.rs:25 (key generation and encryption stay client-side)
 // Fallible reference calls return Result<_, fhe::Error>; here they throw fhe_b200::Error carrying
 // the fhe_b200_status code (same variants, see fhe_b200.h).
 #pragma once
@@ -19,6 +20,7 @@
 #include <mutex>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -270,6 +272,8 @@ struct Encoding {
   static Encoding simd() { return {FHE_B200_ENCODING_SIMD, 0}; }
   static Encoding poly_at_level(uint32_t level) { return {FHE_B200_ENCODING_POLY, level}; }
   static Encoding simd_at_level(uint32_t level) { return {FHE_B200_ENCODING_SIMD, level}; }
+  bool operator==(const Encoding& o) const { return kind == o.kind && level == o.level; }
+  bool operator!=(const Encoding& o) const { return !(*this == o); }
 };
 
 // fhe::bfv::PlaintextVec (bfv/plaintext_vec.rs:20-103): the poly_ntt of every plaintext in a 1-part device batch.
@@ -289,12 +293,35 @@ class PlaintextVec {
     return try_encode(values.data(), values.size(), e, par);
   }
   size_t len() const { return batch_.count(); }
+  // the stored encoding; false for plaintexts without one (SecretKey::try_decrypt's)
+  bool has_encoding() const { return has_encoding_; }
   const Encoding& encoding() const { return encoding_; }
   const Ciphertext& batch() const { return batch_; }
   std::vector<uint64_t> poly_ntt() const { return batch_.to_host(); }   // [count][limbs][N]
 
+  // Plaintext::resolve_encoding (plaintext.rs:137-153); `e` may be null
+  Encoding resolve_encoding(const Encoding* e) const {
+    if (!has_encoding_ && !e) throw Error(FHE_B200_INVALID_ARGUMENT, "PlaintextError::MissingEncoding");
+    if (has_encoding_ && e && *e != encoding_) throw Error(FHE_B200_INVALID_ARGUMENT, "EncodingError::Mismatch");
+    return has_encoding_ ? encoding_ : *e;
+  }
+  // Vec<u64>::try_decode (T = uint64_t) / Vec<i64>::try_decode (T = int64_t) (plaintext.rs:374-459) of every plaintext
+  // on the device: count * N values, plaintext k at [k*N, (k+1)*N)
+  template <typename T>
+  std::vector<T> try_decode(const Encoding* e = nullptr) const {
+    static_assert(std::is_same<T, uint64_t>::value || std::is_same<T, int64_t>::value, "u64 or i64 values");
+    const Encoding enc = resolve_encoding(e);
+    std::vector<T> out(len() * batch_.par()->degree());
+    check(fhe_b200_decode(batch_.par()->encoder(), enc.kind, std::is_signed<T>::value ? 1 : 0, batch_.handle(),
+                          out.data(), out.size(), batch_.stream()));
+    batch_.sync();
+    return out;
+  }
+
  protected:
+  friend class SecretKey;
   PlaintextVec(Ciphertext b, const Encoding& e) : batch_(std::move(b)), encoding_(e) {}
+  explicit PlaintextVec(Ciphertext b) : batch_(std::move(b)), encoding_(Encoding::poly()), has_encoding_(false) {}
   static PlaintextVec encode(const void* values, size_t n, bool is_signed, const Encoding& e,
                              const std::shared_ptr<BfvParameters>& par) {
     const size_t N = par->degree();
@@ -305,6 +332,7 @@ class PlaintextVec {
   }
   Ciphertext batch_;
   Encoding encoding_;
+  bool has_encoding_ = true;
 };
 
 // fhe::bfv::Plaintext (bfv/plaintext.rs:20-27): one plaintext of at most N values (TooManyValues, :311-345)
@@ -328,6 +356,44 @@ inline Ciphertext& Ciphertext::add_plain(const PlaintextVec& pts, bool subtract)
   check(fhe_b200_add_plain_batch(h_, pts.batch().handle(), subtract ? 1 : 0, stream_));
   return *this;
 }
+
+// fhe::bfv::SecretKey (keys/secret_key.rs:25-53) on the device, from its N signed coefficients (SecretKey.coeffs; a
+// Rust host reads them from sk.to_bytes(), see fhe_b200_wire.hpp).  The device copy of s is erased when the key is
+// released; the host copy kept for to_bytes is erased with the object.
+class SecretKey {
+ public:
+  SecretKey(std::shared_ptr<BfvParameters> par, const std::vector<int64_t>& coeffs) : par_(std::move(par)), coeffs_(coeffs) {
+    if (coeffs_.size() != par_->degree()) throw Error(FHE_B200_INVALID_ARGUMENT, "a secret key has N coefficients");
+    check(fhe_b200_secret_key_create(par_->handle(), coeffs_.data(), &h_));
+  }
+  SecretKey(const SecretKey&) = delete;
+  SecretKey& operator=(const SecretKey&) = delete;
+  ~SecretKey() {
+    fhe_b200_secret_key_free(h_);
+    volatile int64_t* c = coeffs_.data();
+    for (size_t i = 0; i < coeffs_.size(); i++) c[i] = 0;
+  }
+  // SecretKey::try_decrypt (secret_key.rs:198-260) of every ciphertext of the batch: plaintexts without an encoding
+  PlaintextVec try_decrypt(const Ciphertext& ct) const {
+    Ciphertext out(par_, ct.count(), 1, ct.level(), Representation::Ntt, ct.stream());
+    check(fhe_b200_decrypt(h_, ct.handle(), out.handle(), ct.stream()));
+    return PlaintextVec(std::move(out));
+  }
+  // SecretKey::measure_noise (secret_key.rs:55-98) of every ciphertext of the batch
+  std::vector<uint32_t> measure_noise(const Ciphertext& ct) const {
+    std::vector<uint32_t> out(ct.count());
+    check(fhe_b200_measure_noise(h_, ct.handle(), out.data(), ct.stream()));
+    ct.sync();
+    return out;
+  }
+  const std::vector<int64_t>& coeffs() const { return coeffs_; }
+  const std::shared_ptr<BfvParameters>& par() const { return par_; }
+
+ private:
+  std::shared_ptr<BfvParameters> par_;
+  std::vector<int64_t> coeffs_;
+  fhe_b200_secret_key* h_ = nullptr;
+};
 
 class KeySwitchingKey {
  public:

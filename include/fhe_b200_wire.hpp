@@ -6,6 +6,7 @@
 //   fhers.bfv.KeySwitchingKey     bfv.proto:16-23,                   fhe/src/bfv/keys/key_switching_key.rs:365-482
 //   fhers.bfv.RelinearizationKey  bfv.proto:25-27 (keys/relinearization_key.rs:113-135), GaloisKey :29-32
 //                                 (keys/galois_key.rs:146-173)
+//   fhers.bfv.SecretKey           bfv.proto:54-56,                   fhe/src/bfv/keys/secret_key.rs:142-175
 // `Rq.coefficients` -- the bit-packed power-basis words, all but a few bytes of every message -- is produced and consumed
 // on the device (fhe_b200_batch_pack / fhe_b200_batch_unpack); this header is the proto3 framing around it, emitting
 // what prost emits (fields in field-number order, zero scalars and empty singular `bytes` omitted) and accepting what
@@ -248,6 +249,47 @@ inline std::string encode_galois_key(const std::string& ksk, uint32_t exponent) 
   put_uint(out, 2, exponent);
   return out;
 }
+// ---- SecretKey (bfv.proto:54-56: repeated sint64 coeffs = 1, packed, zig-zag) -------------------------------------
+// SecretKey::to_bytes (secret_key.rs:142-148)
+inline std::string encode_secret_key(const int64_t* coeffs, size_t n) {
+  std::string payload, out;
+  for (size_t i = 0; i < n; i++) put_varint(payload, ((uint64_t)coeffs[i] << 1) ^ (uint64_t)(coeffs[i] >> 63));
+  if (n) put_len(out, 1, payload);
+  return out;
+}
+// SecretKey::from_bytes (secret_key.rs:151-175): packed and unpacked coefficients are both accepted (as prost does);
+// a count other than `degree` is InvalidSecretKeyCoefficientCount
+inline std::vector<int64_t> decode_secret_key(const void* data, size_t n, size_t degree) {
+  std::vector<int64_t> c;
+  auto unzig = [](uint64_t v) { return (int64_t)((v >> 1) ^ (0 - (v & 1))); };
+  Reader r(data, n);
+  while (r.next()) {
+    if (r.field != 1) continue;
+    if (r.wire_type == 0) {
+      c.push_back(unzig(r.value));
+    } else {
+      r.expect(2);
+      // packed: the payload is a run of varints
+      const uint8_t *p = r.span.p, *end = r.span.p + r.span.n;
+      while (p < end) {
+        uint64_t v = 0;
+        for (int shift = 0;; shift += 7) {
+          if (p >= end) throw WireError("Decode", FHE_B200_INVALID_ARGUMENT, "truncated varint");
+          const uint8_t b = *p++;
+          if (shift == 63 && b > 1) throw WireError("Decode", FHE_B200_INVALID_ARGUMENT, "varint overflows 64 bits");
+          v |= (uint64_t)(b & 0x7f) << shift;
+          if (!(b & 0x80)) break;
+        }
+        c.push_back(unzig(v));
+      }
+    }
+  }
+  if (c.size() != degree)
+    throw WireError("InvalidSecretKeyCoefficientCount", FHE_B200_INVALID_ARGUMENT,
+                    std::to_string(c.size()) + " coefficients, expected " + std::to_string(degree));
+  return c;
+}
+
 // sub-message `field` of a wrapper message; *scalar2 = varint field 2 when present
 inline Span sub_message(const void* data, size_t n, uint32_t field, const char* missing, uint32_t* scalar2 = nullptr) {
   Span s;
@@ -397,6 +439,15 @@ inline GaloisKey galois_key_from_bytes(std::shared_ptr<BfvParameters> par, const
   exponent %= two_n;                        // SubstitutionExponent::new (rq/mod.rs:99-106)
   if (!(exponent & 1)) throw WireError("InvalidSubstitutionExponent", FHE_B200_INVALID_EXPONENT);
   return GaloisKey(exponent, std::move(ksk));
+}
+// SecretKey::to_bytes / from_bytes (secret_key.rs:142-175)
+inline std::string to_bytes(const SecretKey& sk) { return wire::encode_secret_key(sk.coeffs().data(), sk.coeffs().size()); }
+inline std::unique_ptr<SecretKey> secret_key_from_bytes(std::shared_ptr<BfvParameters> par, const std::string& data) {
+  std::vector<int64_t> c = wire::decode_secret_key(data.data(), data.size(), par->degree());
+  std::unique_ptr<SecretKey> sk(new SecretKey(std::move(par), c));
+  volatile int64_t* w = c.data();
+  for (size_t i = 0; i < c.size(); i++) w[i] = 0;
+  return sk;
 }
 
 }  // namespace bfv
