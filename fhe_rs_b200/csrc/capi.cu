@@ -557,6 +557,9 @@ void key_switch_core(const fhe_b200_params* par, const fhe_b200_ksk* k, const u6
   u64 qmax = 0, qmin = ~0ull;
   for (u32 i = 0; i < L; i++) qmax = std::max(qmax, par->moduli[i]);
   for (u32 j = 0; j < Lk; j++) qmin = std::min(qmin, par->moduli[j]);
+  // The lifts of plaintext words (encode, to_poly_from_coefficients, decrypt) test only t > 4 * q_min - 1: the
+  // butterflies take [0, 4p) for any modulus, down to q_min = 193 < 2^8 (tests/test_gpu_client_edges.py).  The extra
+  // clause here changes the choice only when every modulus of the key level is below 2^10, which needs N <= 64.
   const bool reduce = qmax > 4 * qmin - 1 || qmin < (1ull << 8);
   // forward_vt_lazy (rq/mod.rs:580): the digits stay in [0,4q_j); the lazy accumulator of the inner product takes
   // any 64-bit operand and reduces once

@@ -7,6 +7,9 @@ projected onto the limbs of a basis.  Uniform random residues land on these poin
   * the extender (factor one) around (Q - 1)/2;
   * switch_down around the ties of round(x / q_last).
 `residue_rows` gives rows that drive lazy sums to their extremes instead (all q - 1 and friends).
+For the client side: `decrypt_phases` (decryption's ties, Q / 2 and the failure boundary), `noise_points` (the word
+boundaries of Q), `key_extremes` (secret keys at the extremes), and the shapes and plaintext moduli of
+CLIENT_SHAPES / `client_plaintexts`.
 """
 from __future__ import annotations
 
@@ -23,6 +26,57 @@ BOUNDARY_PRIMES = {
     "non_solinas_min": 0x3fffffffeff50001,   # c = 0x100affff: the largest 62-bit prime that is a Barrett limb
     "above_2_61": 0x20000000000b0001,        # a Barrett limb just above 2^61
 }
+
+
+def gen62(degree: int, k: int) -> int:
+    """the k-th 62-bit NTT-friendly prime below 2^62 (the generator's order)"""
+    import fhe_oracle as O
+    ub = 1 << 62
+    for _ in range(k + 1):
+        ub = O.generate_prime(62, 2 * degree, ub)
+    return ub
+
+
+# decryption shapes: name -> (degree, moduli sizes, or the names of the first moduli followed by generated 62-bit
+# ones).  With one output row (q_0) the scaler kernel is scale_small_kernel for N < 128, scale_tma_kernel when every
+# modulus of the plaintext context is Solinas, scale_kernel otherwise.
+CLIENT_SHAPES = {
+    "n16_l5": (16, [62] * 5),
+    "set_a": (1 << 12, [62] * 2),
+    "set_c": (1 << 15, [62] * 14),
+    "q0_barrett": (1 << 13, ["non_solinas_min", 0, 1]),
+    "q0_above_2_61": (1 << 13, ["above_2_61", 0, 1]),
+    "q0_solinas_max_c": (1 << 13, ["solinas_max_c", 0, 1]),
+    "q1_barrett": (1 << 13, [0, "non_solinas_min", 1]),        # t = 1153: plaintext context (q_0, q_1)
+    "l31": (1 << 13, [62] * 31),
+    "n2_16": (1 << 16, [62] * 3),
+    "ten_bit": (64, [62, 62, 10]),
+}
+
+
+def client_moduli(name: str) -> List[int]:
+    import fhe_oracle as O
+    degree, spec = CLIENT_SHAPES[name]
+    if all(isinstance(s, int) and s >= 10 for s in spec):
+        return O.BfvParameters.generate_moduli(spec, degree)
+    return [BOUNDARY_PRIMES[s] if isinstance(s, str) else gen62(degree, s) for s in spec]
+
+
+def coprime_below(bound: int, moduli: Sequence[int]) -> int:
+    """the largest t < bound coprime with every modulus"""
+    from math import gcd
+    t = bound - 1
+    while any(gcd(t, int(q)) != 1 for q in moduli):
+        t -= 1
+    return t
+
+
+def client_plaintexts(degree: int, moduli: Sequence[int]) -> Dict[str, int]:
+    """plaintext moduli for decryption: 2 (a one-modulus plaintext context with a 62-bit q_0), 1153, a 40-bit prime,
+    the largest t below q_0, and the largest t the library takes (t < 2^62), which is above q_0"""
+    import fhe_oracle as O
+    return {"t2": 2, "t1153": 1153, "t40": O.generate_prime(40, 2 * degree, 1 << 40),
+            "below_q0": coprime_below(int(moduli[0]), moduli), "max": coprime_below(1 << 62, moduli)}
 
 
 def product(moduli: Sequence[int]) -> int:
@@ -103,6 +157,66 @@ def polys_from_values(values: Sequence[int], moduli: Sequence[int], degree: int)
     for i, q in enumerate(moduli):
         out[:, i, :] = np.array([v % int(q) for v in vals], dtype=np.uint64).reshape(count, degree)
     return out
+
+
+def decrypt_phases(Q: int, t: int, rng: np.random.Generator, n_m: int = 4) -> List[int]:
+    """phases x in [0, Q) where decryption decides something: the ties of t x / Q and the sign boundary Q / 2
+    (scaler_near_ties, sign_boundary), and Delta m +/- floor(Q / 2t) + d (Delta = floor(Q / t), d in [-3, 3]) for
+    m in {0, 1, t/2, t - 1} -- a ciphertext whose noise is at the decryption-failure boundary"""
+    delta, half = Q // t, Q // (2 * t)
+    out = scaler_near_ties(Q, t, Q, rng, n_m) + sign_boundary(Q)
+    for m in sorted({0, 1, t // 2, t - 1}):
+        for s in (-half, half):
+            out += [(delta * m + s + d) % Q for d in D_RANGE]
+    return out
+
+
+def decrypt_windows(x: int, Q: int, t: int, eps: float = 2.0 ** -40):
+    """(t x / Q within eps of a half-integer, x / Q within eps of 1/2): where the reference's fixed-point scaler may
+    depart from round(t x / Q)"""
+    from fractions import Fraction
+    return (abs(Fraction(x * t % Q, Q) - Fraction(1, 2)) < eps, abs(Fraction(x, Q) - Fraction(1, 2)) < eps)
+
+
+def decrypt_one(par, level: int, x: int) -> int:
+    """the oracle's decryption of one phase coefficient x (its level scaler, then ((v + t) mod q_0) mod t)"""
+    lv, t, q0 = par.level(level), par.plaintext, int(par.moduli[0])
+    v0 = int(lv.scaler.scaler.scale_one(lv.poly_context.rns.project(x), 1, 0)[0])
+    return ((v0 + t) % q0) % t
+
+
+def noise_one(par, level: int, x: int) -> int:
+    """measure_noise of a ciphertext whose phase is x at one coefficient and 0 elsewhere, in plain integers: the
+    phase minus to_poly(decrypt) = x - (m q_mod_t mod t) (-t)^-1 mod Q, then min(bits(v), bits(Q - v))"""
+    lv, t = par.level(level), par.plaintext
+    Q = lv.poly_context.modulus()
+    m = decrypt_one(par, level, x) * lv.q_mod_t % t
+    v = (x - m * pow(-t % Q, -1, Q)) % Q
+    return min(v.bit_length(), (Q - v).bit_length())
+
+
+def noise_points(Q: int) -> List[int]:
+    """phases for measure_noise's multi-word arithmetic: 2^k - 1, 2^k, 2^k + 1 and Q - 2^k at every 64-bit word
+    boundary k below bits(Q), and floor(Q / 2), ceil(Q / 2)"""
+    out = []
+    for k in range(64, Q.bit_length(), 64):
+        out += [(1 << k) - 1, 1 << k, (1 << k) + 1, Q - (1 << k)]
+    out += [Q // 2, (Q + 1) // 2]
+    return [x for x in out if 0 <= x < Q]
+
+
+def key_extremes(degree: int, q0: int, rng: np.random.Generator) -> Dict[str, np.ndarray]:
+    """secret-key coefficients [N] (int64) at the extremes: the constants -1 and 1 (every NTT word of s is q - 1,
+    resp. 1), and i64 min / max, +/-(q_0 - 1), +/-q_0 at random positions among small random coefficients"""
+    i64 = np.iinfo(np.int64)
+    minus, plus = np.zeros(degree, np.int64), np.zeros(degree, np.int64)
+    minus[0], plus[0] = -1, 1
+    mixed = rng.integers(-16, 17, size=degree).astype(np.int64)
+    special = [i64.min, i64.max, q0 - 1, -(q0 - 1), q0, -q0]
+    pos = rng.permutation(degree)[:len(special)] if degree >= len(special) else np.arange(degree)
+    for p, v in zip(pos, special):
+        mixed[p] = v
+    return {"minus_one": minus, "one": plus, "extremes": mixed}
 
 
 def residue_rows(moduli: Sequence[int], degree: int) -> Dict[str, np.ndarray]:
