@@ -67,6 +67,8 @@ SYMBOLS = {
     "fhe_b200_decrypt": (_i, [_vp, _vp, _vp, _vp]),
     "fhe_b200_decode": (_i, [_vp, _i, _i, _vp, _vp, C.c_size_t, _vp]),
     "fhe_b200_measure_noise": (_i, [_vp, _vp, _vp, _vp]),
+    "fhe_b200_encrypt_sk": (_i, [_vp, _vp, _u32, _vp, _vp, _vp]),
+    "fhe_b200_encrypt_pk": (_i, [_vp, _vp, _u32, _vp, _vp, _vp]),
     "fhe_b200_mul": (_i, [_vp, _vp, _vp, _vp]),
     "fhe_b200_relinearize": (_i, [_vp, _vp, _vp, _vp]),
     "fhe_b200_mul_relin": (_i, [_vp, _vp, _vp, _i, _vp, _vp]),

@@ -12,6 +12,7 @@ No CPU fallback exists: every operation is a CUDA launch behind the C ABI."""
 from __future__ import annotations
 
 import ctypes as C
+import os
 from typing import Dict, Optional, Sequence
 
 import numpy as np
@@ -22,7 +23,7 @@ from .wire import WireError
 
 __all__ = ["BfvParameters", "BfvParametersBuilder", "Ciphertext", "KeySwitchingKey", "RelinearizationKey", "RGSWCiphertext",
            "GaloisKey", "EvaluationKey", "Multiplicator", "ScalingFactor", "dot_product_scalar", "FheError", "WireError", "NTT", "POWER_BASIS",
-           "Encoding", "Plaintext", "PlaintextVec", "SecretKey"]
+           "Encoding", "Plaintext", "PlaintextVec", "SecretKey", "PublicKey"]
 
 
 def _release(free_name: str, handle) -> None:
@@ -45,11 +46,15 @@ class BfvParameters:
 
     def __init__(self, degree: int, plaintext_modulus: int, moduli: Optional[Sequence[int]] = None,
                  moduli_sizes: Optional[Sequence[int]] = None, psi: Optional[Sequence[int]] = None,
-                 device: int = 0, plaintext_psi: Optional[int] = None):
+                 device: int = 0, plaintext_psi: Optional[int] = None, variance: int = 10):
         """plaintext_psi: the 2N-th root of unity for the plaintext modulus (the reference's
         NttOperator::new(t).omegas[N/2], for SIMD words interchangeable with a Rust process); None selects the
-        default rule of fhe_b200_params_create."""
+        default rule of fhe_b200_params_create.  variance: BfvParameters::variance, the parameter of the centred
+        binomial errors of encryption, 1..32 (parameters.rs:384-388, :449-454)."""
         L = _capi.lib()
+        if not 1 <= int(variance) <= 32:
+            raise FheError(_capi.INVALID_ARGUMENT, "InvalidVariance: %d is outside 1..32" % variance)
+        self.variance = int(variance)
         self._enc = None
         self._plaintext_psi = plaintext_psi
         if (moduli is None) == (moduli_sizes is None):
@@ -178,6 +183,7 @@ class BfvParametersBuilder:
         self._moduli = None
         self._sizes = None
         self._psi = None
+        self._variance = 10
 
     def set_degree(self, degree: int):
         self._degree = degree
@@ -200,8 +206,14 @@ class BfvParametersBuilder:
         self._psi = list(psi)
         return self
 
+    def set_variance(self, variance: int):
+        """the error variance, 1..32 (checked by build, parameters.rs:384-388)"""
+        self._variance = variance
+        return self
+
     def build(self, device: int = 0) -> BfvParameters:
-        return BfvParameters(self._degree, self._plaintext, self._moduli, self._sizes, self._psi, device)
+        return BfvParameters(self._degree, self._plaintext, self._moduli, self._sizes, self._psi, device,
+                             variance=self._variance)
 
     build_arc = build
 
@@ -600,9 +612,10 @@ class PlaintextVec:
 
 
 class SecretKey:
-    """fhe::bfv::SecretKey (keys/secret_key.rs:25-53) on the device, from its N signed coefficients.  Decryption and
-    noise measurement run on the device; the device copy of s is erased when the key is released.  Key generation and
-    encryption stay with the client (their randomness cannot be reproduced here)."""
+    """fhe::bfv::SecretKey (keys/secret_key.rs:25-53) on the device, from its N signed coefficients.  Encryption,
+    decryption and noise measurement run on the device; the device copy of s is erased when the key is released.
+    Encryption draws its randomness from the seeded ChaCha20 stream of include/fhe_b200.h.  Key generation (the
+    coefficients themselves, relinearization and Galois keys) stays with the client."""
 
     def __init__(self, par: BfvParameters, coeffs):
         c = np.array(coeffs, dtype=np.int64)   # our own copy, kept for to_bytes (the reference keeps SecretKey.coeffs)
@@ -628,6 +641,13 @@ class SecretKey:
     def from_bytes(par: BfvParameters, data: bytes) -> "SecretKey":   # secret_key.rs:151-175
         return SecretKey(par, wire.decode_secret_key(data, par.degree()))
 
+    def try_encrypt(self, pts: Optional[PlaintextVec] = None, seed: Optional[bytes] = None, count: int = 1,
+                    level: int = 0) -> Ciphertext:
+        """SecretKey::try_encrypt (secret_key.rs:100-136, :181-193) of every plaintext of `pts` on the device: a batch
+        of one fresh ciphertext per plaintext, at the plaintexts' level.  pts None encrypts `count` zeros at `level`.
+        seed: the 32 bytes that key the stream; None draws os.urandom(32) (a seed must never be reused)."""
+        return _encrypt(_capi.lib().fhe_b200_encrypt_sk, self._h, self.par, pts, seed, count, level)
+
     def try_decrypt(self, ct: Ciphertext) -> PlaintextVec:
         """SecretKey::try_decrypt (secret_key.rs:198-260) of every ciphertext of the batch: plaintexts with no
         encoding (decode them with try_decode(encoding))."""
@@ -641,6 +661,55 @@ class SecretKey:
         check(_capi.lib().fhe_b200_measure_noise(self._h, ct._h, _ptr(out), ct.stream))
         check(_capi.lib().fhe_b200_sync(ct.stream))
         return out
+
+
+def _encrypt(fn, key, par: BfvParameters, pts: Optional[PlaintextVec], seed: Optional[bytes], count: int,
+             level: int) -> Ciphertext:
+    seed = os.urandom(32) if seed is None else bytes(seed)
+    if len(seed) != 32:
+        raise FheError(_capi.INVALID_ARGUMENT, "a seed is 32 bytes, got %d" % len(seed))
+    b = pts.batch if pts is not None else None
+    out = Ciphertext(par, b.count if b else count, 2, b.level if b else level, NTT, b.stream if b else 0)
+    check(fn(key, b._h if b else None, par.variance, seed, out._h, out.stream))
+    return out
+
+
+class PublicKey:
+    """fhe::bfv::PublicKey (keys/public_key.rs:17-22): its c, one 2-part ciphertext at level 0, on the device."""
+
+    def __init__(self, par: BfvParameters, c: Ciphertext):
+        if c.count != 1 or len(c) != 2:
+            raise FheError(_capi.INVALID_ARGUMENT, "a public key is one 2-part ciphertext")
+        if c.level != 0:
+            raise FheError(_capi.INVALID_LEVEL, "InvalidPublicKeyLevel: %d, expected 0" % c.level)
+        self.par, self.c = par, c
+
+    @staticmethod
+    def new(sk: SecretKey, seed: Optional[bytes] = None) -> "PublicKey":
+        """PublicKey::new (public_key.rs:26-38): a secret-key encryption of zero at level 0"""
+        return PublicKey(sk.par, sk.try_encrypt(None, seed))
+
+    def try_encrypt(self, pts: Optional[PlaintextVec] = None, seed: Optional[bytes] = None, count: int = 1,
+                    level: int = 0) -> Ciphertext:
+        """PublicKey::try_encrypt (public_key.rs:45-92) of every plaintext of `pts`, as SecretKey.try_encrypt"""
+        return _encrypt(_capi.lib().fhe_b200_encrypt_pk, self.c._h, self.par, pts, seed, count, level)
+
+    def to_bytes(self) -> bytes:   # public_key.rs:95-107: both parts (a device-encrypted key carries no seed)
+        return wire.encode_public_key(self.c.to_bytes()[0])
+
+    @staticmethod
+    def from_bytes(par: BfvParameters, data: bytes, seeded_c1: Optional[np.ndarray] = None) -> "PublicKey":
+        """PublicKey::from_bytes (public_key.rs:109-149).  The reference writes a compact message (c0 and the seed
+        of c1); decoding one needs `seeded_c1`, the [limbs][N] NTT words of c1 expanded by the Rust host, as
+        Ciphertext.from_bytes does.  A key at a level other than 0 is InvalidPublicKeyLevel."""
+        msg = wire.decode_public_key(data)
+        _, seed, level = wire.decode_ciphertext(msg)
+        if level != 0:
+            raise WireError("InvalidPublicKeyLevel", _capi.INVALID_LEVEL, "level %d, expected 0" % level)
+        if seed and seeded_c1 is None:
+            raise WireError("SeedExpansion", _capi.UNSUPPORTED, "the message carries a seed: pass the host-expanded c1")
+        halves = None if seeded_c1 is None else np.asarray(seeded_c1, dtype=np.uint64)[None]
+        return PublicKey(par, Ciphertext.from_bytes(par, [msg], halves))
 
 
 class Plaintext(PlaintextVec):

@@ -536,6 +536,17 @@ const RowIds& ids_of(const fhe_b200_batch* b) {
   return b->mul_basis ? lv.mul_ids : lv.ctx_ids;
 }
 
+// Ciphertext::switch_down of `polys` NTT polynomials at `level` (L >= 2), in place: d [polys][L][N] becomes
+// [polys][L-1][N], compacted at the start of the same buffer
+void switch_down_polys(const fhe_b200_params* par, u32 level, u64* d, u32 polys, Workspace& ws, cudaStream_t st) {
+  const LevelData& lv = par->level(level);
+  const LevelData& nl = par->level(level + 1);
+  u64* tmp = ws.words((size_t)polys * nl.L << par->logn);
+  launch_ntt(d, d, polys * lv.L, lv.ctx_ids, par->d_limbs, par->logn, true, 1, false, st);
+  launch_switch_down(lv.sd, d, tmp, polys, lv.L, lv.ctx_ids, par->d_limbs, par->logn, st);
+  launch_ntt(tmp, d, polys * nl.L, nl.ctx_ids, par->d_limbs, par->logn, false, 1, false, st);
+}
+
 // KeySwitchingKey::key_switch core on a contiguous power-basis buffer c2 [cts][L][N]
 // (key_switching_key.rs:241-270): out0/out1 (+ optional bases), rows (ct, j) at (ct*out_ct_rows + j).
 void key_switch_core(const fhe_b200_params* par, const fhe_b200_ksk* k, const u64* c2, u32 cts, const u64* base0,
@@ -1301,6 +1312,17 @@ static void to_poly_from_coefficients(const fhe_b200_params* par, const LevelDat
   launch_ntt(x, m, n * lv.L, lv.ctx_ids, par->d_limbs, par->logn, false, lv.L, reduce, st);
 }
 
+// Plaintext::to_poly (plaintext.rs:172-197) of plaintexts [p0, p0 + n) of the 1-part NTT batch pts into m [n][L][N],
+// before the delta product (t < q_0); x: scratch of n * N words
+static void plain_to_poly(const fhe_b200_params* par, const LevelData& lv, const fhe_b200_batch* pts, u32 p0, u32 n,
+                          u64* m, u64* x, cudaStream_t st) {
+  const size_t N = par->N;
+  FHE_CUDA(cudaMemcpy2DAsync(x, N * 8, pts->d + (size_t)p0 * lv.L * N, lv.L * N * 8, N * 8, n, cudaMemcpyDeviceToDevice,
+                             st));
+  launch_ntt(x, x, n, q0_row_ids(), par->d_limbs, par->logn, true, 1, false, st);   // limb 0 of into_power_basis
+  to_poly_from_coefficients(par, lv, x, n, m, st);
+}
+
 int fhe_b200_add_plain_batch(fhe_b200_batch* a, const fhe_b200_batch* pts, int subtract, void* stream) {
   API_BEGIN
   check_plain_batch(a, pts);
@@ -1311,21 +1333,13 @@ int fhe_b200_add_plain_batch(fhe_b200_batch* a, const fhe_b200_batch* pts, int s
   const LevelData& lv = par->level(a->level);
   const u32 L = lv.L, logn = par->logn;
   const size_t N = par->N;
-  const RowIds q0_ids = q0_row_ids();
-  // Plaintext::to_poly of plaintexts [p0, p0 + n) into m [n][L][N] (before the delta product)
-  auto to_poly = [&](u32 p0, u32 n, u64* m, Workspace& ws, cudaStream_t st) {
-    u64* x = ws.words((size_t)n * N);
-    FHE_CUDA(cudaMemcpy2DAsync(x, N * 8, pts->d + (size_t)p0 * L * N, L * N * 8, N * 8, n, cudaMemcpyDeviceToDevice, st));
-    launch_ntt(x, x, n, q0_ids, par->d_limbs, logn, true, 1, false, st);      // limb 0 of into_power_basis
-    to_poly_from_coefficients(par, lv, x, n, m, st);
-  };
   cudaStream_t user = (cudaStream_t)stream;
   Workspace shared_ws(par, user);
   const bool shared = pts->count == 1;
   u64* m_shared = nullptr;
   if (shared) {   // built once, before the chunks' side streams fork from `user`
     m_shared = shared_ws.words((size_t)L * N);
-    to_poly(0, 1, m_shared, shared_ws, user);
+    plain_to_poly(par, lv, pts, 0, 1, m_shared, shared_ws.words(N), user);
   }
   ChunkRunner chunks(par, a->count, user);
   chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
@@ -1333,7 +1347,7 @@ int fhe_b200_add_plain_batch(fhe_b200_batch* a, const fhe_b200_batch* pts, int s
     const u64* m = m_shared;
     if (!shared) {
       u64* mc = ws.words((size_t)n * L * N);
-      to_poly(c0, n, mc, ws, st);
+      plain_to_poly(par, lv, pts, c0, n, mc, ws.words((size_t)n * N), st);
       m = mc;
     }
     launch_add_scaled(a->d + (size_t)c0 * a->parts * L * N, m, n, a->parts, shared ? 1 : n, lv.d_delta, lv.d_delta_s,
@@ -1569,6 +1583,106 @@ int fhe_b200_decode(const fhe_b200_encoder* e, int encoding, int is_signed, cons
     FHE_CUDA(cudaMemcpyAsync(dst + (size_t)c0 * N * 8, x, (size_t)n * N * 8, cudaMemcpyDefault, st));
   });
   FHE_CUDA(cudaGetLastError());
+  API_END
+}
+
+// ---- encryption (keys/secret_key.rs:100-136, :181-193; keys/public_key.rs:45-92)
+// the checks shared by both entry points; returns the seed as the key words of the ChaCha20 state
+static EncSeed check_encrypt(const fhe_b200_params* par, const fhe_b200_batch* pts, const uint8_t* seed,
+                             const fhe_b200_batch* out) {
+  REQUIRE(seed && out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  REQUIRE(out->par == par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch");
+  REQUIRE(!out->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
+  REQUIRE(out->parts == 2, FHE_B200_INVALID_ARGUMENT, "out must be a batch of 2-part ciphertexts");
+  if (pts) {
+    REQUIRE(pts->par == par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch");
+    REQUIRE(!pts->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
+    REQUIRE(pts->parts == 1 && pts->count == out->count, FHE_B200_INVALID_ARGUMENT,
+            "pts must be a 1-part batch with one plaintext per output ciphertext");
+    REQUIRE(pts->level == out->level, FHE_B200_INVALID_LEVEL, "InvalidLevel: pts and out are at different levels");
+    need_repr(pts, FHE_B200_NTT);
+  }
+  REQUIRE(par->t_small && par->t_mod.t < par->moduli[0], FHE_B200_UNSUPPORTED,
+          "to_poly needs t below the first ciphertext modulus");
+  EncSeed K;
+  for (int i = 0; i < 8; i++)
+    K.w[i] = (u32)seed[4 * i] | (u32)seed[4 * i + 1] << 8 | (u32)seed[4 * i + 2] << 16 | (u32)seed[4 * i + 3] << 24;
+  return K;
+}
+
+static void check_variance(uint32_t variance) {   // BfvParametersBuilder::build (parameters.rs:449-454)
+  REQUIRE(variance >= 1 && variance <= 32, FHE_B200_INVALID_ARGUMENT,
+          "InvalidVariance: " + std::to_string(variance) + " is outside 1..32");
+}
+
+// part 0 of the ciphertexts dst [n][2][L][N] += Plaintext::to_poly of plaintexts [c0, c0 + n) of pts
+static void add_to_poly(const fhe_b200_params* par, const LevelData& lv, const fhe_b200_batch* pts, u32 c0, u32 n,
+                        u64* dst, Workspace& ws, cudaStream_t st) {
+  u64* m = ws.secret_words(((size_t)n * lv.L) << par->logn);
+  plain_to_poly(par, lv, pts, c0, n, m, ws.secret_words((size_t)n << par->logn), st);
+  launch_add_scaled(dst, m, n, 2, n, lv.d_delta, lv.d_delta_s, false, lv.ctx_ids, par->d_limbs, par->logn, st);
+}
+
+int fhe_b200_encrypt_sk(const fhe_b200_secret_key* sk, const fhe_b200_batch* pts, uint32_t variance,
+                        const uint8_t* seed, fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  check_variance(variance);
+  REQUIRE(sk, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = sk->par;
+  const EncSeed K = check_encrypt(par, pts, seed, out);
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(out->level);
+  const u32 L = lv.L, logn = par->logn;
+  ChunkRunner chunks(par, out->count, (cudaStream_t)stream);
+  chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace ws(par, st);
+    u64* e = ws.secret_words(((size_t)n * L) << logn);
+    launch_cbd(e, n, c0, 1, 1, variance, K, lv.ctx_ids, par->d_limbs, logn, st);
+    launch_ntt(e, e, n * L, lv.ctx_ids, par->d_limbs, logn, false, 1, false, st);
+    u64* dst = out->d + (((size_t)c0 * 2 * L) << logn);
+    launch_encrypt_sk(sk->s, e, dst, n, c0, K, lv.ctx_ids, par->d_limbs, logn, st);
+    if (pts) add_to_poly(par, lv, pts, c0, n, dst, ws, st);
+  });
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
+  API_END
+}
+
+int fhe_b200_encrypt_pk(const fhe_b200_batch* pk, const fhe_b200_batch* pts, uint32_t variance, const uint8_t* seed,
+                        fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  check_variance(variance);
+  REQUIRE(pk, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = pk->par;
+  REQUIRE(!pk->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
+  REQUIRE(pk->count == 1 && pk->parts == 2, FHE_B200_INVALID_ARGUMENT, "a public key is one 2-part ciphertext");
+  REQUIRE(pk->level == 0, FHE_B200_INVALID_LEVEL, "InvalidPublicKeyLevel: " + std::to_string(pk->level));
+  need_repr(pk, FHE_B200_NTT);
+  const EncSeed K = check_encrypt(par, pts, seed, out);
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(out->level);
+  const u32 L = lv.L, logn = par->logn;
+  cudaStream_t user = (cudaStream_t)stream;
+  Workspace key_ws(par, user);
+  const u64* c = pk->d;
+  if (out->level > 0) {   // a copy of the key switched down to the plaintext level (public_key.rs:60-70)
+    u64* sw = key_ws.words(((size_t)2 * par->Lmax) << logn);
+    FHE_CUDA(cudaMemcpyAsync(sw, pk->d, pk->words_per_ct() * sizeof(u64), cudaMemcpyDeviceToDevice, user));
+    for (u32 l = 0; l < out->level; l++) switch_down_polys(par, l, sw, 2, key_ws, user);
+    c = sw;
+  }
+  ChunkRunner chunks(par, out->count, user);
+  chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace ws(par, st);
+    u64* uee = ws.secret_words(((size_t)n * 3 * L) << logn);   // u, e1, e2
+    launch_cbd(uee, n, c0, 2, 3, variance, K, lv.ctx_ids, par->d_limbs, logn, st);
+    launch_ntt(uee, uee, n * 3 * L, lv.ctx_ids, par->d_limbs, logn, false, 1, false, st);
+    u64* dst = out->d + (((size_t)c0 * 2 * L) << logn);
+    launch_encrypt_pk(uee, c, dst, n, lv.ctx_ids, par->d_limbs, logn, st);
+    if (pts) add_to_poly(par, lv, pts, c0, n, dst, ws, st);
+  });
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
   API_END
 }
 
@@ -1983,10 +2097,7 @@ int fhe_b200_switch_down(fhe_b200_batch* b, void* stream) {
   // transform writes them back, compacted, at the start of the batch's own allocation (which keeps its size: the
   // pointer handed out by fhe_b200_batch_device_ptr stays valid, nothing is allocated, freed or synchronised here).
   Workspace ws(par, st);
-  u64* tmp = ws.words((size_t)polys * nl.L << par->logn);
-  launch_ntt(b->d, b->d, polys * lv.L, lv.ctx_ids, par->d_limbs, par->logn, true, 1, false, st);
-  launch_switch_down(lv.sd, b->d, tmp, polys, lv.L, lv.ctx_ids, par->d_limbs, par->logn, st);
-  launch_ntt(tmp, b->d, polys * nl.L, nl.ctx_ids, par->d_limbs, par->logn, false, 1, false, st);
+  switch_down_polys(par, b->level, b->d, polys, ws, st);
   FHE_CUDA(cudaGetLastError());
   b->level += 1;
   b->limbs = nl.L;

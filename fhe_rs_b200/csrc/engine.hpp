@@ -207,6 +207,22 @@ void launch_center(u64* x, size_t n_words, u64 t, cudaStream_t st);
 void launch_noise(const u64* x, u32* out, u32 cts, u32 L, const u64* garner, const u64* q_words, u32 W,
                   const LimbDev* limbs, u32 logn, cudaStream_t st);
 
+// ---- encryption (keys/secret_key.rs:100-136, keys/public_key.rs:45-92) from the seeded ChaCha20 stream of
+// include/fhe_b200.h; ct_base is the call-wide index of the first ciphertext (state word 13)
+struct EncSeed {
+  u32 w[8];   // the 32-byte seed as eight little-endian words (state words 4..11)
+};
+// out [cts][2][L][N]: part 1 = a (role 0, uniform NTT words), part 0 = e - a*s; e [cts][L][N] NTT; s row j at s + j*N
+void launch_encrypt_sk(const u64* s, const u64* e, u64* out, u32 cts, u32 ct_base, const EncSeed& K, const RowIds& ids,
+                       const LimbDev* limbs, u32 logn, cudaStream_t st);
+// out [cts][n_roles][L][N]: the centred binomial polynomial of roles role0 .. role0 + n_roles - 1 (drawn from limb 0's
+// row) as canonical residues in every limb; variance 1..32
+void launch_cbd(u64* out, u32 cts, u32 ct_base, u32 role0, u32 n_roles, u32 variance, const EncSeed& K,
+                const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st);
+// out [cts][2][L][N] = (u*pk0 + e1, u*pk1 + e2); uee [cts][3][L][N] = (u, e1, e2), pk [2][L][N], all NTT
+void launch_encrypt_pk(const u64* uee, const u64* pk, u64* out, u32 cts, const RowIds& ids, const LimbDev* limbs,
+                       u32 logn, cudaStream_t st);
+
 // bit (un)packing of power-basis rows (fhe-util/src/lib.rs:71-146): row r of `rows` uses nbits[r % limbs] bits per
 // coefficient; packed row r starts at byte  (r / limbs) * poly_bytes + offs[r % limbs]
 struct PackDev {

@@ -1176,6 +1176,146 @@ __global__ void __launch_bounds__(256) noise_kernel(NoiseArgs A) {
   }
 }
 
+// ------------------------------------------------------------------ encryption (keys/secret_key.rs:100-136,
+// keys/public_key.rs:45-92).  The random words come from the seeded ChaCha20 stream of include/fhe_b200.h: block b of
+// the row (ciphertext ct, role, limb) is the RFC 8439 block function of the state (constants, seed, b, ct,
+// role << 8 | limb, 0); value m of the block (u64 words 2m, 2m + 1) drives coefficient 4b + m.
+__device__ __forceinline__ void chacha_qr(u32& a, u32& b, u32& c, u32& d) {
+  a += b; d = __funnelshift_l(d ^ a, d ^ a, 16);
+  c += d; b = __funnelshift_l(b ^ c, b ^ c, 12);
+  a += b; d = __funnelshift_l(d ^ a, d ^ a, 8);
+  c += d; b = __funnelshift_l(b ^ c, b ^ c, 7);
+}
+// the four 128-bit values (lo[m], hi[m]) of one block
+__device__ __forceinline__ void chacha_block(const EncSeed& K, u32 b, u32 ct, u32 role_limb, u64 (&lo)[4],
+                                             u64 (&hi)[4]) {
+  const u32 in[16] = {0x61707865u, 0x3320646eu, 0x79622d32u, 0x6b206574u, K.w[0], K.w[1], K.w[2], K.w[3],
+                      K.w[4],      K.w[5],      K.w[6],      K.w[7],      b,      ct,     role_limb, 0u};
+  u32 x[16];
+#pragma unroll
+  for (int i = 0; i < 16; i++) x[i] = in[i];
+#pragma unroll 2
+  for (int r = 0; r < 10; r++) {
+    chacha_qr(x[0], x[4], x[8], x[12]);
+    chacha_qr(x[1], x[5], x[9], x[13]);
+    chacha_qr(x[2], x[6], x[10], x[14]);
+    chacha_qr(x[3], x[7], x[11], x[15]);
+    chacha_qr(x[0], x[5], x[10], x[15]);
+    chacha_qr(x[1], x[6], x[11], x[12]);
+    chacha_qr(x[2], x[7], x[8], x[13]);
+    chacha_qr(x[3], x[4], x[9], x[14]);
+  }
+#pragma unroll
+  for (int m = 0; m < 4; m++) {
+    lo[m] = (u64)(x[4 * m] + in[4 * m]) | ((u64)(x[4 * m + 1] + in[4 * m + 1]) << 32);
+    hi[m] = (u64)(x[4 * m + 2] + in[4 * m + 2]) | ((u64)(x[4 * m + 3] + in[4 * m + 3]) << 32);
+  }
+}
+
+struct EncSkArgs {
+  const u64* s;       // row j: s modulo the j-th limb (NTT)
+  const u64* e;       // [cts][L][N] NTT of the error
+  u64* out;           // [cts][2][L][N]
+  EncSeed K;
+  u32 cts, ct_base, logn, limbs_per_poly;
+  const LimbDev* limbs;
+  unsigned short ids[kMaxPos];
+};
+// SecretKey::encrypt_poly up to + m: a = (hi 2^64 + lo) mod q_j drawn as NTT words (Poly::random_from_seed into Ntt),
+// part 1 = a, part 0 = e - a s.  One thread per (ciphertext, limb, 4 coefficients): a never leaves the registers.  No
+// branch depends on the data.
+__global__ void encrypt_sk_kernel(EncSkArgs A) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const u32 g_per_row = 1u << (A.logn - 2);
+  const size_t total = (size_t)A.cts * A.limbs_per_poly * g_per_row;
+  if (idx >= total) return;
+  const u32 g = (u32)(idx % g_per_row);
+  const size_t row = idx / g_per_row;
+  const u32 j = (u32)(row % A.limbs_per_poly), ct = (u32)(row / A.limbs_per_poly);
+  const LimbDev& M = A.limbs[A.ids[j]];
+  u64 lo[4], hi[4];
+  chacha_block(A.K, g, A.ct_base + ct, j, lo, hi);   // role 0 (a), limb j
+  const size_t c = (size_t)g * 4;
+  const ulonglong2* sp = reinterpret_cast<const ulonglong2*>(A.s + ((size_t)j << A.logn) + c);
+  const ulonglong2* ep = reinterpret_cast<const ulonglong2*>(A.e + (row << A.logn) + c);
+  const ulonglong2 s01 = sp[0], s23 = sp[1], e01 = ep[0], e23 = ep[1];
+  const u64 s[4] = {s01.x, s01.y, s23.x, s23.y}, e[4] = {e01.x, e01.y, e23.x, e23.y};
+  u64 a[4], b[4];
+#pragma unroll
+  for (int m = 0; m < 4; m++) {
+    a[m] = reduce128_limb(lo[m], hi[m], M);
+    b[m] = csub(e[m] + M.p - mulmod_limb(a[m], s[m], M), M.p);
+  }
+  const size_t stride = (size_t)A.limbs_per_poly << A.logn;
+  u64* b_row = A.out + (size_t)ct * 2 * stride + ((size_t)j << A.logn) + c;
+  reinterpret_cast<ulonglong2*>(b_row)[0] = make_ulonglong2(b[0], b[1]);
+  reinterpret_cast<ulonglong2*>(b_row)[1] = make_ulonglong2(b[2], b[3]);
+  reinterpret_cast<ulonglong2*>(b_row + stride)[0] = make_ulonglong2(a[0], a[1]);
+  reinterpret_cast<ulonglong2*>(b_row + stride)[1] = make_ulonglong2(a[2], a[3]);
+}
+
+struct CbdArgs {
+  u64* out;           // [cts][n_roles][L][N]
+  EncSeed K;
+  u64 add_lo, add_hi, sub_lo, sub_hi;   // mask_add = low 2 variance bits, mask_sub = the next 2 variance bits
+  u32 cts, ct_base, role0, n_roles, logn, limbs_per_poly;
+  const LimbDev* limbs;
+  unsigned short ids[kMaxPos];
+};
+// Poly::small (rq/mod.rs, fhe-util sample_vec_cbd): x = popc(v & mask_add) - popc(v & mask_sub) on the 128-bit value
+// of the (ct, role, limb 0) row, written as its canonical residue into every limb of the level (q_j - |x| for x < 0,
+// by a select).  One thread per (ciphertext, role, 4 coefficients).
+__global__ void cbd_kernel(CbdArgs A) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const u32 g_per_row = 1u << (A.logn - 2);
+  const size_t total = (size_t)A.cts * A.n_roles * g_per_row;
+  if (idx >= total) return;
+  const u32 g = (u32)(idx % g_per_row);
+  const size_t poly = idx / g_per_row;
+  const u32 r = (u32)(poly % A.n_roles), ct = (u32)(poly / A.n_roles);
+  u64 lo[4], hi[4];
+  chacha_block(A.K, g, A.ct_base + ct, (A.role0 + r) << 8, lo, hi);
+  long long x[4];
+#pragma unroll
+  for (int m = 0; m < 4; m++)
+    x[m] = (long long)(__popcll(lo[m] & A.add_lo) + __popcll(hi[m] & A.add_hi)) -
+           (long long)(__popcll(lo[m] & A.sub_lo) + __popcll(hi[m] & A.sub_hi));
+  const size_t c = (size_t)g * 4;
+  u64* dst = A.out + ((poly * A.limbs_per_poly) << A.logn) + c;
+  for (u32 j = 0; j < A.limbs_per_poly; j++) {
+    const u64 p = A.limbs[A.ids[j]].p;
+    u64 w[4];
+#pragma unroll
+    for (int m = 0; m < 4; m++) w[m] = (u64)x[m] + (p & (u64)(x[m] >> 63));
+    reinterpret_cast<ulonglong2*>(dst)[0] = make_ulonglong2(w[0], w[1]);
+    reinterpret_cast<ulonglong2*>(dst)[1] = make_ulonglong2(w[2], w[3]);
+    dst += (size_t)1 << A.logn;
+  }
+}
+
+struct EncPkArgs {
+  const u64* uee;     // [cts][3][L][N]: u, e1, e2 (NTT)
+  const u64* pk;      // [2][L][N] (NTT, at the level)
+  u64* out;           // [cts][2][L][N]
+  u32 cts, logn, limbs_per_poly;
+  const LimbDev* limbs;
+  unsigned short ids[kMaxPos];
+};
+// PublicKey::try_encrypt up to + m: c0 = u pk0 + e1, c1 = u pk1 + e2, one coefficient per thread
+__global__ void encrypt_pk_kernel(EncPkArgs A) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t stride = (size_t)A.limbs_per_poly << A.logn;
+  if (idx >= (size_t)A.cts * stride) return;
+  const size_t ct = idx / stride, in_ct = idx % stride;
+  const u32 j = (u32)(in_ct >> A.logn);
+  const LimbDev& M = A.limbs[A.ids[j]];
+  const u64* src = A.uee + ct * 3 * stride + in_ct;
+  const u64 u = src[0], e1 = src[stride], e2 = src[2 * stride];
+  u64* dst = A.out + ct * 2 * stride + in_ct;
+  dst[0] = csub(mulmod_limb(u, A.pk[in_ct], M) + e1, M.p);
+  dst[stride] = csub(mulmod_limb(u, A.pk[stride + in_ct], M) + e2, M.p);
+}
+
 void copy_ids(unsigned short* dst, const RowIds& ids) {
   for (int i = 0; i < kMaxPos; i++) dst[i] = ids.ids[i];
 }
@@ -1242,6 +1382,45 @@ void launch_noise(const u64* x, u32* out, u32 cts, u32 L, const u64* garner, con
   A.x = x; A.out = out; A.garner = garner; A.q_words = q_words; A.L = L; A.W = W; A.logn = logn; A.limbs = limbs;
   const u32 N = 1u << logn;
   noise_kernel<<<dim3((N + 255) / 256, cts), 256, 0, st>>>(A);
+  g_launches++;
+}
+
+void launch_encrypt_sk(const u64* s, const u64* e, u64* out, u32 cts, u32 ct_base, const EncSeed& K, const RowIds& ids,
+                       const LimbDev* limbs, u32 logn, cudaStream_t st) {
+  EncSkArgs A;
+  A.s = s; A.e = e; A.out = out; A.K = K; A.cts = cts; A.ct_base = ct_base; A.logn = logn;
+  A.limbs_per_poly = ids.limbs_per_poly; A.limbs = limbs;
+  copy_ids(A.ids, ids);
+  const size_t total = ((size_t)cts * ids.limbs_per_poly) << (logn - 2);
+  if (!total) return;
+  encrypt_sk_kernel<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(A);
+  g_launches++;
+}
+
+void launch_cbd(u64* out, u32 cts, u32 ct_base, u32 role0, u32 n_roles, u32 variance, const EncSeed& K,
+                const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st) {
+  CbdArgs A;
+  const u128 add = (((u128)1) << (2 * variance)) - 1;   // variance <= 32: 2 variance <= 64 bits each
+  const u128 sub = add << (2 * variance);
+  A.add_lo = (u64)add; A.add_hi = (u64)(add >> 64); A.sub_lo = (u64)sub; A.sub_hi = (u64)(sub >> 64);
+  A.out = out; A.K = K; A.cts = cts; A.ct_base = ct_base; A.role0 = role0; A.n_roles = n_roles; A.logn = logn;
+  A.limbs_per_poly = ids.limbs_per_poly; A.limbs = limbs;
+  copy_ids(A.ids, ids);
+  const size_t total = ((size_t)cts * n_roles) << (logn - 2);
+  if (!total) return;
+  cbd_kernel<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(A);
+  g_launches++;
+}
+
+void launch_encrypt_pk(const u64* uee, const u64* pk, u64* out, u32 cts, const RowIds& ids, const LimbDev* limbs,
+                       u32 logn, cudaStream_t st) {
+  EncPkArgs A;
+  A.uee = uee; A.pk = pk; A.out = out; A.cts = cts; A.logn = logn; A.limbs_per_poly = ids.limbs_per_poly;
+  A.limbs = limbs;
+  copy_ids(A.ids, ids);
+  const size_t total = ((size_t)cts * ids.limbs_per_poly) << logn;
+  if (!total) return;
+  encrypt_pk_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(A);
   g_launches++;
 }
 

@@ -315,6 +315,20 @@ def decode_rgsw(data: Bytes) -> Tuple[memoryview, memoryview]:  # rgsw_ciphertex
     return f[1], f[2]
 
 
+def encode_public_key(ciphertext: Bytes) -> bytes:         # public_key.rs:95-107, bfv.proto:50-52
+    out: List[Bytes] = []
+    _put_len(out, 1, ciphertext)
+    return _join(out)
+
+
+def decode_public_key(data: Bytes) -> memoryview:           # public_key.rs:109-149
+    """the encoded Ciphertext inside a PublicKey message"""
+    f = _sub_messages(data, (1,))
+    if f[1] is None:
+        raise WireError("MissingField", detail="PublicKeyCiphertext")
+    return f[1]
+
+
 # ------------------------------------------------------------------------------------------ SecretKey
 def _zigzag(n: int) -> int:
     return ((n << 1) ^ (n >> 63)) & 0xFFFFFFFFFFFFFFFF

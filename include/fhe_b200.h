@@ -240,6 +240,46 @@ int fhe_b200_decode(const fhe_b200_encoder* e, int encoding, int is_signed, cons
  * time, as the reference's (unsafe) function.  Errors: as fhe_b200_decrypt; t >= q_0 -> UNSUPPORTED. */
 int fhe_b200_measure_noise(const fhe_b200_secret_key* sk, const fhe_b200_batch* ct, uint32_t* noise_bits, void* stream);
 
+/* ---- encryption ----------------------------------------------------------------------------------
+ * The random words come from a seeded ChaCha20 stream that this library defines (the reference draws from rand::rng()
+ * and a caller-supplied rng, secret_key.rs:100-136, public_key.rs:45-92, so no host depends on which words are drawn;
+ * what it depends on is their distribution and the algebra built on them).  Block b of a row is the RFC 8439 block
+ * function (20 rounds) of the state
+ *     words 0..3   "expand 32-byte k"
+ *     words 4..11  the 32-byte seed as eight little-endian u32
+ *     word 12      b, the block index within the row
+ *     word 13      the index of the ciphertext within the call (0 .. out.count - 1)
+ *     word 14      role << 8 | limb: role 0 = a, 1 = e (secret-key encryption), 2 = u, 3 = e1, 4 = e2 (public-key
+ *                  encryption); the small polynomials use limb 0
+ *     word 15      0
+ * Each block is addressed only by its position, so the words do not depend on chunking or streams.  One 64-byte block
+ * gives four 128-bit values: value m is u64 words 2m (low) and 2m + 1 (high) of the block, and coefficient 4b + m of
+ * the row takes value m of block b.
+ *  - a (uniform, drawn directly as NTT words like Poly::random_from_seed into Ntt): (hi 2^64 + lo) mod q_j.  Its
+ *    statistical distance from uniform is below q_j / 2^128 <= 2^-66 per word (the reference samples exactly).
+ *  - e, u, e1, e2 (centred binomial, sample_vec_cbd, fhe-util/src/lib.rs:22-67): popc(v & mask_add) - popc(v & mask_sub)
+ *    of the 128-bit value v, mask_add the low 2 variance bits and mask_sub the next 2 variance bits.  Same distribution
+ *    as the reference for every variance in 1..32 (which reads its bits differently).
+ * seed: 32 bytes of fresh entropy per call (a Rust host passes OsRng bytes); reusing a seed repeats a and the errors
+ * and breaks security.  variance: BfvParameters::variance, 1..32 (reference default 10).  Both calls write out whole
+ * (2-part NTT batch) and are only enqueued.  Scratch holding e, u, e1, e2 or the plaintext is zeroed before it goes
+ * back to the pool; the kernels have no branch that depends on the data.
+ * Errors: variance outside 1..32 (InvalidVariance), a NULL key, seed or out, out not 2-part, pts not 1-part or with a
+ * count other than out.count -> INVALID_ARGUMENT; a batch of another parameter set or over the multiplication basis ->
+ * CONTEXT_MISMATCH; pts at another level than out -> INVALID_LEVEL; power-basis pts -> INVALID_REPRESENTATION;
+ * t >= q_0 (as fhe_b200_add_plain_batch's to_poly) -> UNSUPPORTED. */
+/* SecretKey::try_encrypt (secret_key.rs:100-136, :181-193) into out: b = e - a s + to_poly(m), a.  pts: a 1-part NTT
+ * batch from fhe_b200_encode (one plaintext per output ciphertext, at out's level), or NULL to encrypt zeros at out's
+ * level (PublicKey::new, public_key.rs:26-38: a 1 x 2 batch at level 0 is then the public key's c). */
+int fhe_b200_encrypt_sk(const fhe_b200_secret_key* sk, const fhe_b200_batch* pts, uint32_t variance,
+                        const uint8_t* seed, fhe_b200_batch* out, void* stream);
+/* PublicKey::try_encrypt (public_key.rs:45-92) into out: (u pk0 + e1 + to_poly(m), u pk1 + e2).  pk: the public key's
+ * c as a 1-ciphertext, 2-part, level-0 NTT batch, switched down to out's level on every call as the reference does;
+ * pts as for fhe_b200_encrypt_sk.  Extra errors: pk not at level 0 -> INVALID_LEVEL (InvalidPublicKeyLevel); pk not
+ * one 2-part ciphertext -> INVALID_ARGUMENT; power-basis pk -> INVALID_REPRESENTATION. */
+int fhe_b200_encrypt_pk(const fhe_b200_batch* pk, const fhe_b200_batch* pts, uint32_t variance, const uint8_t* seed,
+                        fhe_b200_batch* out, void* stream);
+
 /* &Ciphertext * &Ciphertext (bfv/ops/mod.rs:259-358): n parts x m parts -> n + m - 1 parts (out3 must have that many;
  * 2 x 2 -> 3 is the fused path) */
 int fhe_b200_mul(const fhe_b200_batch* a, const fhe_b200_batch* b, fhe_b200_batch* out3, void* stream);

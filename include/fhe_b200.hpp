@@ -9,11 +9,13 @@
 //   bfv::GaloisKey / EvaluationKey              bfv/keys/galois_key.rs:18, evaluation_key.rs:110-170
 //   bfv::Multiplicator                          bfv/ops/mul.rs:22
 //   bfv::Encoding / Plaintext / PlaintextVec    bfv/encoding.rs, bfv/plaintext.rs:20, plaintext_vec.rs:20
-//   bfv::SecretKey (decryption, measure_noise)  bfv/keys/secret_key.rs:25 (key generation and encryption stay client-side)
+//   bfv::SecretKey / PublicKey                  bfv/keys/secret_key.rs:25, public_key.rs:17 (encryption, decryption,
+//                                               measure_noise; key generation stays client-side)
 // Fallible reference calls return Result<_, fhe::Error>; here they throw fhe_b200::Error carrying
 // the fhe_b200_status code (same variants, see fhe_b200.h).
 #pragma once
 #include <cstdint>
+#include <cstring>
 #include <map>
 #include <algorithm>
 #include <memory>
@@ -23,6 +25,8 @@
 #include <type_traits>
 #include <utility>
 #include <vector>
+
+#include <sys/random.h>
 
 #include "fhe_b200.h"
 
@@ -51,6 +55,8 @@ class BfvParameters {
     return m;
   }
   size_t max_level() const { return fhe_b200_params_n_moduli(h_) - 1; }
+  // BfvParameters::variance (parameters.rs:98-99): the centred binomial parameter of encryption's errors
+  uint32_t variance() const { return variance_; }
   std::vector<uint64_t> mul_basis(uint32_t level) const {
     uint32_t n = 0;
     check(fhe_b200_params_mul_basis(h_, level, nullptr, &n));
@@ -69,11 +75,12 @@ class BfvParameters {
 
  private:
   friend class BfvParametersBuilder;
-  BfvParameters(fhe_b200_params* h, bool has_psi_t, uint64_t psi_t)
-      : h_(h), has_plaintext_psi_(has_psi_t), plaintext_psi_(psi_t) {}
+  BfvParameters(fhe_b200_params* h, bool has_psi_t, uint64_t psi_t, uint32_t variance)
+      : h_(h), has_plaintext_psi_(has_psi_t), plaintext_psi_(psi_t), variance_(variance) {}
   fhe_b200_params* h_;
   bool has_plaintext_psi_;
   uint64_t plaintext_psi_;
+  uint32_t variance_;
   mutable std::once_flag enc_once_;
   mutable fhe_b200_encoder* enc_ = nullptr;
 
@@ -89,6 +96,8 @@ class BfvParametersBuilder {
   BfvParametersBuilder& set_moduli_sizes(const std::vector<uint32_t>& s) { sizes_ = s; return *this; }
   BfvParametersBuilder& set_ntt_roots(const std::vector<uint64_t>& psi) { psi_ = psi; return *this; }
   BfvParametersBuilder& set_device(int device) { device_ = device; return *this; }
+  // the error variance, 1..32 (parameters.rs:384-388; build throws InvalidVariance outside)
+  BfvParametersBuilder& set_variance(uint32_t v) { variance_ = v; return *this; }
   // 2N-th root for the plaintext modulus (the reference's NttOperator::new(t).omegas[N/2]); default rule otherwise
   BfvParametersBuilder& set_plaintext_ntt_root(uint64_t psi_t) { psi_t_ = psi_t; has_psi_t_ = true; return *this; }
   // BfvParametersBuilder::build_arc (bfv/parameters.rs:555)
@@ -96,6 +105,7 @@ class BfvParametersBuilder {
     uint8_t pt[8];
     for (int i = 0; i < 8; i++) pt[i] = (uint8_t)(plaintext_ >> (8 * i));
     fhe_b200_params* h = nullptr;
+    if (variance_ < 1 || variance_ > 32) throw Error(FHE_B200_INVALID_ARGUMENT, "InvalidVariance");
     if (!moduli_.empty() && !sizes_.empty())
       throw Error(FHE_B200_INVALID_ARGUMENT, "ConflictingCiphertextModulusSpecifications");
     if (!moduli_.empty())
@@ -103,7 +113,7 @@ class BfvParametersBuilder {
                                    psi_.empty() ? nullptr : psi_.data(), &h));
     else
       check(fhe_b200_params_create_from_sizes(device_, degree_, sizes_.data(), (uint32_t)sizes_.size(), pt, 8, &h));
-    return std::shared_ptr<BfvParameters>(new BfvParameters(h, has_psi_t_, psi_t_));
+    return std::shared_ptr<BfvParameters>(new BfvParameters(h, has_psi_t_, psi_t_, variance_));
   }
 
  private:
@@ -111,6 +121,7 @@ class BfvParametersBuilder {
   uint64_t plaintext_ = 0;
   uint64_t psi_t_ = 0;
   bool has_psi_t_ = false;
+  uint32_t variance_ = 10;
   std::vector<uint64_t> moduli_, psi_;
   std::vector<uint32_t> sizes_;
   int device_ = 0;
@@ -373,6 +384,15 @@ class SecretKey {
     volatile int64_t* c = coeffs_.data();
     for (size_t i = 0; i < coeffs_.size(); i++) c[i] = 0;
   }
+  // SecretKey::try_encrypt (secret_key.rs:100-136, :181-193) of every plaintext of pts: one fresh ciphertext per
+  // plaintext at their level.  seed: the 32 bytes keying the stream of fhe_b200.h (nullptr: fresh getrandom bytes).
+  Ciphertext try_encrypt(const PlaintextVec& pts, const uint8_t* seed = nullptr) const {
+    return encrypt_into(&pts.batch(), pts.len(), pts.batch().level(), seed, pts.batch().stream());
+  }
+  // `count` encryptions of zero at `level` (PublicKey::new takes one at level 0)
+  Ciphertext try_encrypt_zero(uint32_t count, uint32_t level, const uint8_t* seed = nullptr) const {
+    return encrypt_into(nullptr, count, level, seed, nullptr);
+  }
   // SecretKey::try_decrypt (secret_key.rs:198-260) of every ciphertext of the batch: plaintexts without an encoding
   PlaintextVec try_decrypt(const Ciphertext& ct) const {
     Ciphertext out(par_, ct.count(), 1, ct.level(), Representation::Ntt, ct.stream());
@@ -390,9 +410,58 @@ class SecretKey {
   const std::shared_ptr<BfvParameters>& par() const { return par_; }
 
  private:
+  Ciphertext encrypt_into(const Ciphertext* pts, uint32_t count, uint32_t level, const uint8_t* seed, void* stream) const;
   std::shared_ptr<BfvParameters> par_;
   std::vector<int64_t> coeffs_;
   fhe_b200_secret_key* h_ = nullptr;
+};
+
+// 32 bytes of fresh entropy for one encryption call (getrandom(2), the system CSPRNG)
+struct EncryptionSeed {
+  uint8_t bytes[32];
+  explicit EncryptionSeed(const uint8_t* given) {
+    if (given) { std::memcpy(bytes, given, 32); return; }
+    for (size_t got = 0; got < 32;) {
+      const ssize_t r = getrandom(bytes + got, 32 - got, 0);
+      if (r < 0) throw Error(FHE_B200_INVALID_ARGUMENT, "getrandom failed");
+      got += (size_t)r;
+    }
+  }
+};
+
+inline Ciphertext SecretKey::encrypt_into(const Ciphertext* pts, uint32_t count, uint32_t level, const uint8_t* seed,
+                                          void* stream) const {
+  const EncryptionSeed s(seed);
+  Ciphertext out(par_, count, 2, level, Representation::Ntt, stream);
+  check(fhe_b200_encrypt_sk(h_, pts ? pts->handle() : nullptr, par_->variance(), s.bytes, out.handle(), stream));
+  return out;
+}
+
+// fhe::bfv::PublicKey (keys/public_key.rs:17-22): its c, one 2-part ciphertext at level 0, on the device
+class PublicKey {
+ public:
+  PublicKey(std::shared_ptr<BfvParameters> par, Ciphertext c) : par_(std::move(par)), c_(std::move(c)) {
+    if (c_.count() != 1 || c_.len() != 2) throw Error(FHE_B200_INVALID_ARGUMENT, "a public key is one 2-part ciphertext");
+    if (c_.level() != 0) throw Error(FHE_B200_INVALID_LEVEL, "InvalidPublicKeyLevel");
+  }
+  // PublicKey::new (public_key.rs:26-38): a secret-key encryption of zero at level 0
+  static PublicKey new_key(const SecretKey& sk, const uint8_t* seed = nullptr) {
+    return PublicKey(sk.par(), sk.try_encrypt_zero(1, 0, seed));
+  }
+  // PublicKey::try_encrypt (public_key.rs:45-92) of every plaintext of pts, as SecretKey::try_encrypt
+  Ciphertext try_encrypt(const PlaintextVec& pts, const uint8_t* seed = nullptr) const {
+    const EncryptionSeed s(seed);
+    void* stream = pts.batch().stream();
+    Ciphertext out(par_, pts.len(), 2, pts.batch().level(), Representation::Ntt, stream);
+    check(fhe_b200_encrypt_pk(c_.handle(), pts.batch().handle(), par_->variance(), s.bytes, out.handle(), stream));
+    return out;
+  }
+  const Ciphertext& c() const { return c_; }
+  const std::shared_ptr<BfvParameters>& par() const { return par_; }
+
+ private:
+  std::shared_ptr<BfvParameters> par_;
+  Ciphertext c_;
 };
 
 class KeySwitchingKey {

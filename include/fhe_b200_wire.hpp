@@ -7,6 +7,7 @@
 //   fhers.bfv.RelinearizationKey  bfv.proto:25-27 (keys/relinearization_key.rs:113-135), GaloisKey :29-32
 //                                 (keys/galois_key.rs:146-173)
 //   fhers.bfv.SecretKey           bfv.proto:54-56,                   fhe/src/bfv/keys/secret_key.rs:142-175
+//   fhers.bfv.PublicKey           bfv.proto:50-52,                   fhe/src/bfv/keys/public_key.rs:95-149
 // `Rq.coefficients` -- the bit-packed power-basis words, all but a few bytes of every message -- is produced and consumed
 // on the device (fhe_b200_batch_pack / fhe_b200_batch_unpack); this header is the proto3 framing around it, emitting
 // what prost emits (fields in field-number order, zero scalars and empty singular `bytes` omitted) and accepting what
@@ -290,6 +291,12 @@ inline std::vector<int64_t> decode_secret_key(const void* data, size_t n, size_t
   return c;
 }
 
+inline std::string encode_public_key(const std::string& ciphertext) {   // public_key.rs:95-107, bfv.proto:50-52
+  std::string out;
+  put_len(out, 1, ciphertext);
+  return out;
+}
+
 // sub-message `field` of a wrapper message; *scalar2 = varint field 2 when present
 inline Span sub_message(const void* data, size_t n, uint32_t field, const char* missing, uint32_t* scalar2 = nullptr) {
   Span s;
@@ -448,6 +455,22 @@ inline std::unique_ptr<SecretKey> secret_key_from_bytes(std::shared_ptr<BfvParam
   volatile int64_t* w = c.data();
   for (size_t i = 0; i < c.size(); i++) w[i] = 0;
   return sk;
+}
+
+// PublicKey::to_bytes (public_key.rs:95-107): both parts (a device-encrypted key carries no seed)
+inline std::string to_bytes(const PublicKey& pk) { return wire::encode_public_key(to_bytes(pk.c())[0]); }
+// PublicKey::from_bytes (public_key.rs:109-149).  The reference writes a compact message (c0 and the seed of c1):
+// decoding one needs seeded_c1, the [limbs][N] NTT words of c1 expanded by the Rust host.  A key at a level other than
+// 0 is InvalidPublicKeyLevel.
+inline PublicKey public_key_from_bytes(std::shared_ptr<BfvParameters> par, const std::string& data,
+                                       const uint64_t* seeded_c1 = nullptr) {
+  wire::Span s = wire::sub_message(data.data(), data.size(), 1, "PublicKeyCiphertext");
+  const wire::CiphertextMsg m = wire::decode_ciphertext(s.p, s.n);
+  if (m.level != 0) throw WireError("InvalidPublicKeyLevel", FHE_B200_INVALID_LEVEL);
+  if (m.seed.n && !seeded_c1)
+    throw WireError("SeedExpansion", FHE_B200_UNSUPPORTED, "pass the host-expanded c1 (ciphertext.rs:287-300)");
+  Ciphertext c = ciphertext_from_bytes(par, {std::string((const char*)s.p, s.n)}, seeded_c1);
+  return PublicKey(std::move(par), std::move(c));
 }
 
 }  // namespace bfv
