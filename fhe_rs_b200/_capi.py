@@ -49,6 +49,7 @@ SYMBOLS = {
     "fhe_b200_batch_device_ptr": (_i, [_vp, _pp, C.POINTER(C.c_size_t)]),
     "fhe_b200_ksk_upload": (_i, [_vp, _u32, _u32, _vp, _vp, _u32, _pp]),
     "fhe_b200_ksk_free": (_i, [_vp]),
+    "fhe_b200_ksk_download": (_i, [_vp, _vp, _vp, _vp]),
     "fhe_b200_ntt_forward": (_i, [_vp, _vp]),
     "fhe_b200_ntt_backward": (_i, [_vp, _vp]),
     "fhe_b200_add": (_i, [_vp, _vp, _vp]),
@@ -69,6 +70,9 @@ SYMBOLS = {
     "fhe_b200_measure_noise": (_i, [_vp, _vp, _vp, _vp]),
     "fhe_b200_encrypt_sk": (_i, [_vp, _vp, _u32, _vp, _vp, _vp]),
     "fhe_b200_encrypt_pk": (_i, [_vp, _vp, _u32, _vp, _vp, _vp]),
+    "fhe_b200_relin_key_generate": (_i, [_vp, _u32, _u32, _u32, _vp, _pp, _vp]),
+    "fhe_b200_galois_keys_generate": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _vp, _pp, _vp]),
+    "fhe_b200_rgsw_encrypt": (_i, [_vp, _vp, _u32, _vp, _pp, _vp]),
     "fhe_b200_mul": (_i, [_vp, _vp, _vp, _vp]),
     "fhe_b200_relinearize": (_i, [_vp, _vp, _vp, _vp]),
     "fhe_b200_mul_relin": (_i, [_vp, _vp, _vp, _i, _vp, _vp]),

@@ -6,14 +6,14 @@ Same names, argument meaning and error behaviour as the reference items cited in
 docstring (paths relative to /root/reference/crates).  Differences forced by the device:
 a `Ciphertext` here is a *batch* of ciphertexts of one level resident in HBM (the reference's
 operators act on one ciphertext; per-ciphertext FFI would be launch/PCIe bound, SURVEY 8b),
-and keys are constructed from their NTT-domain words (as after deserialization,
-key_switching_key.rs:418-482) -- key generation is client-side code outside this path.
+and keys are either generated on the device from a SecretKey and a seeded ChaCha20 stream or constructed from
+their NTT-domain words (as after deserialization, key_switching_key.rs:418-482).
 No CPU fallback exists: every operation is a CUDA launch behind the C ABI."""
 from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Dict, Optional, Sequence
+from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
@@ -23,7 +23,7 @@ from .wire import WireError
 
 __all__ = ["BfvParameters", "BfvParametersBuilder", "Ciphertext", "KeySwitchingKey", "RelinearizationKey", "RGSWCiphertext",
            "GaloisKey", "EvaluationKey", "Multiplicator", "ScalingFactor", "dot_product_scalar", "FheError", "WireError", "NTT", "POWER_BASIS",
-           "Encoding", "Plaintext", "PlaintextVec", "SecretKey", "PublicKey"]
+           "Encoding", "Plaintext", "PlaintextVec", "SecretKey", "PublicKey", "EvaluationKeyBuilder"]
 
 
 def _release(free_name: str, handle) -> None:
@@ -614,8 +614,9 @@ class PlaintextVec:
 class SecretKey:
     """fhe::bfv::SecretKey (keys/secret_key.rs:25-53) on the device, from its N signed coefficients.  Encryption,
     decryption and noise measurement run on the device; the device copy of s is erased when the key is released.
-    Encryption draws its randomness from the seeded ChaCha20 stream of include/fhe_b200.h.  Key generation (the
-    coefficients themselves, relinearization and Galois keys) stays with the client."""
+    Encryption and key generation (RelinearizationKey.new, GaloisKey.new, EvaluationKeyBuilder, try_encrypt_rgsw) draw
+    their randomness from the seeded ChaCha20 stream of include/fhe_b200.h.  The coefficients themselves
+    (SecretKey::random) come from the client."""
 
     def __init__(self, par: BfvParameters, coeffs):
         c = np.array(coeffs, dtype=np.int64)   # our own copy, kept for to_bytes (the reference keeps SecretKey.coeffs)
@@ -648,6 +649,16 @@ class SecretKey:
         seed: the 32 bytes that key the stream; None draws os.urandom(32) (a seed must never be reused)."""
         return _encrypt(_capi.lib().fhe_b200_encrypt_sk, self._h, self.par, pts, seed, count, level)
 
+    def try_encrypt_rgsw(self, pts: PlaintextVec, seed: Optional[bytes] = None) -> "List[RGSWCiphertext]":
+        """SecretKey::try_encrypt into an RGSWCiphertext (rgsw_ciphertext.rs:94-120) of every plaintext of `pts`, at
+        the plaintexts' level, in one device call.  seed as for try_encrypt."""
+        b = pts.batch
+        hs = (C.c_void_p * (2 * b.count))()
+        check(_capi.lib().fhe_b200_rgsw_encrypt(self._h, b._h, self.par.variance, _seed(seed),
+                                                C.cast(hs, C.POINTER(C.c_void_p)), b.stream))
+        k = [KeySwitchingKey._adopt(self.par, h, b.level, b.level, b.stream) for h in hs]
+        return [RGSWCiphertext(k[2 * p], k[2 * p + 1]) for p in range(b.count)]
+
     def try_decrypt(self, ct: Ciphertext) -> PlaintextVec:
         """SecretKey::try_decrypt (secret_key.rs:198-260) of every ciphertext of the batch: plaintexts with no
         encoding (decode them with try_decode(encoding))."""
@@ -663,11 +674,17 @@ class SecretKey:
         return out
 
 
-def _encrypt(fn, key, par: BfvParameters, pts: Optional[PlaintextVec], seed: Optional[bytes], count: int,
-             level: int) -> Ciphertext:
+def _seed(seed: Optional[bytes]) -> bytes:
+    """the 32 bytes that key the device's ChaCha20 stream; None draws os.urandom(32)"""
     seed = os.urandom(32) if seed is None else bytes(seed)
     if len(seed) != 32:
         raise FheError(_capi.INVALID_ARGUMENT, "a seed is 32 bytes, got %d" % len(seed))
+    return seed
+
+
+def _encrypt(fn, key, par: BfvParameters, pts: Optional[PlaintextVec], seed: Optional[bytes], count: int,
+             level: int) -> Ciphertext:
+    seed = _seed(seed)
     b = pts.batch if pts is not None else None
     out = Ciphertext(par, b.count if b else count, 2, b.level if b else level, NTT, b.stream if b else 0)
     check(fn(key, b._h if b else None, par.variance, seed, out._h, out.stream))
@@ -762,11 +779,31 @@ class KeySwitchingKey:
         h = C.c_void_p()
         check(_capi.lib().fhe_b200_ksk_upload(par._h, ciphertext_level, ksk_level, _ptr(c0), _ptr(c1),
                                               c0.shape[0], C.byref(h)))
-        self._h, self.par = h, par
+        self._set(par, h, ciphertext_level, ksk_level, 0)
+
+    def _set(self, par: BfvParameters, h, ciphertext_level: int, ksk_level: int, stream: int):
+        self._h, self.par, self._stream = h, par, stream
         self.ciphertext_level, self.ksk_level = ciphertext_level, ksk_level
-        self._words = (c0, c1)                   # the caller's key material, for to_bytes (no device read-back entry)
-        # key_switching_key.rs:92-97: a key level with one modulus decomposes in base 2^(log_modulus / 2)
-        self.log_base = ((int(par.moduli()[0]) - 1).bit_length() // 2) if c0.shape[1] == 1 else 0
+        # key_switching_key.rs:92-126: a key level with one modulus decomposes in base 2^(log_modulus / 2), otherwise
+        # there is one digit per ciphertext limb
+        log_modulus = (int(par.moduli()[0]) - 1).bit_length()
+        single = len(par.moduli()) - ksk_level == 1
+        self.log_base = log_modulus // 2 if single else 0
+        self.n_digits = -(-log_modulus // self.log_base) if single else len(par.moduli()) - ciphertext_level
+
+    @staticmethod
+    def _adopt(par: BfvParameters, h, ciphertext_level: int, ksk_level: int, stream: int = 0) -> "KeySwitchingKey":
+        """a key handle the library generated on `stream`"""
+        k = KeySwitchingKey.__new__(KeySwitchingKey)
+        k._set(par, C.c_void_p(h), ciphertext_level, ksk_level, stream)
+        return k
+
+    def arrays(self):
+        """the key's NTT-domain words read back from the device: (c0, c1), each [n_digits][ksk_limbs][N]"""
+        shape = (self.n_digits, len(self.par.moduli()) - self.ksk_level, self.par.degree())
+        c0, c1 = np.empty(shape, np.uint64), np.empty(shape, np.uint64)
+        check(_capi.lib().fhe_b200_ksk_download(self._h, _ptr(c0), _ptr(c1), self._stream))
+        return c0, c1
 
     def __del__(self):
         h, self._h = getattr(self, "_h", None), None
@@ -777,7 +814,7 @@ class KeySwitchingKey:
     def to_bytes(self) -> bytes:
         """KeySwitchingKeyProto::from(&ksk).encode_to_vec(), unseeded branch: every c0_i and c1_i as an Rq with
         representation NTTSHOUP (its coefficients are the power-basis words, packed on the device)."""
-        c0, c1 = self._words
+        c0, c1 = self.arrays()
         par, nd = self.par, c0.shape[0]
         tmp = Ciphertext.from_host(par, np.ascontiguousarray(np.stack([c0, c1], axis=1)), self.ksk_level, NTT)
         blobs = tmp.to_packed()
@@ -894,6 +931,21 @@ class RelinearizationKey:
         self.ksk = ksk
 
     @staticmethod
+    def new(sk: SecretKey, seed: Optional[bytes] = None) -> "RelinearizationKey":
+        """RelinearizationKey::new (relinearization_key.rs:28-31), generated on the device"""
+        return RelinearizationKey.new_leveled(sk, 0, 0, seed)
+
+    @staticmethod
+    def new_leveled(sk: SecretKey, ciphertext_level: int, key_level: int,
+                    seed: Optional[bytes] = None) -> "RelinearizationKey":
+        """RelinearizationKey::new_leveled (relinearization_key.rs:33-65), generated on the device from the seeded
+        stream (seed as for SecretKey.try_encrypt)"""
+        h = C.c_void_p()
+        check(_capi.lib().fhe_b200_relin_key_generate(sk._h, ciphertext_level, key_level, sk.par.variance, _seed(seed),
+                                                      C.byref(h), 0))
+        return RelinearizationKey(KeySwitchingKey._adopt(sk.par, h.value, ciphertext_level, key_level))
+
+    @staticmethod
     def from_arrays(par: BfvParameters, c0, c1, ciphertext_level: int = 0, key_level: int = 0):
         return RelinearizationKey(KeySwitchingKey(par, c0, c1, ciphertext_level, key_level))
 
@@ -919,6 +971,12 @@ class GaloisKey:
         self.exponent, self.ksk = exponent, ksk
 
     @staticmethod
+    def new(sk: SecretKey, exponent: int, ciphertext_level: int = 0, key_level: int = 0,
+            seed: Optional[bytes] = None) -> "GaloisKey":
+        """GaloisKey::new (galois_key.rs:26-60), generated on the device (seed as for SecretKey.try_encrypt)"""
+        return _galois_keys(sk, [exponent], ciphertext_level, key_level, seed)[0]
+
+    @staticmethod
     def from_arrays(par: BfvParameters, exponent: int, c0, c1, ciphertext_level: int = 0, key_level: int = 0):
         return GaloisKey(exponent, KeySwitchingKey(par, c0, c1, ciphertext_level, key_level))
 
@@ -939,6 +997,20 @@ class GaloisKey:
         out = ct._like()
         check(_capi.lib().fhe_b200_galois(ct._h, self.exponent, self.ksk._h, out._h, ct.stream))
         return out
+
+
+def _galois_keys(sk: SecretKey, exponents: Sequence[int], ciphertext_level: int, key_level: int,
+                 seed: Optional[bytes]) -> "List[GaloisKey]":
+    """one device call for every exponent: key k of the call (stream word 13) is exponents[k]"""
+    two_n = 2 * sk.par.degree()
+    exps = [int(e) % two_n for e in exponents]      # SubstitutionExponent::new (rq/mod.rs:99-106)
+    arr = (C.c_uint32 * max(1, len(exps)))(*exps)
+    hs = (C.c_void_p * max(1, len(exps)))()
+    check(_capi.lib().fhe_b200_galois_keys_generate(sk._h, arr, len(exps), ciphertext_level, key_level,
+                                                    sk.par.variance, _seed(seed), C.cast(hs, C.POINTER(C.c_void_p)),
+                                                    0))
+    return [GaloisKey(e, KeySwitchingKey._adopt(sk.par, hs[k], ciphertext_level, key_level))
+            for k, e in enumerate(exps)]
 
 
 class EvaluationKey:
@@ -1017,6 +1089,81 @@ class EvaluationKey:
         if e not in self.gk:
             raise FheError(_capi.INVALID_ARGUMENT, "EvaluationKeyError: column rotation not supported by this key")
         return self.gk[e].relinearize(ct)
+
+
+class EvaluationKeyBuilder:
+    """fhe::bfv::EvaluationKeyBuilder (keys/evaluation_key.rs:318-491): the Galois keys of an EvaluationKey, generated
+    on the device in one call."""
+
+    def __init__(self, sk: SecretKey, ciphertext_level: int = 0, evaluation_key_level: int = 0):
+        self.sk = sk
+        self.ciphertext_level, self.evaluation_key_level = ciphertext_level, evaluation_key_level
+        self.inner_sum = self.row_rotation = False
+        self.expansion_level = 0
+        self.column_rotation = set()
+
+    @staticmethod
+    def new(sk: SecretKey) -> "EvaluationKeyBuilder":
+        return EvaluationKeyBuilder(sk)
+
+    @staticmethod
+    def new_leveled(sk: SecretKey, ciphertext_level: int, evaluation_key_level: int) -> "EvaluationKeyBuilder":
+        """evaluation_key.rs:353-383"""
+        if ciphertext_level > sk.par.max_level():
+            raise FheError(_capi.INVALID_LEVEL, "InvalidLevel: %d, max %d" % (ciphertext_level, sk.par.max_level()))
+        if evaluation_key_level > ciphertext_level:
+            raise FheError(_capi.INVALID_LEVEL, "InvalidLevel: %d, max %d" % (evaluation_key_level, ciphertext_level))
+        return EvaluationKeyBuilder(sk, ciphertext_level, evaluation_key_level)
+
+    def enable_expansion(self, level: int) -> "EvaluationKeyBuilder":
+        """evaluation_key.rs:386-398"""
+        max_level = self.sk.par.degree().bit_length() - 1
+        if level > max_level:
+            raise FheError(_capi.INVALID_LEVEL, "InvalidLevel: %d, max %d" % (level, max_level))
+        self.expansion_level = level
+        return self
+
+    def enable_inner_sum(self) -> "EvaluationKeyBuilder":
+        self.inner_sum = True
+        return self
+
+    def enable_row_rotation(self) -> "EvaluationKeyBuilder":
+        self.row_rotation = True
+        return self
+
+    def enable_column_rotation(self, i: int) -> "EvaluationKeyBuilder":
+        """evaluation_key.rs:414-426: steps 1 .. N/2 - 1"""
+        n = self.sk.par.degree()
+        if not 1 <= i < n // 2:
+            raise FheError(_capi.INVALID_ARGUMENT,
+                           "EvaluationKeyError::InvalidRotationStep: %d, expected 1..%d" % (i, n // 2 - 1))
+        self.column_rotation.add(pow(3, i, 2 * n))
+        return self
+
+    def exponents(self) -> List[int]:
+        """the Galois exponents build() generates keys for (evaluation_key.rs:439-463), ascending"""
+        n = self.sk.par.degree()
+        idx = set(self.column_rotation)
+        if self.row_rotation or self.inner_sum:
+            idx.add(2 * n - 1)
+        if self.inner_sum:
+            i = 1
+            while i < n // 2:
+                idx.add(pow(3, i, 2 * n))
+                i *= 2
+        for l in range(self.expansion_level):
+            idx.add((n >> l) + 1)
+        return sorted(idx)
+
+    def build(self, seed: Optional[bytes] = None) -> EvaluationKey:
+        """EvaluationKeyBuilder::build (evaluation_key.rs:429-491): every Galois key in one device call, the exponents
+        ascending, so a seed fixes the key of each exponent"""
+        ek = EvaluationKey(self.sk.par)
+        exps = self.exponents()
+        if exps:
+            for gk in _galois_keys(self.sk, exps, self.ciphertext_level, self.evaluation_key_level, seed):
+                ek.add_galois_key(gk)
+        return ek
 
 
 def dot_product_scalar(cts: "Ciphertext", pts, n_terms: Optional[int] = None) -> "Ciphertext":

@@ -4,6 +4,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -488,7 +489,9 @@ struct ChunkRunner {
   u32 count, chunk, ns;
   cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
   static u32 streams() { return switches().streams; }
-  ChunkRunner(const fhe_b200_params* p, u32 n, cudaStream_t st) : par(p), user(st), count(n), chunk(chunk_size()), ns(1) {
+  // items_per_chunk: 0 for chunk_size() ciphertexts; a call whose items are larger than a ciphertext passes its own
+  ChunkRunner(const fhe_b200_params* p, u32 n, cudaStream_t st, u32 items_per_chunk = 0)
+      : par(p), user(st), count(n), chunk(items_per_chunk ? items_per_chunk : chunk_size()), ns(1) {
     if (streams() < 2 || count <= chunk || chunk < streams()) return;
     ns = streams();
     chunk = (chunk + ns - 1) / ns;
@@ -1027,6 +1030,19 @@ int fhe_b200_batch_device_ptr(const fhe_b200_batch* b, uint64_t** dptr, size_t* 
 }
 
 // ------------------------------------------------------------------------------ keys
+// The digit count of a key from its two levels (key_switching_key.rs:92-126).  log_base receives 0 for RNS digits (one
+// per ciphertext limb) or, for a single-modulus key level, the base-2^(log_modulus/2) decomposition of the residue.
+static u32 ksk_digits(const fhe_b200_params* p, const LevelData& cl, const LevelData& kl, u32& log_base) {
+  log_base = 0;
+  if (kl.L > 1) return cl.L;
+  REQUIRE(cl.L == 1, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch: a single-modulus key serves the last level only");
+  const u64 q = p->moduli[0];
+  const u32 log_modulus = 64 - (u32)clz64(q - 1);   // next_power_of_two().ilog2()
+  log_base = log_modulus / 2;
+  REQUIRE(log_base >= 1, FHE_B200_UNSUPPORTED, "modulus too small for the decomposition");
+  return (log_modulus + log_base - 1) / log_base;
+}
+
 int fhe_b200_ksk_upload(const fhe_b200_params* p, uint32_t ciphertext_level, uint32_t ksk_level, const uint64_t* c0,
                         const uint64_t* c1, uint32_t n_digits, fhe_b200_ksk** out) {
   API_BEGIN
@@ -1036,18 +1052,10 @@ int fhe_b200_ksk_upload(const fhe_b200_params* p, uint32_t ciphertext_level, uin
   const LevelData& kl = p->level(ksk_level);
   REQUIRE(ksk_level <= ciphertext_level, FHE_B200_INVALID_LEVEL, "key level must not exceed the ciphertext level");
   u32 log_base = 0;
-  if (kl.L == 1) {
-    // KeySwitchingKey::new (key_switching_key.rs:92-97): base-2^(log_modulus/2) decomposition of the single residue
-    REQUIRE(cl.L == 1, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch: a single-modulus key serves the last level only");
-    const u64 q = p->moduli[0];
-    const u32 log_modulus = 64 - (u32)clz64(q - 1);   // next_power_of_two().ilog2()
-    log_base = log_modulus / 2;
-    REQUIRE(log_base >= 1, FHE_B200_UNSUPPORTED, "modulus too small for the decomposition");
-    REQUIRE(n_digits == (log_modulus + log_base - 1) / log_base, FHE_B200_CONTEXT_MISMATCH,
-            "n_digits must be ceil(log_modulus / log_base) for a single-modulus key");
-  } else {
-    REQUIRE(n_digits == cl.L, FHE_B200_CONTEXT_MISMATCH, "n_digits must equal the ciphertext level's limb count");
-  }
+  const u32 want = ksk_digits(p, cl, kl, log_base);
+  REQUIRE(n_digits == want, FHE_B200_CONTEXT_MISMATCH,
+          log_base ? "n_digits must be ceil(log_modulus / log_base) for a single-modulus key"
+                   : "n_digits must equal the ciphertext level's limb count");
   std::unique_ptr<fhe_b200_ksk> k(new fhe_b200_ksk());
   k->par = p; k->ct_level = ciphertext_level; k->ksk_level = ksk_level; k->n_dig = n_digits; k->Lk = kl.L;
   k->log_base = log_base;
@@ -1067,6 +1075,22 @@ int fhe_b200_ksk_upload(const fhe_b200_params* p, uint32_t ciphertext_level, uin
   k->k1 = (u64*)g1.release();
   params_retain(p);
   *out = k.release();
+  API_END
+}
+int fhe_b200_ksk_download(const fhe_b200_ksk* k, uint64_t* c0, uint64_t* c1, void* stream) {
+  API_BEGIN
+  REQUIRE(k && c0 && c1, FHE_B200_INVALID_ARGUMENT, "null argument");
+  DeviceGuard g(k->par);
+  cudaStream_t st = (cudaStream_t)stream;
+  // device layout [limb][digit][N] -> host layout [digit][limb][N], the reverse of fhe_b200_ksk_upload
+  const size_t rowb = sizeof(u64) << k->par->logn, row = (size_t)1 << k->par->logn;
+  for (u32 i = 0; i < k->n_dig; i++) {
+    FHE_CUDA(cudaMemcpy2DAsync(c0 + (size_t)i * k->Lk * row, rowb, k->k0 + i * row, k->n_dig * rowb, rowb, k->Lk,
+                               cudaMemcpyDeviceToHost, st));
+    FHE_CUDA(cudaMemcpy2DAsync(c1 + (size_t)i * k->Lk * row, rowb, k->k1 + i * row, k->n_dig * rowb, rowb, k->Lk,
+                               cudaMemcpyDeviceToHost, st));
+  }
+  FHE_CUDA(cudaStreamSynchronize(st));
   API_END
 }
 int fhe_b200_ksk_free(fhe_b200_ksk* k) {
@@ -1587,6 +1611,14 @@ int fhe_b200_decode(const fhe_b200_encoder* e, int encoding, int is_signed, cons
 }
 
 // ---- encryption (keys/secret_key.rs:100-136, :181-193; keys/public_key.rs:45-92)
+// the 32-byte seed as the key words of the ChaCha20 state
+static EncSeed seed_words(const uint8_t* seed) {
+  EncSeed K;
+  for (int i = 0; i < 8; i++)
+    K.w[i] = (u32)seed[4 * i] | (u32)seed[4 * i + 1] << 8 | (u32)seed[4 * i + 2] << 16 | (u32)seed[4 * i + 3] << 24;
+  return K;
+}
+
 // the checks shared by both entry points; returns the seed as the key words of the ChaCha20 state
 static EncSeed check_encrypt(const fhe_b200_params* par, const fhe_b200_batch* pts, const uint8_t* seed,
                              const fhe_b200_batch* out) {
@@ -1604,10 +1636,7 @@ static EncSeed check_encrypt(const fhe_b200_params* par, const fhe_b200_batch* p
   }
   REQUIRE(par->t_small && par->t_mod.t < par->moduli[0], FHE_B200_UNSUPPORTED,
           "to_poly needs t below the first ciphertext modulus");
-  EncSeed K;
-  for (int i = 0; i < 8; i++)
-    K.w[i] = (u32)seed[4 * i] | (u32)seed[4 * i + 1] << 8 | (u32)seed[4 * i + 2] << 16 | (u32)seed[4 * i + 3] << 24;
-  return K;
+  return seed_words(seed);
 }
 
 static void check_variance(uint32_t variance) {   // BfvParametersBuilder::build (parameters.rs:449-454)
@@ -1683,6 +1712,153 @@ int fhe_b200_encrypt_pk(const fhe_b200_batch* pk, const fhe_b200_batch* pts, uin
   });
   FHE_CUDA(cudaGetLastError());
   out->repr = FHE_B200_NTT;
+  API_END
+}
+
+// ---- key generation (key_switching_key.rs:71-238, relinearization_key.rs:43-65, galois_key.rs:26-60,
+// rgsw_ciphertext.rs:94-120).  Every value is a canonical residue and the NTT is linear, so the key is built in the NTT
+// domain: c0_i = NTT(e_i) - c1_i s + G[i] x, with x the key's polynomial at the ciphertext level.  The switch-up of x
+// to the key level (Switcher) is x (Q_key / Q_ct) on the ciphertext limbs and 0 on the others, and the Garner
+// coefficient g_i of the ciphertext basis is δ_ij modulo its limbs, so G[i][j] = δ_ij (Q_key / Q_ct mod q_j).
+static void check_key_levels(const fhe_b200_params* par, uint32_t ciphertext_level, uint32_t key_level) {
+  REQUIRE(ciphertext_level < par->Lmax, FHE_B200_INVALID_LEVEL,
+          "InvalidLevel: ciphertext level " + std::to_string(ciphertext_level));
+  REQUIRE(key_level <= ciphertext_level, FHE_B200_INVALID_LEVEL,
+          "InvalidLevel: key level " + std::to_string(key_level) + " above the ciphertext level");
+}
+
+// Makes n_keys keys at (ct_level, key_level) into out[0 .. n_keys).  x_of(k, x, st) writes key k's x [L_ct][N] (NTT)
+// into scratch.  The (key, digit) items go through the chunk runner, per chunk at most chunk_size() error rows
+// (chunk_size() / Lk items of Lk rows each; at set C 18 items, 64 MiB of errors) whatever the number of keys: per chunk
+// the errors (role 6) are drawn and transformed at once, then the generator runs once per key the chunk touches.  On
+// failure the keys made so far are freed and out is left untouched.
+static void generate_keys(const fhe_b200_secret_key* sk, u32 n_keys, u32 ct_level, u32 key_level, u32 variance,
+                          const EncSeed& K, const std::function<void(u32, u64*, cudaStream_t)>& x_of,
+                          fhe_b200_ksk** out, cudaStream_t user) {
+  const fhe_b200_params* par = sk->par;
+  const LevelData& cl = par->level(ct_level);
+  const LevelData& kl = par->level(key_level);
+  u32 log_base = 0;
+  const u32 n_dig = ksk_digits(par, cl, kl, log_base);
+  const u32 Lk = kl.L, logn = par->logn;
+  const size_t row = (size_t)1 << logn;
+  KskG G;
+  std::memset(&G, 0, sizeof(G));
+  G.decomp = log_base ? 1 : 0;
+  for (u32 j = 0; j < (log_base ? n_dig : cl.L); j++) {
+    const u64 q = log_base ? par->moduli[0] : par->moduli[j];
+    u64 v = log_base ? ((1ull << (j * log_base)) % q) : 1;   // i log_base < 64 (at most 3 digits of <= 31 bits)
+    for (u32 l = cl.L; l < Lk; l++) v = mulmod_h(v, par->moduli[l] % q, q);
+    G.g[j] = v;
+    G.g_s[j] = ModulusH(q).shoup(v);
+  }
+  struct Made {   // the handles made so far, freed again unless the call succeeds
+    std::vector<fhe_b200_ksk*> k;
+    ~Made() { for (fhe_b200_ksk* h : k) fhe_b200_ksk_free(h); }
+  } made;
+  const size_t bytes = (size_t)n_dig * Lk * row * sizeof(u64);
+  for (u32 k = 0; k < n_keys; k++) {
+    DevPtr g0, g1;
+    FHE_CUDA(cudaMalloc(&g0.p, bytes));
+    FHE_CUDA(cudaMalloc(&g1.p, bytes));
+    fhe_b200_ksk* h = new fhe_b200_ksk();
+    h->par = params_retain(par); h->ct_level = ct_level; h->ksk_level = key_level; h->n_dig = n_dig; h->Lk = Lk;
+    h->log_base = log_base;
+    h->k0 = (u64*)g0.release();
+    h->k1 = (u64*)g1.release();
+    made.k.push_back(h);
+  }
+  ChunkRunner chunks(par, n_keys * n_dig, user, std::max(1u, chunk_size() / Lk));
+  chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace ws(par, st);
+    u64* e = ws.secret_words((size_t)n * Lk * row);
+    launch_cbd(e, n, c0, 6, 1, variance, K, kl.ctx_ids, par->d_limbs, logn, st, n_dig);
+    launch_ntt(e, e, n * Lk, kl.ctx_ids, par->d_limbs, logn, false, 1, false, st);
+    u64* x = ws.secret_words((size_t)cl.L * row);
+    for (u32 it = c0; it < c0 + n;) {
+      const u32 key = it / n_dig, d0 = it % n_dig, nd = std::min(n_dig - d0, c0 + n - it);
+      x_of(key, x, st);
+      const fhe_b200_ksk* h = made.k[key];
+      launch_ksk_gen(sk->s, e + (size_t)(it - c0) * Lk * row, x, h->k0, h->k1, key, d0, nd, n_dig, G, K, kl.ctx_ids,
+                     par->d_limbs, logn, st);
+      it += nd;
+    }
+  });
+  FHE_CUDA(cudaGetLastError());
+  for (u32 k = 0; k < n_keys; k++) out[k] = made.k[k];
+  made.k.clear();
+}
+
+// x = a * s on the limbs of the level (a: [L][N] NTT words, s the secret key's rows)
+static void times_s(const fhe_b200_secret_key* sk, const LevelData& lv, const u64* a, u64* x, cudaStream_t st) {
+  const fhe_b200_params* par = sk->par;
+  const size_t words = (size_t)lv.L << par->logn;
+  FHE_CUDA(cudaMemcpyAsync(x, a, words * sizeof(u64), cudaMemcpyDeviceToDevice, st));
+  launch_mul_plain(x, sk->s, 1, 1, 1, lv.ctx_ids, par->d_limbs, par->logn, st, 0);
+}
+
+int fhe_b200_relin_key_generate(const fhe_b200_secret_key* sk, uint32_t ciphertext_level, uint32_t key_level,
+                                uint32_t variance, const uint8_t* seed, fhe_b200_ksk** out, void* stream) {
+  API_BEGIN
+  check_variance(variance);
+  REQUIRE(sk && seed && out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = sk->par;
+  check_key_levels(par, ciphertext_level, key_level);
+  REQUIRE(par->Lmax - key_level > 1, FHE_B200_UNSUPPORTED,
+          "EvaluationKeyError::KeySwitchingNotSupported: a relinearization key needs two or more key moduli");
+  DeviceGuard g(par);
+  const LevelData& cl = par->level(ciphertext_level);
+  // x = s * s (relinearization_key.rs:56-60)
+  generate_keys(sk, 1, ciphertext_level, key_level, variance, seed_words(seed),
+                [&](u32, u64* x, cudaStream_t st) { times_s(sk, cl, sk->s, x, st); }, out, (cudaStream_t)stream);
+  API_END
+}
+
+int fhe_b200_galois_keys_generate(const fhe_b200_secret_key* sk, const uint32_t* exponents, uint32_t n_keys,
+                                  uint32_t ciphertext_level, uint32_t key_level, uint32_t variance,
+                                  const uint8_t* seed, fhe_b200_ksk** out, void* stream) {
+  API_BEGIN
+  check_variance(variance);
+  REQUIRE(sk && seed && out && (exponents || !n_keys), FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = sk->par;
+  check_key_levels(par, ciphertext_level, key_level);
+  std::vector<u32> exps(n_keys);
+  for (u32 k = 0; k < n_keys; k++) {   // SubstitutionExponent::new (rq/mod.rs:99-121)
+    exps[k] = (u32)(exponents[k] % (2 * par->N));
+    REQUIRE(exps[k] & 1, FHE_B200_INVALID_EXPONENT, "InvalidSubstitutionExponent: " + std::to_string(exponents[k]));
+  }
+  DeviceGuard g(par);
+  const LevelData& cl = par->level(ciphertext_level);
+  std::vector<const int*> perms(n_keys);
+  for (u32 k = 0; k < n_keys; k++) perms[k] = par->perm(exps[k]);
+  // x = s substituted by the exponent (galois_key.rs:40-46), a gather of the NTT words
+  generate_keys(sk, n_keys, ciphertext_level, key_level, variance, seed_words(seed),
+                [&](u32 k, u64* x, cudaStream_t st) { launch_gather(sk->s, x, cl.L, perms[k], par->logn, st); }, out,
+                (cudaStream_t)stream);
+  API_END
+}
+
+int fhe_b200_rgsw_encrypt(const fhe_b200_secret_key* sk, const fhe_b200_batch* pts, uint32_t variance,
+                          const uint8_t* seed, fhe_b200_ksk** out, void* stream) {
+  API_BEGIN
+  check_variance(variance);
+  REQUIRE(sk && pts && seed && out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = sk->par;
+  REQUIRE(pts->par == par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch");
+  REQUIRE(!pts->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
+  REQUIRE(pts->parts == 1, FHE_B200_INVALID_ARGUMENT, "pts must be a 1-part batch");
+  need_repr(pts, FHE_B200_NTT);
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(pts->level);
+  const size_t words = (size_t)lv.L << par->logn;
+  // ksk0 of plaintext p has x = m, ksk1 has x = m s (rgsw_ciphertext.rs:106-116); m = pt.poly_ntt
+  generate_keys(sk, 2 * pts->count, pts->level, pts->level, variance, seed_words(seed),
+                [&](u32 k, u64* x, cudaStream_t st) {
+                  const u64* m = pts->d + (k / 2) * words;
+                  if (k & 1) times_s(sk, lv, m, x, st);
+                  else FHE_CUDA(cudaMemcpyAsync(x, m, words * sizeof(u64), cudaMemcpyDeviceToDevice, st));
+                },
+                out, (cudaStream_t)stream);
   API_END
 }
 

@@ -217,11 +217,26 @@ void launch_encrypt_sk(const u64* s, const u64* e, u64* out, u32 cts, u32 ct_bas
                        const LimbDev* limbs, u32 logn, cudaStream_t st);
 // out [cts][n_roles][L][N]: the centred binomial polynomial of roles role0 .. role0 + n_roles - 1 (drawn from limb 0's
 // row) as canonical residues in every limb; variance 1..32
+// digits > 1 addresses the rows as key generation does: row c of the call is digit c % digits (state word 15) of key
+// c / digits (state word 13)
 void launch_cbd(u64* out, u32 cts, u32 ct_base, u32 role0, u32 n_roles, u32 variance, const EncSeed& K,
-                const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st);
+                const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st, u32 digits = 1);
 // out [cts][2][L][N] = (u*pk0 + e1, u*pk1 + e2); uee [cts][3][L][N] = (u, e1, e2), pk [2][L][N], all NTT
 void launch_encrypt_pk(const u64* uee, const u64* pk, u64* out, u32 cts, const RowIds& ids, const LimbDev* limbs,
                        u32 logn, cudaStream_t st);
+
+// key generation (key_switching_key.rs:71-238): G, the gadget factor of digit i on key limb j, as Shoup pairs.  RNS
+// digits (decomp = 0): G[i][j] = (i == j) g[j], g[j] = (Q_key / Q_ct) mod q_j; decomposition (decomp = 1, one key
+// limb): G[i][0] = g[i] = 2^(i log_base) mod q_0
+struct KskG {
+  u32 decomp;
+  u64 g[kMaxPos], g_s[kMaxPos];
+};
+// digits digit0 .. digit0 + digits - 1 of key `key` of the call: k0/k1 [Lk][n_dig][N] receive c0 = NTT(e_i) - c1 s +
+// G[i][j] x and c1 (role 5, drawn directly as NTT words); e [digits][Lk][N] NTT, x [L_ct][N] NTT, s row j at s + j*N
+void launch_ksk_gen(const u64* s, const u64* e, const u64* x, u64* k0, u64* k1, u32 key, u32 digit0, u32 digits,
+                    u32 n_dig, const KskG& G, const EncSeed& K, const RowIds& ids, const LimbDev* limbs, u32 logn,
+                    cudaStream_t st);
 
 // bit (un)packing of power-basis rows (fhe-util/src/lib.rs:71-146): row r of `rows` uses nbits[r % limbs] bits per
 // coefficient; packed row r starts at byte  (r / limbs) * poly_bytes + offs[r % limbs]

@@ -1177,9 +1177,10 @@ __global__ void __launch_bounds__(256) noise_kernel(NoiseArgs A) {
 }
 
 // ------------------------------------------------------------------ encryption (keys/secret_key.rs:100-136,
-// keys/public_key.rs:45-92).  The random words come from the seeded ChaCha20 stream of include/fhe_b200.h: block b of
-// the row (ciphertext ct, role, limb) is the RFC 8439 block function of the state (constants, seed, b, ct,
-// role << 8 | limb, 0); value m of the block (u64 words 2m, 2m + 1) drives coefficient 4b + m.
+// keys/public_key.rs:45-92) and key generation.  The random words come from the seeded ChaCha20 stream of
+// include/fhe_b200.h: block b of the row (ciphertext or key ct, role, limb, digit) is the RFC 8439 block function of
+// the state (constants, seed, b, ct, role << 8 | limb, digit); value m of the block (u64 words 2m, 2m + 1) drives
+// coefficient 4b + m.  Encryption rows have digit 0.
 __device__ __forceinline__ void chacha_qr(u32& a, u32& b, u32& c, u32& d) {
   a += b; d = __funnelshift_l(d ^ a, d ^ a, 16);
   c += d; b = __funnelshift_l(b ^ c, b ^ c, 12);
@@ -1187,10 +1188,10 @@ __device__ __forceinline__ void chacha_qr(u32& a, u32& b, u32& c, u32& d) {
   c += d; b = __funnelshift_l(b ^ c, b ^ c, 7);
 }
 // the four 128-bit values (lo[m], hi[m]) of one block
-__device__ __forceinline__ void chacha_block(const EncSeed& K, u32 b, u32 ct, u32 role_limb, u64 (&lo)[4],
+__device__ __forceinline__ void chacha_block(const EncSeed& K, u32 b, u32 ct, u32 role_limb, u32 digit, u64 (&lo)[4],
                                              u64 (&hi)[4]) {
   const u32 in[16] = {0x61707865u, 0x3320646eu, 0x79622d32u, 0x6b206574u, K.w[0], K.w[1], K.w[2], K.w[3],
-                      K.w[4],      K.w[5],      K.w[6],      K.w[7],      b,      ct,     role_limb, 0u};
+                      K.w[4],      K.w[5],      K.w[6],      K.w[7],      b,      ct,     role_limb, digit};
   u32 x[16];
 #pragma unroll
   for (int i = 0; i < 16; i++) x[i] = in[i];
@@ -1234,7 +1235,7 @@ __global__ void encrypt_sk_kernel(EncSkArgs A) {
   const u32 j = (u32)(row % A.limbs_per_poly), ct = (u32)(row / A.limbs_per_poly);
   const LimbDev& M = A.limbs[A.ids[j]];
   u64 lo[4], hi[4];
-  chacha_block(A.K, g, A.ct_base + ct, j, lo, hi);   // role 0 (a), limb j
+  chacha_block(A.K, g, A.ct_base + ct, j, 0, lo, hi);   // role 0 (a), limb j
   const size_t c = (size_t)g * 4;
   const ulonglong2* sp = reinterpret_cast<const ulonglong2*>(A.s + ((size_t)j << A.logn) + c);
   const ulonglong2* ep = reinterpret_cast<const ulonglong2*>(A.e + (row << A.logn) + c);
@@ -1259,12 +1260,13 @@ struct CbdArgs {
   EncSeed K;
   u64 add_lo, add_hi, sub_lo, sub_hi;   // mask_add = low 2 variance bits, mask_sub = the next 2 variance bits
   u32 cts, ct_base, role0, n_roles, logn, limbs_per_poly;
+  u32 digits;         // rows per key: row c of the call is digit c % digits of key c / digits (encryption: 1)
   const LimbDev* limbs;
   unsigned short ids[kMaxPos];
 };
 // Poly::small (rq/mod.rs, fhe-util sample_vec_cbd): x = popc(v & mask_add) - popc(v & mask_sub) on the 128-bit value
-// of the (ct, role, limb 0) row, written as its canonical residue into every limb of the level (q_j - |x| for x < 0,
-// by a select).  One thread per (ciphertext, role, 4 coefficients).
+// of the (ct, role, limb 0, digit) row, written as its canonical residue into every limb of the level (q_j - |x| for
+// x < 0, by a select).  One thread per (ciphertext or (key, digit), role, 4 coefficients).
 __global__ void cbd_kernel(CbdArgs A) {
   const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const u32 g_per_row = 1u << (A.logn - 2);
@@ -1272,9 +1274,9 @@ __global__ void cbd_kernel(CbdArgs A) {
   if (idx >= total) return;
   const u32 g = (u32)(idx % g_per_row);
   const size_t poly = idx / g_per_row;
-  const u32 r = (u32)(poly % A.n_roles), ct = (u32)(poly / A.n_roles);
+  const u32 r = (u32)(poly % A.n_roles), row = A.ct_base + (u32)(poly / A.n_roles);
   u64 lo[4], hi[4];
-  chacha_block(A.K, g, A.ct_base + ct, (A.role0 + r) << 8, lo, hi);
+  chacha_block(A.K, g, row / A.digits, (A.role0 + r) << 8, row % A.digits, lo, hi);
   long long x[4];
 #pragma unroll
   for (int m = 0; m < 4; m++)
@@ -1314,6 +1316,60 @@ __global__ void encrypt_pk_kernel(EncPkArgs A) {
   u64* dst = A.out + ct * 2 * stride + in_ct;
   dst[0] = csub(mulmod_limb(u, A.pk[in_ct], M) + e1, M.p);
   dst[stride] = csub(mulmod_limb(u, A.pk[stride + in_ct], M) + e2, M.p);
+}
+
+struct KskGenArgs {
+  const u64* s;       // row j: s modulo the j-th limb (NTT)
+  const u64* e;       // [digits][Lk][N]: NTT(e_i) of the digits digit0 .. digit0 + digits - 1
+  const u64* x;       // [L_ct][N]: the key's x at the ciphertext level (NTT)
+  u64 *k0, *k1;       // the key, [Lk][n_dig][N]
+  EncSeed K;
+  u32 key, digit0, digits, n_dig, logn, limbs_per_poly, decomp;
+  const LimbDev* limbs;
+  // G as Shoup pairs: RNS digits G[i][j] = (i == j) g[j]; decomposition G[i][0] = g[i]
+  u64 g[kMaxPos], g_s[kMaxPos];
+  unsigned short ids[kMaxPos];
+};
+// KeySwitchingKey::new (key_switching_key.rs:71-238) in the NTT domain, for digits of one key: c1 = (hi 2^64 + lo) mod
+// q_j of the role-5 row (key, limb j, digit i), c0 = NTT(e_i) - c1 s + G[i][j] x.  One thread per (digit, key limb, 4
+// coefficients); both words go from the registers straight into the [limb][digit][N] layout the key switch reads.
+// x is read only where G[i][j] is not zero, which depends on the indices alone; no branch depends on the data.
+__global__ void ksk_gen_kernel(KskGenArgs A) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const u32 g_per_row = 1u << (A.logn - 2);
+  const size_t total = (size_t)A.digits * A.limbs_per_poly * g_per_row;
+  if (idx >= total) return;
+  const u32 g = (u32)(idx % g_per_row);
+  const size_t row = idx / g_per_row;
+  const u32 j = (u32)(row % A.limbs_per_poly), d = (u32)(row / A.limbs_per_poly), i = A.digit0 + d;
+  const LimbDev& M = A.limbs[A.ids[j]];
+  u64 lo[4], hi[4];
+  chacha_block(A.K, g, A.key, (5u << 8) | j, i, lo, hi);   // role 5 (c1), limb j, digit i
+  const size_t c = (size_t)g * 4;
+  const ulonglong2* sp = reinterpret_cast<const ulonglong2*>(A.s + ((size_t)j << A.logn) + c);
+  const ulonglong2* ep = reinterpret_cast<const ulonglong2*>(A.e + (row << A.logn) + c);
+  const ulonglong2 s01 = sp[0], s23 = sp[1], e01 = ep[0], e23 = ep[1];
+  const u64 s[4] = {s01.x, s01.y, s23.x, s23.y}, e[4] = {e01.x, e01.y, e23.x, e23.y};
+  const u32 gi = A.decomp ? i : j;
+  u64 x[4] = {0, 0, 0, 0};
+  if (A.decomp || i == j) {
+    const ulonglong2* xp = reinterpret_cast<const ulonglong2*>(A.x + ((size_t)(A.decomp ? 0 : j) << A.logn) + c);
+    const ulonglong2 x01 = xp[0], x23 = xp[1];
+    x[0] = x01.x; x[1] = x01.y; x[2] = x23.x; x[3] = x23.y;
+  }
+  const u64 gw = A.g[gi], gw_s = A.g_s[gi];
+  u64 a[4], b[4];
+#pragma unroll
+  for (int m = 0; m < 4; m++) {
+    a[m] = reduce128_limb(lo[m], hi[m], M);
+    b[m] = csub(e[m] + M.p - mulmod_limb(a[m], s[m], M), M.p);
+    b[m] = csub(b[m] + mul_shoup(x[m], gw, gw_s, M.p), M.p);
+  }
+  const size_t off = ((size_t)j * A.n_dig + i) << A.logn;
+  reinterpret_cast<ulonglong2*>(A.k0 + off + c)[0] = make_ulonglong2(b[0], b[1]);
+  reinterpret_cast<ulonglong2*>(A.k0 + off + c)[1] = make_ulonglong2(b[2], b[3]);
+  reinterpret_cast<ulonglong2*>(A.k1 + off + c)[0] = make_ulonglong2(a[0], a[1]);
+  reinterpret_cast<ulonglong2*>(A.k1 + off + c)[1] = make_ulonglong2(a[2], a[3]);
 }
 
 void copy_ids(unsigned short* dst, const RowIds& ids) {
@@ -1398,13 +1454,13 @@ void launch_encrypt_sk(const u64* s, const u64* e, u64* out, u32 cts, u32 ct_bas
 }
 
 void launch_cbd(u64* out, u32 cts, u32 ct_base, u32 role0, u32 n_roles, u32 variance, const EncSeed& K,
-                const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st) {
+                const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st, u32 digits) {
   CbdArgs A;
   const u128 add = (((u128)1) << (2 * variance)) - 1;   // variance <= 32: 2 variance <= 64 bits each
   const u128 sub = add << (2 * variance);
   A.add_lo = (u64)add; A.add_hi = (u64)(add >> 64); A.sub_lo = (u64)sub; A.sub_hi = (u64)(sub >> 64);
   A.out = out; A.K = K; A.cts = cts; A.ct_base = ct_base; A.role0 = role0; A.n_roles = n_roles; A.logn = logn;
-  A.limbs_per_poly = ids.limbs_per_poly; A.limbs = limbs;
+  A.digits = digits; A.limbs_per_poly = ids.limbs_per_poly; A.limbs = limbs;
   copy_ids(A.ids, ids);
   const size_t total = ((size_t)cts * n_roles) << (logn - 2);
   if (!total) return;
@@ -1421,6 +1477,20 @@ void launch_encrypt_pk(const u64* uee, const u64* pk, u64* out, u32 cts, const R
   const size_t total = ((size_t)cts * ids.limbs_per_poly) << logn;
   if (!total) return;
   encrypt_pk_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(A);
+  g_launches++;
+}
+
+void launch_ksk_gen(const u64* s, const u64* e, const u64* x, u64* k0, u64* k1, u32 key, u32 digit0, u32 digits,
+                    u32 n_dig, const KskG& G, const EncSeed& K, const RowIds& ids, const LimbDev* limbs, u32 logn,
+                    cudaStream_t st) {
+  KskGenArgs A;
+  A.s = s; A.e = e; A.x = x; A.k0 = k0; A.k1 = k1; A.K = K; A.key = key; A.digit0 = digit0; A.digits = digits;
+  A.n_dig = n_dig; A.logn = logn; A.limbs_per_poly = ids.limbs_per_poly; A.decomp = G.decomp; A.limbs = limbs;
+  for (int i = 0; i < kMaxPos; i++) { A.g[i] = G.g[i]; A.g_s[i] = G.g_s[i]; }
+  copy_ids(A.ids, ids);
+  const size_t total = ((size_t)digits * ids.limbs_per_poly) << (logn - 2);
+  if (!total) return;
+  ksk_gen_kernel<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(A);
   g_launches++;
 }
 

@@ -147,6 +147,9 @@ int fhe_b200_batch_device_ptr(const fhe_b200_batch* b, uint64_t** dptr, size_t* 
 int fhe_b200_ksk_upload(const fhe_b200_params* p, uint32_t ciphertext_level, uint32_t ksk_level,
                         const uint64_t* c0, const uint64_t* c1, uint32_t n_digits, fhe_b200_ksk** out);
 int fhe_b200_ksk_free(fhe_b200_ksk* k);
+/* the key's words back in the host layout of fhe_b200_ksk_upload: c0, c1 [n_digits][key limbs][N] (NTT); waits for
+ * `stream` (a generated key is complete once the stream reaches this call) */
+int fhe_b200_ksk_download(const fhe_b200_ksk* k, uint64_t* c0, uint64_t* c1, void* stream);
 
 /* ---- primitives (each parity-tested one by one) --------------------------------------- */
 /* Poly::into_ntt / NttOperator::forward[_vt] on every row (rq/mod.rs:535, ntt/native.rs:77,183) */
@@ -250,8 +253,8 @@ int fhe_b200_measure_noise(const fhe_b200_secret_key* sk, const fhe_b200_batch* 
  *     word 12      b, the block index within the row
  *     word 13      the index of the ciphertext within the call (0 .. out.count - 1)
  *     word 14      role << 8 | limb: role 0 = a, 1 = e (secret-key encryption), 2 = u, 3 = e1, 4 = e2 (public-key
- *                  encryption); the small polynomials use limb 0
- *     word 15      0
+ *                  encryption), 5 = c1, 6 = e (key generation, below); the small polynomials use limb 0
+ *     word 15      0 (encryption), the digit of the key (key generation)
  * Each block is addressed only by its position, so the words do not depend on chunking or streams.  One 64-byte block
  * gives four 128-bit values: value m is u64 words 2m (low) and 2m + 1 (high) of the block, and coefficient 4b + m of
  * the row takes value m of block b.
@@ -279,6 +282,39 @@ int fhe_b200_encrypt_sk(const fhe_b200_secret_key* sk, const fhe_b200_batch* pts
  * one 2-part ciphertext -> INVALID_ARGUMENT; power-basis pk -> INVALID_REPRESENTATION. */
 int fhe_b200_encrypt_pk(const fhe_b200_batch* pk, const fhe_b200_batch* pts, uint32_t variance, const uint8_t* seed,
                         fhe_b200_batch* out, void* stream);
+
+/* ---- key generation ------------------------------------------------------------------------------
+ * KeySwitchingKey::new (key_switching_key.rs:71-238) on the device, for every digit i of every key of the call:
+ * c1_i uniform at the key level and c0_i = e_i - c1_i s + g_i from, computed in the NTT domain (every value is a
+ * canonical residue and the NTT is linear, so the words are those of the reference's power-basis computation).  The
+ * words come from the stream above with word 13 = the index k of the key within the call, word 15 = the digit i:
+ *  - c1 (role 5, limb j of the key level): (hi 2^64 + lo) mod q_j, drawn directly as NTT words;
+ *  - e_i (role 6, limb 0): the centred binomial sample, lifted to every key limb.
+ * Key indices: 0 for the relinearization key, the position in `exponents` for Galois keys, 2p (ksk0) and 2p + 1
+ * (ksk1) for plaintext p of an RGSW encryption.  The digits: one per ciphertext limb, g_i the Garner coefficient of the
+ * ciphertext basis and `from` x switched up to the key level; or, when the key level has a single modulus (then the
+ * last level, as fhe_b200_ksk_upload requires), the base-2^log_base decomposition with g_i = 2^(i log_base).  The
+ * handles are ordinary keys: fhe_b200_relinearize, fhe_b200_galois, fhe_b200_expand, fhe_b200_key_switch and the
+ * multiplicator take them.  Compact (seeded) key messages need the reference's ChaCha8 stream, which this library does
+ * not reproduce: fhe_b200_ksk_download gives both rows for an uncompact message.  Scratch holding errors or x is zeroed
+ * before it goes back to the pool.  Errors: variance outside 1..32 (InvalidVariance), a NULL argument ->
+ * INVALID_ARGUMENT; key_level > ciphertext_level or ciphertext_level above the max level -> INVALID_LEVEL; a
+ * decomposition base below 1 -> UNSUPPORTED.  A failed call returns no handle and frees every key it made. */
+/* RelinearizationKey::new_leveled (relinearization_key.rs:43-65): x = s s.  A single-modulus key level ->
+ * UNSUPPORTED (EvaluationKeyError::KeySwitchingNotSupported). */
+int fhe_b200_relin_key_generate(const fhe_b200_secret_key* sk, uint32_t ciphertext_level, uint32_t key_level,
+                                uint32_t variance, const uint8_t* seed, fhe_b200_ksk** out, void* stream);
+/* GaloisKey::new (galois_key.rs:26-60) for each of n_keys exponents (reduced mod 2N): x = s substituted by the
+ * exponent; out receives n_keys handles.  An even exponent -> INVALID_EXPONENT. */
+int fhe_b200_galois_keys_generate(const fhe_b200_secret_key* sk, const uint32_t* exponents, uint32_t n_keys,
+                                  uint32_t ciphertext_level, uint32_t key_level, uint32_t variance,
+                                  const uint8_t* seed, fhe_b200_ksk** out, void* stream);
+/* SecretKey::try_encrypt into RGSWCiphertext (rgsw_ciphertext.rs:94-120) of every plaintext of pts (a 1-part NTT
+ * batch from fhe_b200_encode) at its level: out receives 2 pts.count handles, ksk0 (x = m) and ksk1 (x = m s) of each
+ * plaintext.  pts of another parameter set or over the multiplication basis -> CONTEXT_MISMATCH, not 1-part ->
+ * INVALID_ARGUMENT, power basis -> INVALID_REPRESENTATION. */
+int fhe_b200_rgsw_encrypt(const fhe_b200_secret_key* sk, const fhe_b200_batch* pts, uint32_t variance,
+                          const uint8_t* seed, fhe_b200_ksk** out, void* stream);
 
 /* &Ciphertext * &Ciphertext (bfv/ops/mod.rs:259-358): n parts x m parts -> n + m - 1 parts (out3 must have that many;
  * 2 x 2 -> 3 is the fused path) */

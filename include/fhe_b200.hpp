@@ -20,6 +20,7 @@
 #include <algorithm>
 #include <memory>
 #include <mutex>
+#include <set>
 #include <stdexcept>
 #include <string>
 #include <type_traits>
@@ -150,6 +151,7 @@ class PinnedWords {
 };
 
 class PlaintextVec;
+class RGSWCiphertext;
 
 class Ciphertext {
  public:
@@ -406,8 +408,12 @@ class SecretKey {
     ct.sync();
     return out;
   }
+  // SecretKey::try_encrypt into RGSWCiphertext (rgsw_ciphertext.rs:94-120) of every plaintext of pts, at their level,
+  // in one device call; seed as for try_encrypt
+  inline std::vector<RGSWCiphertext> try_encrypt_rgsw(const PlaintextVec& pts, const uint8_t* seed = nullptr) const;
   const std::vector<int64_t>& coeffs() const { return coeffs_; }
   const std::shared_ptr<BfvParameters>& par() const { return par_; }
+  const fhe_b200_secret_key* handle() const { return h_; }
 
  private:
   Ciphertext encrypt_into(const Ciphertext* pts, uint32_t count, uint32_t level, const uint8_t* seed, void* stream) const;
@@ -469,14 +475,35 @@ class KeySwitchingKey {
   // c0, c1: NTT-domain words [n_digits][ksk_limbs][N] of the key polynomials (key_switching_key.rs:22-45)
   KeySwitchingKey(std::shared_ptr<BfvParameters> par, const std::vector<uint64_t>& c0, const std::vector<uint64_t>& c1,
                   uint32_t n_digits, uint32_t ciphertext_level = 0, uint32_t ksk_level = 0)
-      : par_(std::move(par)), ciphertext_level_(ciphertext_level), ksk_level_(ksk_level) {
+      : par_(std::move(par)), ciphertext_level_(ciphertext_level), ksk_level_(ksk_level), n_digits_(n_digits) {
     check(fhe_b200_ksk_upload(par_->handle(), ciphertext_level, ksk_level, c0.data(), c1.data(), n_digits, &h_));
+  }
+  // takes ownership of a key the library generated on `stream` (fhe_b200_relin_key_generate and the other generators)
+  KeySwitchingKey(std::shared_ptr<BfvParameters> par, fhe_b200_ksk* generated, uint32_t ciphertext_level,
+                  uint32_t ksk_level, void* stream)
+      : par_(std::move(par)), h_(generated), ciphertext_level_(ciphertext_level), ksk_level_(ksk_level),
+        stream_(stream) {
+    const std::vector<uint64_t> q = par_->moduli();   // key_switching_key.rs:92-126
+    n_digits_ = log_base() ? (bits(q[0] - 1) + log_base() - 1) / log_base() : (uint32_t)(q.size() - ciphertext_level);
   }
   KeySwitchingKey(const KeySwitchingKey&) = delete;
   ~KeySwitchingKey() { fhe_b200_ksk_free(h_); }
   const fhe_b200_ksk* handle() const { return h_; }
   uint32_t ciphertext_level() const { return ciphertext_level_; }
   uint32_t ksk_level() const { return ksk_level_; }
+  uint32_t n_digits() const { return n_digits_; }
+  // a key level with one modulus decomposes in base 2^(log_modulus / 2) (key_switching_key.rs:92-97), else 0
+  uint32_t log_base() const {
+    const std::vector<uint64_t> q = par_->moduli();
+    return q.size() - ksk_level_ == 1 ? bits(q[0] - 1) / 2 : 0;
+  }
+  // the key's words read back from the device: c0, c1 [n_digits][ksk_limbs][N] (NTT)
+  std::pair<std::vector<uint64_t>, std::vector<uint64_t>> arrays() const {
+    const size_t n = (size_t)n_digits_ * (par_->moduli().size() - ksk_level_) * par_->degree();
+    std::pair<std::vector<uint64_t>, std::vector<uint64_t>> w{std::vector<uint64_t>(n), std::vector<uint64_t>(n)};
+    check(fhe_b200_ksk_download(h_, w.first.data(), w.second.data(), stream_));
+    return w;
+  }
   // KeySwitchingKey::key_switch (key_switching_key.rs:241-270, :323-362) on polynomial `part` of a power-basis batch:
   // the (c0, c1) pair as a 2-part NTT batch at the key level
   Ciphertext key_switch(const Ciphertext& p, uint32_t part = 0) const {
@@ -487,14 +514,27 @@ class KeySwitchingKey {
   const std::shared_ptr<BfvParameters>& par() const { return par_; }
 
  private:
+  static uint32_t bits(uint64_t v) { uint32_t b = 0; while (v) { b++; v >>= 1; } return b; }
   std::shared_ptr<BfvParameters> par_;
   fhe_b200_ksk* h_ = nullptr;
-  uint32_t ciphertext_level_, ksk_level_;
+  uint32_t ciphertext_level_, ksk_level_, n_digits_ = 0;
+  void* stream_ = nullptr;
 };
 
 class RelinearizationKey {
  public:
   explicit RelinearizationKey(std::shared_ptr<KeySwitchingKey> ksk) : ksk(std::move(ksk)) {}
+  // RelinearizationKey::new / new_leveled (relinearization_key.rs:28-65), generated on the device from the seeded
+  // stream (seed as for SecretKey::try_encrypt)
+  static RelinearizationKey new_key(const SecretKey& sk, const uint8_t* seed = nullptr) { return new_leveled(sk, 0, 0, seed); }
+  static RelinearizationKey new_leveled(const SecretKey& sk, uint32_t ciphertext_level, uint32_t key_level,
+                                        const uint8_t* seed = nullptr) {
+    const EncryptionSeed s(seed);
+    fhe_b200_ksk* h = nullptr;
+    check(fhe_b200_relin_key_generate(sk.handle(), ciphertext_level, key_level, sk.par()->variance(), s.bytes, &h,
+                                      nullptr));
+    return RelinearizationKey(std::make_shared<KeySwitchingKey>(sk.par(), h, ciphertext_level, key_level, nullptr));
+  }
   // RelinearizationKey::relinearizes (relinearization_key.rs:70): (c0,c1,c2) -> (c0,c1)
   Ciphertext relinearizes(const Ciphertext& ct) const {
     Ciphertext out(ct.par(), ct.count(), 2, ct.level(), Representation::Ntt, ct.stream());
@@ -507,6 +547,26 @@ class RelinearizationKey {
 class GaloisKey {
  public:
   GaloisKey(uint32_t exponent, std::shared_ptr<KeySwitchingKey> ksk) : exponent(exponent), ksk(std::move(ksk)) {}
+  // GaloisKey::new (galois_key.rs:26-60), generated on the device (seed as for SecretKey::try_encrypt)
+  static GaloisKey new_key(const SecretKey& sk, uint64_t exponent, uint32_t ciphertext_level = 0, uint32_t key_level = 0,
+                           const uint8_t* seed = nullptr) {
+    return std::move(generate(sk, {exponent}, ciphertext_level, key_level, seed)[0]);
+  }
+  // one device call for every exponent (reduced mod 2N): key k of the call (stream word 13) is exponents[k]
+  static std::vector<GaloisKey> generate(const SecretKey& sk, const std::vector<uint64_t>& exponents,
+                                         uint32_t ciphertext_level, uint32_t key_level, const uint8_t* seed = nullptr) {
+    const EncryptionSeed s(seed);
+    const uint64_t two_n = 2 * (uint64_t)sk.par()->degree();
+    std::vector<uint32_t> e;
+    for (uint64_t x : exponents) e.push_back((uint32_t)(x % two_n));   // SubstitutionExponent::new (rq/mod.rs:99-106)
+    std::vector<fhe_b200_ksk*> h(std::max<size_t>(1, e.size()), nullptr);
+    check(fhe_b200_galois_keys_generate(sk.handle(), e.data(), (uint32_t)e.size(), ciphertext_level, key_level,
+                                        sk.par()->variance(), s.bytes, h.data(), nullptr));
+    std::vector<GaloisKey> out;
+    for (size_t k = 0; k < e.size(); k++)
+      out.emplace_back(e[k], std::make_shared<KeySwitchingKey>(sk.par(), h[k], ciphertext_level, key_level, nullptr));
+    return out;
+  }
   // GaloisKey::relinearize (galois_key.rs:63)
   Ciphertext relinearize(const Ciphertext& ct) const {
     Ciphertext out(ct.par(), ct.count(), 2, ct.level(), Representation::Ntt, ct.stream());
@@ -609,6 +669,79 @@ class EvaluationKey {
   }
   std::shared_ptr<BfvParameters> par_;
   std::map<uint32_t, std::shared_ptr<GaloisKey>> gk_;
+};
+
+inline std::vector<RGSWCiphertext> SecretKey::try_encrypt_rgsw(const PlaintextVec& pts, const uint8_t* seed) const {
+  const EncryptionSeed s(seed);
+  const Ciphertext& b = pts.batch();
+  std::vector<fhe_b200_ksk*> h(2 * (size_t)b.count(), nullptr);
+  check(fhe_b200_rgsw_encrypt(h_, b.handle(), par_->variance(), s.bytes, h.data(), b.stream()));
+  std::vector<std::shared_ptr<KeySwitchingKey>> k;   // adopt every handle before anything can throw
+  for (fhe_b200_ksk* x : h) k.push_back(std::make_shared<KeySwitchingKey>(par_, x, b.level(), b.level(), b.stream()));
+  std::vector<RGSWCiphertext> out;
+  for (size_t p = 0; p < b.count(); p++) out.emplace_back(k[2 * p], k[2 * p + 1]);
+  return out;
+}
+
+// fhe::bfv::EvaluationKeyBuilder (keys/evaluation_key.rs:318-491): the Galois keys of an EvaluationKey, generated on
+// the device in one call
+class EvaluationKeyBuilder {
+ public:
+  explicit EvaluationKeyBuilder(const SecretKey& sk) : sk_(sk) {}
+  // evaluation_key.rs:353-383
+  static EvaluationKeyBuilder new_leveled(const SecretKey& sk, uint32_t ciphertext_level, uint32_t evaluation_key_level) {
+    if (ciphertext_level > sk.par()->max_level()) throw Error(FHE_B200_INVALID_LEVEL, "InvalidLevel");
+    if (evaluation_key_level > ciphertext_level) throw Error(FHE_B200_INVALID_LEVEL, "InvalidLevel");
+    EvaluationKeyBuilder b(sk);
+    b.ciphertext_level_ = ciphertext_level;
+    b.key_level_ = evaluation_key_level;
+    return b;
+  }
+  EvaluationKeyBuilder& enable_expansion(uint32_t level) {   // evaluation_key.rs:386-398
+    uint32_t max_level = 0;
+    while ((2ull << max_level) <= sk_.par()->degree()) max_level++;
+    if (level > max_level) throw Error(FHE_B200_INVALID_LEVEL, "InvalidLevel");
+    expansion_level_ = level;
+    return *this;
+  }
+  EvaluationKeyBuilder& enable_inner_sum() { inner_sum_ = true; return *this; }
+  EvaluationKeyBuilder& enable_row_rotation() { row_rotation_ = true; return *this; }
+  EvaluationKeyBuilder& enable_column_rotation(uint32_t i) {   // evaluation_key.rs:414-426: steps 1 .. N/2 - 1
+    if (i < 1 || i >= sk_.par()->degree() / 2) throw Error(FHE_B200_INVALID_ARGUMENT, "EvaluationKeyError::InvalidRotationStep");
+    columns_.insert(column_exponent(i));
+    return *this;
+  }
+  // the Galois exponents build() generates keys for (evaluation_key.rs:439-463), ascending
+  std::vector<uint64_t> exponents() const {
+    const uint64_t n = sk_.par()->degree();
+    std::set<uint64_t> idx(columns_.begin(), columns_.end());
+    if (row_rotation_ || inner_sum_) idx.insert(2 * n - 1);
+    if (inner_sum_)
+      for (uint64_t i = 1; i < n / 2; i *= 2) idx.insert(column_exponent((uint32_t)i));
+    for (uint32_t l = 0; l < expansion_level_; l++) idx.insert((n >> l) + 1);
+    return std::vector<uint64_t>(idx.begin(), idx.end());
+  }
+  // EvaluationKeyBuilder::build (evaluation_key.rs:429-491): every Galois key in one device call, the exponents
+  // ascending, so a seed fixes the key of each exponent
+  EvaluationKey build(const uint8_t* seed = nullptr) const {
+    EvaluationKey ek(sk_.par());
+    const std::vector<uint64_t> e = exponents();
+    if (e.empty()) return ek;
+    for (GaloisKey& gk : GaloisKey::generate(sk_, e, ciphertext_level_, key_level_, seed))
+      ek.add_galois_key(std::make_shared<GaloisKey>(std::move(gk)));
+    return ek;
+  }
+
+ private:
+  uint64_t column_exponent(uint32_t i) const {   // evaluation_key.rs:278-286
+    uint64_t e = 1, m = 2 * sk_.par()->degree();
+    for (uint32_t k = 0; k < i; k++) e = e * 3 % m;
+    return e;
+  }
+  const SecretKey& sk_;
+  uint32_t ciphertext_level_ = 0, key_level_ = 0, expansion_level_ = 0;
+  bool inner_sum_ = false, row_rotation_ = false;
+  std::set<uint64_t> columns_;
 };
 
 // fhe::bfv::dot_product_scalar (bfv/ops/dot_product.rs:55): out[g] = sum_{i<n_terms} cts[g*n_terms+i] * pts[g*n_terms+i];

@@ -250,6 +250,12 @@ inline std::string encode_galois_key(const std::string& ksk, uint32_t exponent) 
   put_uint(out, 2, exponent);
   return out;
 }
+inline std::string encode_rgsw(const std::string& ksk0, const std::string& ksk1) {   // rgsw_ciphertext.rs:30-37
+  std::string out;
+  put_len(out, 1, ksk0);
+  put_len(out, 2, ksk1);
+  return out;
+}
 // ---- SecretKey (bfv.proto:54-56: repeated sint64 coeffs = 1, packed, zig-zag) -------------------------------------
 // SecretKey::to_bytes (secret_key.rs:142-148)
 inline std::string encode_secret_key(const int64_t* coeffs, size_t n) {
@@ -447,6 +453,34 @@ inline GaloisKey galois_key_from_bytes(std::shared_ptr<BfvParameters> par, const
   if (!(exponent & 1)) throw WireError("InvalidSubstitutionExponent", FHE_B200_INVALID_EXPONENT);
   return GaloisKey(exponent, std::move(ksk));
 }
+// KeySwitchingKeyProto::from(&ksk).encode_to_vec() (key_switching_key.rs:365-386), unseeded branch: the words read
+// back from the device, every c0_i and c1_i as an Rq with representation NTTSHOUP (packed on the device)
+inline std::string to_bytes(const KeySwitchingKey& k) {
+  const auto w = k.arrays();
+  const uint32_t nd = k.n_digits(), deg = (uint32_t)k.par()->degree();
+  const size_t poly = w.first.size() / nd;
+  std::vector<uint64_t> both(2 * w.first.size());   // [digit][c0, c1][limb][N]
+  for (uint32_t i = 0; i < nd; i++) {
+    std::memcpy(&both[(2 * (size_t)i) * poly], &w.first[(size_t)i * poly], poly * 8);
+    std::memcpy(&both[(2 * (size_t)i + 1) * poly], &w.second[(size_t)i * poly], poly * 8);
+  }
+  const Ciphertext tmp = Ciphertext::from_host(k.par(), both, nd, 2, k.ksk_level());
+  const size_t nbytes = tmp.packed_bytes();
+  const std::vector<uint8_t> blobs = tmp.to_packed();
+  tmp.sync();
+  std::vector<std::string> c0(nd), c1(nd);
+  for (uint32_t i = 0; i < nd; i++) {
+    c0[i] = wire::encode_rq(wire::REP_NTTSHOUP, deg, blobs.data() + (2 * (size_t)i) * nbytes, nbytes);
+    c1[i] = wire::encode_rq(wire::REP_NTTSHOUP, deg, blobs.data() + (2 * (size_t)i + 1) * nbytes, nbytes);
+  }
+  return wire::encode_ksk(c0, c1, std::string(), k.ciphertext_level(), k.ksk_level(), k.log_base());
+}
+// RelinearizationKey::to_bytes (relinearization_key.rs:113-119, :137-141), GaloisKey::to_bytes (galois_key.rs:146-153),
+// RGSWCiphertext::to_bytes (rgsw_ciphertext.rs:30-37)
+inline std::string to_bytes(const RelinearizationKey& rk) { return wire::encode_relinearization_key(to_bytes(*rk.ksk)); }
+inline std::string to_bytes(const GaloisKey& gk) { return wire::encode_galois_key(to_bytes(*gk.ksk), gk.exponent); }
+inline std::string to_bytes(const RGSWCiphertext& r) { return wire::encode_rgsw(to_bytes(*r.ksk0), to_bytes(*r.ksk1)); }
+
 // SecretKey::to_bytes / from_bytes (secret_key.rs:142-175)
 inline std::string to_bytes(const SecretKey& sk) { return wire::encode_secret_key(sk.coeffs().data(), sk.coeffs().size()); }
 inline std::unique_ptr<SecretKey> secret_key_from_bytes(std::shared_ptr<BfvParameters> par, const std::string& data) {
