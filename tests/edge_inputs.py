@@ -240,3 +240,80 @@ def residue_rows(moduli: Sequence[int], degree: int) -> Dict[str, np.ndarray]:
         "one_first": first,
         "one_last": last,
     }
+
+
+# ------------------------------------------------------------------------------------------------ modulus widths
+
+def prime_of_width(bits: int, degree: int, k: int = 0) -> int:
+    """the k-th NTT-friendly prime (== 1 mod 2N) of exactly `bits` bits, from the top (the generator's order)"""
+    import fhe_oracle as O
+    ub = 1 << bits
+    for _ in range(k + 1):
+        ub = O.generate_prime(bits, 2 * degree, ub)
+    return ub
+
+
+def decomposition_moduli(q0_bits: int, degree: int) -> List[int]:
+    """a q_0 of the given width followed by two 62-bit moduli: the last level's key decomposes q_0 in base
+    2^(bits / 2), in 3 digits when the width is odd and 2 when it is even"""
+    import fhe_oracle as O
+    return O.BfvParameters.generate_moduli([q0_bits, 62, 62], degree)
+
+
+# name -> (degree, t, moduli sizes).  The N = 64 sets cover every width from 10 to 62 once; two start narrow (q_0 of
+# 10 and 11 bits), two wide (60 and 61 bits); t = 257 is below every q_0 and a SIMD modulus at N = 64.
+WIDTH_SETS = {
+    "n64_up_10": (64, 257, list(range(10, 63, 4))),
+    "n64_up_11": (64, 257, list(range(11, 63, 4))),
+    "n64_down_60": (64, 257, list(range(60, 9, -4))),
+    "n64_down_61": (64, 257, list(range(61, 9, -4))),
+    "n2_13": (1 << 13, 786433, [61, 55, 47, 39, 31, 23, 17]),
+}
+
+
+def lazy_bound_bases(degree: int) -> Dict[str, List[int]]:
+    """Bases around the reduce-on-load decision of the RNS-digit transform (a digit below q_i goes into the forward
+    transform modulo q_j unreduced while max q_i <= 4 min q_j - 1):
+      * "unreduced": q_j the first NTT-friendly prime above 2^60 and q_i primes just below 2^62: an all-(q_i - 1)
+        digit sits a hair under 4 q_j, and the transform takes it as it is;
+      * "reduced": q_j the first one below 2^60 with 4 q_j < q_i (q_i the same primes): the same digits are at or
+        above 4 q_j, and are reduced on load;
+      * "reduced_8x": q_j the first one above 2^59: the digits reach 8 q_j - 2^52, far above 4 q_j (and below the
+        8 q_j a laxer threshold might allow).
+    Only an unreduced digit >= 4 q_j would tell a skipped reduction, and the lazy forward transform keeps even those
+    exact: its first butterfly subtracts 2p once (X < x), every output stays below max(x, 4p) < 2^64, the Shoup
+    products are exact for any 64-bit operand, and the inner product after the transform reduces whatever it gets."""
+    import fhe_oracle as O
+    m = 2 * degree
+
+    def first_above(x):
+        p = x // m * m + 1
+        while p < x or not O.is_prime(p):
+            p += m
+        return p
+    up, up59 = first_above(1 << 60), first_above(1 << 59)
+    big = [prime_of_width(62, degree, k) for k in range(2)]
+    down = O.generate_prime(60, m, min(big) // 4 + 1)
+    assert max(big) - 1 < 4 * up - 1 and 4 * down < min(big) and 4 * up59 < min(big) and max(big) < 8 * up59
+    return {"unreduced": [big[0], up, big[1]], "reduced": [big[0], down, big[1]], "reduced_8x": [big[0], up59, big[1]]}
+
+
+def pack_rows(q: int, degree: int, rng: np.random.Generator) -> Dict[str, np.ndarray]:
+    """[N] power-basis rows for the bit packer of a modulus q: 0, q - 1, alternating 0 / q - 1, random below q; and
+    fields no reduced word reaches, which a message may still carry (transcode_from_bytes yields up to 2^nbits - 1
+    < 2q): q itself, all 2^nbits - 1, alternating q / 2^nbits - 1, random in [q, 2^nbits)"""
+    top = (1 << (q - 1).bit_length()) - 1
+    alt = np.zeros(degree, np.uint64)
+    alt[1::2] = q - 1
+    over = np.full(degree, q, np.uint64)
+    over[1::2] = top
+    return {
+        "zero": np.zeros(degree, np.uint64),
+        "max": np.full(degree, q - 1, np.uint64),
+        "alternating": alt,
+        "random": rng.integers(0, q, size=degree, dtype=np.uint64),
+        "field_q": np.full(degree, q, np.uint64),
+        "field_top": np.full(degree, top, np.uint64),
+        "field_alternating": over,
+        "field_random": rng.integers(q, top, size=degree, dtype=np.uint64, endpoint=True),
+    }
