@@ -5,3 +5,4 @@ tlepoint/fhe.rs, behind the C ABI of include/fhe_b200.h.
 extension (libfhe_b200.so) is mandatory: there is no CPU fallback."""
 from . import _capi  # noqa: F401
 from .bfv import *  # noqa: F401,F403
+from . import mbfv  # noqa: F401,E402  (fhe::mbfv, multiparty BFV)

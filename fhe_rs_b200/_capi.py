@@ -73,6 +73,20 @@ SYMBOLS = {
     "fhe_b200_relin_key_generate": (_i, [_vp, _u32, _u32, _u32, _vp, _pp, _vp]),
     "fhe_b200_galois_keys_generate": (_i, [_vp, _vp, _u32, _u32, _u32, _u32, _vp, _pp, _vp]),
     "fhe_b200_rgsw_encrypt": (_i, [_vp, _vp, _u32, _vp, _pp, _vp]),
+    "fhe_b200_crp_generate": (_i, [_vp, _vp, _vp, _vp]),
+    "fhe_b200_pk_share": (_i, [_vp, _vp, _u32, _vp, _vp, _vp]),
+    "fhe_b200_pk_aggregate": (_i, [_pp, _u32, _vp, _vp, _vp]),
+    "fhe_b200_shares_sum": (_i, [_pp, _u32, _vp, _vp]),
+    "fhe_b200_sks_share": (_i, [_vp, _vp, _vp, _u32, _vp, _vp, _vp]),
+    "fhe_b200_sks_aggregate": (_i, [_vp, _pp, _u32, _vp, _vp]),
+    "fhe_b200_pks_share": (_i, [_vp, _vp, _vp, _u32, _vp, _vp, _vp]),
+    "fhe_b200_pks_aggregate": (_i, [_vp, _pp, _u32, _vp, _vp]),
+    "fhe_b200_decryption_aggregate": (_i, [_vp, _vp, _pp, _u32, _vp, _vp]),
+    "fhe_b200_rkg_create": (_i, [_vp, _vp, _u32, _vp, _pp, _vp]),
+    "fhe_b200_rkg_free": (_i, [_vp]),
+    "fhe_b200_rkg_round1": (_i, [_vp, _vp, _vp, _vp, _vp]),
+    "fhe_b200_rkg_round2": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "fhe_b200_rkg_aggregate": (_i, [_pp, _pp, _u32, _vp, _pp, _vp]),
     "fhe_b200_mul": (_i, [_vp, _vp, _vp, _vp]),
     "fhe_b200_relinearize": (_i, [_vp, _vp, _vp, _vp]),
     "fhe_b200_mul_relin": (_i, [_vp, _vp, _vp, _i, _vp, _vp]),

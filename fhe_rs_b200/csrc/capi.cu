@@ -315,6 +315,10 @@ struct fhe_b200_encoder {
   u32* d_inv_map = nullptr;             // coefficient index -> slot
   int* d_index_map = nullptr;           // index_map on the device (the decoders' gather)
   RowIds t_ids;                         // one row per plaintext, all modulo t
+  // cipher_plain_context.scaler of each level (parameters.rs:638-643), built on first use by
+  // fhe_b200_decryption_aggregate: the aggregator of a collective decryption holds no secret key
+  std::mutex mu;
+  std::map<u32, std::unique_ptr<ScalerData>> plain_scalers;
   std::vector<void*> d_allocs;
   template <typename T>
   T* to_dev(const std::vector<T>& v) {
@@ -1382,6 +1386,18 @@ int fhe_b200_add_plain_batch(fhe_b200_batch* a, const fhe_b200_batch* pts, int s
 }
 
 // ---- decryption, decoding and noise measurement
+// the plaintext context: the first moduli whose sizes add up to bits(t) + 60 (parameters.rs:579-595)
+static u32 plaintext_moduli_count(const fhe_b200_params* p) {
+  const size_t t_bits = p->t.bits();
+  u32 pc = 0, acc = 0;
+  for (u32 sz : p->moduli_sizes) {
+    acc += sz;
+    pc++;
+    if (acc >= t_bits + 60) break;
+  }
+  return std::min(std::max(pc, 1u), p->Lmax);
+}
+
 int fhe_b200_secret_key_create(const fhe_b200_params* p, const int64_t* coeffs, fhe_b200_secret_key** out) {
   API_BEGIN
   REQUIRE(p && coeffs && out, FHE_B200_INVALID_ARGUMENT, "null argument");
@@ -1416,16 +1432,7 @@ int fhe_b200_secret_key_create(const fhe_b200_params* p, const int64_t* coeffs, 
   launch_ntt(sk->s, sk->s, Lmax, l0.ctx_ids, p->d_limbs, p->logn, false, 1, false, nullptr);   // into_ntt
   FHE_CUDA(cudaGetLastError());
   FHE_CUDA(cudaStreamSynchronize(nullptr));
-  // the plaintext context: the first moduli whose sizes add up to bits(t) + 60 (parameters.rs:579-595)
-  const size_t t_bits = p->t.bits();
-  u32 pc = 0, acc = 0;
-  for (u32 sz : p->moduli_sizes) {
-    acc += sz;
-    pc++;
-    if (acc >= t_bits + 60) break;
-  }
-  pc = std::min(std::max(pc, 1u), Lmax);
-  const std::vector<u64> plain(p->moduli.begin(), p->moduli.begin() + pc);
+  const std::vector<u64> plain(p->moduli.begin(), p->moduli.begin() + plaintext_moduli_count(p));
   const RnsContextH to(plain);
   sk->levels.resize(Lmax);
   for (u32 lv = 0; lv < Lmax; lv++) {
@@ -1677,29 +1684,39 @@ int fhe_b200_encrypt_sk(const fhe_b200_secret_key* sk, const fhe_b200_batch* pts
   API_END
 }
 
-int fhe_b200_encrypt_pk(const fhe_b200_batch* pk, const fhe_b200_batch* pts, uint32_t variance, const uint8_t* seed,
-                        fhe_b200_batch* out, void* stream) {
-  API_BEGIN
-  check_variance(variance);
+// the checks of a public key operand: one 2-part level-0 NTT ciphertext
+static void check_public_key(const fhe_b200_batch* pk) {
   REQUIRE(pk, FHE_B200_INVALID_ARGUMENT, "null argument");
-  const fhe_b200_params* par = pk->par;
   REQUIRE(!pk->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
   REQUIRE(pk->count == 1 && pk->parts == 2, FHE_B200_INVALID_ARGUMENT, "a public key is one 2-part ciphertext");
   REQUIRE(pk->level == 0, FHE_B200_INVALID_LEVEL, "InvalidPublicKeyLevel: " + std::to_string(pk->level));
   need_repr(pk, FHE_B200_NTT);
+}
+
+// the public key's c at `level`: the key itself at level 0, else a copy in ws switched down to the level
+// (public_key.rs:60-70), enqueued on st
+static const u64* public_key_at_level(const fhe_b200_batch* pk, u32 level, Workspace& ws, cudaStream_t st) {
+  if (level == 0) return pk->d;
+  const fhe_b200_params* par = pk->par;
+  u64* sw = ws.words(((size_t)2 * par->Lmax) << par->logn);
+  FHE_CUDA(cudaMemcpyAsync(sw, pk->d, pk->words_per_ct() * sizeof(u64), cudaMemcpyDeviceToDevice, st));
+  for (u32 l = 0; l < level; l++) switch_down_polys(par, l, sw, 2, ws, st);
+  return sw;
+}
+
+int fhe_b200_encrypt_pk(const fhe_b200_batch* pk, const fhe_b200_batch* pts, uint32_t variance, const uint8_t* seed,
+                        fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  check_variance(variance);
+  check_public_key(pk);
+  const fhe_b200_params* par = pk->par;
   const EncSeed K = check_encrypt(par, pts, seed, out);
   DeviceGuard g(par);
   const LevelData& lv = par->level(out->level);
   const u32 L = lv.L, logn = par->logn;
   cudaStream_t user = (cudaStream_t)stream;
   Workspace key_ws(par, user);
-  const u64* c = pk->d;
-  if (out->level > 0) {   // a copy of the key switched down to the plaintext level (public_key.rs:60-70)
-    u64* sw = key_ws.words(((size_t)2 * par->Lmax) << logn);
-    FHE_CUDA(cudaMemcpyAsync(sw, pk->d, pk->words_per_ct() * sizeof(u64), cudaMemcpyDeviceToDevice, user));
-    for (u32 l = 0; l < out->level; l++) switch_down_polys(par, l, sw, 2, key_ws, user);
-    c = sw;
-  }
+  const u64* c = public_key_at_level(pk, out->level, key_ws, user);
   ChunkRunner chunks(par, out->count, user);
   chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
     Workspace ws(par, st);
@@ -1859,6 +1876,462 @@ int fhe_b200_rgsw_encrypt(const fhe_b200_secret_key* sk, const fhe_b200_batch* p
                   else FHE_CUDA(cudaMemcpyAsync(x, m, words * sizeof(u64), cudaMemcpyDeviceToDevice, st));
                 },
                 out, (cudaStream_t)stream);
+  API_END
+}
+
+// ---- multiparty BFV (fhe::mbfv, crates/fhe/src/mbfv).  Experimental, incomplete, not audited, as the reference's
+// module: the share errors are the ordinary variance errors, not smudging noise.
+// a batch argument of this parameter set, over the level's own basis, NTT
+static void check_operand(const fhe_b200_params* par, const fhe_b200_batch* b) {
+  REQUIRE(b, FHE_B200_INVALID_ARGUMENT, "null argument");
+  REQUIRE(b->par == par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch");
+  REQUIRE(!b->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
+  need_repr(b, FHE_B200_NTT);
+}
+// a 2-part ciphertext batch (InvalidPolynomialCount otherwise, secret_key_switch.rs:56-64)
+static void check_ciphertexts(const fhe_b200_params* par, const fhe_b200_batch* ct) {
+  check_operand(par, ct);
+  REQUIRE(ct->parts == 2, FHE_B200_BAD_POLY_COUNT, "InvalidPolynomialCount: multiparty protocols take 2-part ciphertexts");
+}
+// an output batch: `parts` polynomials per entry, `count` entries at `level`
+static void check_output(const fhe_b200_params* par, const fhe_b200_batch* out, u32 count, u32 parts, u32 level) {
+  REQUIRE(out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  REQUIRE(out->par == par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch");
+  REQUIRE(!out->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
+  REQUIRE(out->count == count && out->parts == parts && out->level == level, FHE_B200_INVALID_ARGUMENT,
+          "out must be a " + std::to_string(parts) + "-part batch of " + std::to_string(count) + " entries at level " +
+              std::to_string(level));
+}
+// n shares, every one of the shape (count, parts, level) (MultipartyError::NoShares for n == 0)
+static void check_shares(const fhe_b200_params* par, const fhe_b200_batch* const* shares, uint32_t n, u32 count,
+                         u32 parts, u32 level) {
+  REQUIRE(shares && n, FHE_B200_INVALID_ARGUMENT, "MultipartyError::NoShares");
+  for (uint32_t i = 0; i < n; i++) {
+    check_operand(par, shares[i]);
+    REQUIRE(shares[i]->count == count && shares[i]->parts == parts && shares[i]->level == level,
+            FHE_B200_INVALID_ARGUMENT, "share " + std::to_string(i) + " does not have the shape of the others");
+  }
+}
+
+// entries [c0, c0 + n) of the shares: out item k = base item k + the sum of item c0 + k of every share.  An item is
+// item_words words at word offset `part_off` of a share entry; base (nullable) and out point at the items of entry c0
+// and have their own strides.
+static void sum_shares(const fhe_b200_batch* const* shares, uint32_t n_sh, size_t part_off, size_t item_words,
+                       const u64* base, size_t base_stride, u64* out, size_t out_stride, u32 c0, u32 n,
+                       const LevelData& lv, cudaStream_t st) {
+  const fhe_b200_params* par = shares[0]->par;
+  const size_t src_stride = shares[0]->words_per_ct();
+  std::vector<const u64*> src(n_sh);
+  for (uint32_t i = 0; i < n_sh; i++) src[i] = shares[i]->d + (size_t)c0 * src_stride + part_off;
+  launch_shares_sum(src.data(), n_sh, src_stride, base, base_stride, out, out_stride, n, item_words, lv.ctx_ids,
+                    par->d_limbs, par->logn, st);
+}
+
+int fhe_b200_crp_generate(const fhe_b200_params* p, const uint8_t* seed, fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  REQUIRE(p && seed, FHE_B200_INVALID_ARGUMENT, "null argument");
+  DeviceGuard g(p);
+  REQUIRE(out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  check_output(p, out, out->count, 1, out->level);
+  const EncSeed K = seed_words(seed);
+  const LevelData& lv = p->level(out->level);
+  ChunkRunner chunks(p, out->count, (cudaStream_t)stream);
+  chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+    launch_crp(out->d + (((size_t)c0 * lv.L) << p->logn), n, c0, K, lv.ctx_ids, p->d_limbs, p->logn, st);
+  });
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
+  API_END
+}
+
+int fhe_b200_pk_share(const fhe_b200_secret_key* sk, const fhe_b200_batch* crp, uint32_t variance, const uint8_t* seed,
+                      fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  check_variance(variance);
+  REQUIRE(sk && seed, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = sk->par;
+  check_operand(par, crp);
+  REQUIRE(crp->parts == 1, FHE_B200_INVALID_ARGUMENT, "a crp batch holds one polynomial per entry");
+  REQUIRE(crp->level == 0, FHE_B200_INVALID_LEVEL, "InvalidLevel: a public key share is made at level 0");
+  check_output(par, out, crp->count, 1, 0);
+  const EncSeed K = seed_words(seed);
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(0);
+  const u32 L = lv.L, logn = par->logn;
+  ChunkRunner chunks(par, out->count, (cudaStream_t)stream);
+  chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace ws(par, st);
+    u64* e = ws.secret_words(((size_t)n * L) << logn);
+    launch_cbd(e, n, c0, 8, 1, variance, K, lv.ctx_ids, par->d_limbs, logn, st);
+    launch_ntt(e, e, n * L, lv.ctx_ids, par->d_limbs, logn, false, 1, false, st);
+    const size_t off = ((size_t)c0 * L) << logn;
+    launch_mbfv_share(SHARE_PK, sk->s, nullptr, crp->d + off, nullptr, e, out->d + off, n, lv.ctx_ids, par->d_limbs,
+                      logn, st);
+  });
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
+  API_END
+}
+
+int fhe_b200_pk_aggregate(const fhe_b200_batch* const* shares, uint32_t n, const fhe_b200_batch* crp,
+                          fhe_b200_batch* pk, void* stream) {
+  API_BEGIN
+  REQUIRE(crp, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = crp->par;
+  check_operand(par, crp);
+  REQUIRE(crp->parts == 1, FHE_B200_INVALID_ARGUMENT, "a crp batch holds one polynomial per entry");
+  REQUIRE(crp->level == 0, FHE_B200_INVALID_LEVEL, "InvalidLevel: a public key is made at level 0");
+  check_shares(par, shares, n, crp->count, 1, 0);
+  check_output(par, pk, crp->count, 2, 0);
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(0);
+  const size_t words = (size_t)lv.L << par->logn;
+  ChunkRunner chunks(par, pk->count, (cudaStream_t)stream);
+  chunks.run([&](u32 c0, u32 m, cudaStream_t st) {
+    // PublicKey { c: (sum p0_i, crp) } (public_key_gen.rs:60-77)
+    sum_shares(shares, n, 0, words, nullptr, 0, pk->d + 2 * (size_t)c0 * words, 2 * words, c0, m, lv, st);
+    FHE_CUDA(cudaMemcpy2DAsync(pk->d + (2 * (size_t)c0 + 1) * words, 2 * words * 8, crp->d + (size_t)c0 * words,
+                               words * 8, words * 8, m, cudaMemcpyDeviceToDevice, st));
+  });
+  FHE_CUDA(cudaGetLastError());
+  pk->repr = FHE_B200_NTT;
+  API_END
+}
+
+int fhe_b200_shares_sum(const fhe_b200_batch* const* shares, uint32_t n, fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  REQUIRE(out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = out->par;
+  check_operand(par, out);
+  check_shares(par, shares, n, out->count, out->parts, out->level);
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(out->level);
+  const size_t words = out->words_per_ct();
+  ChunkRunner chunks(par, out->count, (cudaStream_t)stream);
+  chunks.run([&](u32 c0, u32 m, cudaStream_t st) {
+    sum_shares(shares, n, 0, words, nullptr, 0, out->d + (size_t)c0 * words, words, c0, m, lv, st);
+  });
+  FHE_CUDA(cudaGetLastError());
+  API_END
+}
+
+int fhe_b200_sks_share(const fhe_b200_secret_key* sk_in, const fhe_b200_secret_key* sk_out, const fhe_b200_batch* ct,
+                       uint32_t variance, const uint8_t* seed, fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  check_variance(variance);
+  REQUIRE(sk_in && seed, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = sk_in->par;
+  REQUIRE(!sk_out || sk_out->par == par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch: input and output keys");
+  check_ciphertexts(par, ct);
+  check_output(par, out, ct->count, 1, ct->level);
+  const EncSeed K = seed_words(seed);
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(ct->level);
+  const u32 L = lv.L, logn = par->logn;
+  ChunkRunner chunks(par, ct->count, (cudaStream_t)stream);
+  chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace ws(par, st);
+    u64* e = ws.secret_words(((size_t)n * L) << logn);
+    launch_cbd(e, n, c0, 14, 1, variance, K, lv.ctx_ids, par->d_limbs, logn, st);
+    launch_ntt(e, e, n * L, lv.ctx_ids, par->d_limbs, logn, false, 1, false, st);
+    launch_mbfv_share(SHARE_SKS, sk_in->s, sk_out ? sk_out->s : nullptr, ct->d + ((2 * (size_t)c0 * L) << logn),
+                      nullptr, e, out->d + (((size_t)c0 * L) << logn), n, lv.ctx_ids, par->d_limbs, logn, st);
+  });
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
+  API_END
+}
+
+int fhe_b200_sks_aggregate(const fhe_b200_batch* ct, const fhe_b200_batch* const* shares, uint32_t n,
+                           fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  REQUIRE(ct, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = ct->par;
+  check_ciphertexts(par, ct);
+  check_shares(par, shares, n, ct->count, 1, ct->level);
+  check_output(par, out, ct->count, 2, ct->level);
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(ct->level);
+  const size_t words = (size_t)lv.L << par->logn;
+  ChunkRunner chunks(par, ct->count, (cudaStream_t)stream);
+  chunks.run([&](u32 c0, u32 m, cudaStream_t st) {
+    // (c0 + sum h_i, c1) (secret_key_switch.rs:98-115)
+    const size_t off = 2 * (size_t)c0 * words;
+    sum_shares(shares, n, 0, words, ct->d + off, 2 * words, out->d + off, 2 * words, c0, m, lv, st);
+    if (out != ct)
+      FHE_CUDA(cudaMemcpy2DAsync(out->d + (2 * (size_t)c0 + 1) * words, 2 * words * 8,
+                                 ct->d + (2 * (size_t)c0 + 1) * words, 2 * words * 8, words * 8, m,
+                                 cudaMemcpyDeviceToDevice, st));
+  });
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
+  API_END
+}
+
+int fhe_b200_pks_share(const fhe_b200_secret_key* sk, const fhe_b200_batch* pk, const fhe_b200_batch* ct,
+                       uint32_t variance, const uint8_t* seed, fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  check_variance(variance);
+  REQUIRE(sk && seed, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = sk->par;
+  check_public_key(pk);
+  REQUIRE(pk->par == par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch: secret key and public key");
+  check_ciphertexts(par, ct);
+  check_output(par, out, ct->count, 2, ct->level);
+  const EncSeed K = seed_words(seed);
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(ct->level);
+  const u32 L = lv.L, logn = par->logn;
+  cudaStream_t user = (cudaStream_t)stream;
+  Workspace key_ws(par, user);
+  const u64* c = public_key_at_level(pk, ct->level, key_ws, user);
+  ChunkRunner chunks(par, ct->count, user);
+  chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace ws(par, st);
+    u64* uee = ws.secret_words(((size_t)n * 3 * L) << logn);   // u, e0, e1
+    launch_cbd(uee, n, c0, 15, 3, variance, K, lv.ctx_ids, par->d_limbs, logn, st);
+    launch_ntt(uee, uee, n * 3 * L, lv.ctx_ids, par->d_limbs, logn, false, 1, false, st);
+    const size_t off = ((2 * (size_t)c0 * L) << logn);
+    launch_mbfv_share(SHARE_PKS, sk->s, nullptr, ct->d + off, c, uee, out->d + off, n, lv.ctx_ids, par->d_limbs, logn,
+                      st);
+  });
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
+  API_END
+}
+
+int fhe_b200_pks_aggregate(const fhe_b200_batch* ct, const fhe_b200_batch* const* shares, uint32_t n,
+                           fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  REQUIRE(ct, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = ct->par;
+  check_ciphertexts(par, ct);
+  check_shares(par, shares, n, ct->count, 2, ct->level);
+  check_output(par, out, ct->count, 2, ct->level);
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(ct->level);
+  const size_t words = (size_t)lv.L << par->logn;
+  ChunkRunner chunks(par, ct->count, (cudaStream_t)stream);
+  chunks.run([&](u32 c0, u32 m, cudaStream_t st) {
+    // (c0 + sum h0_i, sum h1_i) (public_key_switch.rs:95-112)
+    const size_t off = 2 * (size_t)c0 * words;
+    sum_shares(shares, n, 0, words, ct->d + off, 2 * words, out->d + off, 2 * words, c0, m, lv, st);
+    sum_shares(shares, n, words, words, nullptr, 0, out->d + off + words, 2 * words, c0, m, lv, st);
+  });
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
+  API_END
+}
+
+// RelinKeyGenerator (relin_key_gen.rs:36-96): the party's secret key, the level-0 CRPs a_i (one per level-0 limb,
+// borrowed as in the reference) and u on the device, erased when the generator is freed.
+struct fhe_b200_rkg {
+  const fhe_b200_params* par;   // a reference of its own: freeing the generator never reads sk
+  const fhe_b200_secret_key* sk;
+  const fhe_b200_batch* crp;
+  u32 variance;
+  u64* u;   // [Lmax][N] NTT
+};
+
+int fhe_b200_rkg_create(const fhe_b200_secret_key* sk, const fhe_b200_batch* crp, uint32_t variance,
+                        const uint8_t* seed, fhe_b200_rkg** out, void* stream) {
+  API_BEGIN
+  check_variance(variance);
+  REQUIRE(sk && seed && out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = sk->par;
+  REQUIRE(par->Lmax > 1, FHE_B200_UNSUPPORTED, "EvaluationKeyError::KeySwitchingNotSupported: a single modulus");
+  check_operand(par, crp);
+  REQUIRE(crp->parts == 1, FHE_B200_INVALID_ARGUMENT, "a crp batch holds one polynomial per entry");
+  REQUIRE(crp->level == 0, FHE_B200_INVALID_LEVEL, "InvalidLevel: the relinearization key protocol runs at level 0");
+  REQUIRE(crp->count == par->Lmax, FHE_B200_INVALID_ARGUMENT,
+          "MultipartyError::InvalidCommonRandomPolynomialCount: " + std::to_string(crp->count) + ", expected " +
+              std::to_string(par->Lmax));
+  const EncSeed K = seed_words(seed);
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(0);
+  const size_t words = (size_t)lv.L << par->logn;
+  DevPtr du;
+  FHE_CUDA(cudaMalloc(&du.p, words * sizeof(u64)));
+  cudaStream_t st = (cudaStream_t)stream;
+  launch_cbd((u64*)du.p, 1, 0, 9, 1, variance, K, lv.ctx_ids, par->d_limbs, par->logn, st);   // u: role 9
+  launch_ntt((u64*)du.p, (u64*)du.p, lv.L, lv.ctx_ids, par->d_limbs, par->logn, false, 1, false, st);
+  FHE_CUDA(cudaGetLastError());
+  std::unique_ptr<fhe_b200_rkg> r(new fhe_b200_rkg());
+  r->par = par; r->sk = sk; r->crp = crp; r->variance = variance;
+  r->u = (u64*)du.release();
+  params_retain(par);
+  *out = r.release();
+  API_END
+}
+
+int fhe_b200_rkg_free(fhe_b200_rkg* r) {
+  if (!r) return FHE_B200_OK;
+  const fhe_b200_params* par = r->par;
+  {
+    ScopedDevice g(par->device);
+    // u is erased as SecretKey's s is (fhe_b200_secret_key_free): wait for work that may still read it, then zero it
+    cudaDeviceSynchronize();
+    cudaMemset(r->u, 0, ((size_t)par->Lmax << par->logn) * sizeof(u64));
+    cudaDeviceSynchronize();
+    cudaFree(r->u);
+    cudaGetLastError();
+  }
+  params_release(par);
+  delete r;
+  return FHE_B200_OK;
+}
+
+// one round of the generator: entries i of h0, h1 (1-part level-0 batches of Lmax entries) from the errors of roles
+// role0, role0 + 1 (state word 15 = i)
+static void rkg_round(const fhe_b200_rkg* r, MbfvShare kind, const fhe_b200_batch* x, const fhe_b200_batch* y,
+                      const uint8_t* seed, fhe_b200_batch* h0, fhe_b200_batch* h1, u32 role0, cudaStream_t user) {
+  const fhe_b200_params* par = r->par;
+  const u32 L = par->Lmax, logn = par->logn;
+  check_output(par, h0, L, 1, 0);
+  check_output(par, h1, L, 1, 0);
+  REQUIRE(h0 != h1, FHE_B200_INVALID_ARGUMENT, "h0 and h1 must be different batches");
+  const EncSeed K = seed_words(seed);
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(0);
+  ChunkRunner chunks(par, L, user, std::max(1u, chunk_size() / (2 * L)));
+  chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace ws(par, st);
+    u64* e = ws.secret_words(((size_t)n * 2 * L) << logn);
+    launch_cbd(e, n, c0, role0, 2, r->variance, K, lv.ctx_ids, par->d_limbs, logn, st, L);
+    launch_ntt(e, e, n * 2 * L, lv.ctx_ids, par->d_limbs, logn, false, 1, false, st);
+    const size_t off = ((size_t)c0 * L) << logn;
+    launch_mbfv_share(kind, r->sk->s, nullptr, x->d + off, y ? y->d + off : nullptr, e, h0->d + off, n, lv.ctx_ids,
+                      par->d_limbs, logn, st, r->u, h1->d + off, c0);
+  });
+  FHE_CUDA(cudaGetLastError());
+  h0->repr = h1->repr = FHE_B200_NTT;
+}
+
+int fhe_b200_rkg_round1(const fhe_b200_rkg* r, const uint8_t* seed, fhe_b200_batch* h0, fhe_b200_batch* h1,
+                        void* stream) {
+  API_BEGIN
+  REQUIRE(r && seed, FHE_B200_INVALID_ARGUMENT, "null argument");
+  rkg_round(r, SHARE_RKG1, r->crp, nullptr, seed, h0, h1, 10, (cudaStream_t)stream);
+  API_END
+}
+
+int fhe_b200_rkg_round2(const fhe_b200_rkg* r, const fhe_b200_batch* r1_h0, const fhe_b200_batch* r1_h1,
+                        const uint8_t* seed, fhe_b200_batch* h0, fhe_b200_batch* h1, void* stream) {
+  API_BEGIN
+  REQUIRE(r && seed, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = r->par;
+  for (const fhe_b200_batch* b : {r1_h0, r1_h1}) {
+    check_operand(par, b);
+    REQUIRE(b->parts == 1 && b->count == par->Lmax, FHE_B200_INVALID_ARGUMENT,
+            "a round-1 aggregate holds one polynomial per level-0 limb");
+    REQUIRE(b->level == 0, FHE_B200_INVALID_LEVEL, "InvalidLevel: the round-1 aggregate is at level 0");
+  }
+  rkg_round(r, SHARE_RKG2, r1_h0, r1_h1, seed, h0, h1, 12, (cudaStream_t)stream);
+  API_END
+}
+
+int fhe_b200_rkg_aggregate(const fhe_b200_batch* const* h0s, const fhe_b200_batch* const* h1s, uint32_t n,
+                           const fhe_b200_batch* r1_h1, fhe_b200_ksk** out, void* stream) {
+  API_BEGIN
+  REQUIRE(r1_h1 && out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = r1_h1->par;
+  const u32 L = par->Lmax, logn = par->logn;
+  REQUIRE(L > 1, FHE_B200_UNSUPPORTED, "EvaluationKeyError::KeySwitchingNotSupported: a single modulus");
+  check_operand(par, r1_h1);
+  REQUIRE(r1_h1->parts == 1 && r1_h1->count == L, FHE_B200_INVALID_ARGUMENT,
+          "a round-1 aggregate holds one polynomial per level-0 limb");
+  REQUIRE(r1_h1->level == 0, FHE_B200_INVALID_LEVEL, "InvalidLevel: the round-1 aggregate is at level 0");
+  check_shares(par, h0s, n, L, 1, 0);
+  check_shares(par, h1s, n, L, 1, 0);
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(0);
+  const size_t words = (size_t)L << logn, row = (size_t)1 << logn;
+  DevPtr g0, g1;
+  FHE_CUDA(cudaMalloc(&g0.p, L * words * sizeof(u64)));
+  FHE_CUDA(cudaMalloc(&g1.p, L * words * sizeof(u64)));
+  std::vector<const fhe_b200_batch*> all(h0s, h0s + n);
+  all.insert(all.end(), h1s, h1s + n);
+  const fhe_b200_batch* r1[] = {r1_h1};
+  u64 *k0 = (u64*)g0.p, *k1 = (u64*)g1.p;
+  // digit i of the key: c0_i = sum h0'_i + sum h1'_i, c1_i = r1_h1_i, written straight into the key's device layout
+  // [limb j][digit i][N] (relin_key_gen.rs:299-350): item i of the sum starts at digit i's row, rows L * N apart
+  ChunkRunner chunks(par, L, (cudaStream_t)stream, std::max(1u, chunk_size() / L));
+  chunks.run([&](u32 c0, u32 m, cudaStream_t st) {
+    std::vector<const u64*> src(all.size());
+    for (size_t i = 0; i < all.size(); i++) src[i] = all[i]->d + (size_t)c0 * words;
+    launch_shares_sum(src.data(), (u32)src.size(), words, nullptr, 0, k0 + c0 * row, row, m, words, lv.ctx_ids,
+                      par->d_limbs, logn, st, L * row);
+    const u64* s1 = r1[0]->d + (size_t)c0 * words;
+    launch_shares_sum(&s1, 1, words, nullptr, 0, k1 + c0 * row, row, m, words, lv.ctx_ids, par->d_limbs, logn, st,
+                      L * row);
+  });
+  FHE_CUDA(cudaGetLastError());
+  std::unique_ptr<fhe_b200_ksk> k(new fhe_b200_ksk());
+  k->par = par; k->ct_level = 0; k->ksk_level = 0; k->n_dig = L; k->Lk = L; k->log_base = 0;
+  k->k0 = (u64*)g0.release();
+  k->k1 = (u64*)g1.release();
+  params_retain(par);
+  *out = k.release();
+  API_END
+}
+
+// cipher_plain_context.scaler of `level` (parameters.rs:638-643) on the encoder, built on first use
+static const ScalerDev& plain_scaler(const fhe_b200_encoder* ce, u32 level) {
+  fhe_b200_encoder* e = const_cast<fhe_b200_encoder*>(ce);
+  const fhe_b200_params* p = e->par;
+  std::lock_guard<std::mutex> lock(e->mu);
+  auto it = e->plain_scalers.find(level);
+  if (it != e->plain_scalers.end()) return it->second->dev;
+  const std::vector<u64> plain(p->moduli.begin(), p->moduli.begin() + plaintext_moduli_count(p));
+  const std::vector<u64> ctx(p->moduli.begin(), p->moduli.begin() + (p->Lmax - level));
+  const RnsContextH from(ctx), to(plain);
+  std::unique_ptr<ScalerData> s(new ScalerData());
+  s->h = make_scaler_tables(from, to, p->t, from.product);
+  upload_scaler_tables(*s, plain, [&](const auto& v) { return e->to_dev(v); }, [&](u64 q) { return p->prime_index(q); });
+  const ScalerDev& d = s->dev;
+  e->plain_scalers[level] = std::move(s);
+  return d;
+}
+
+int fhe_b200_decryption_aggregate(const fhe_b200_encoder* e, const fhe_b200_batch* ct,
+                                  const fhe_b200_batch* const* shares, uint32_t n, fhe_b200_batch* pts_out,
+                                  void* stream) {
+  API_BEGIN
+  REQUIRE(e, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = e->par;
+  DeviceGuard g(par);   // NO_DEVICE first: an encoder, unlike a batch, exists on a host-only parameter set
+  check_ciphertexts(par, ct);
+  check_shares(par, shares, n, ct->count, 1, ct->level);
+  check_output(par, pts_out, ct->count, 1, ct->level);
+  REQUIRE(par->t_small && par->t_mod.t < par->moduli[0], FHE_B200_UNSUPPORTED,
+          "Plaintext::from_shares needs t below the first ciphertext modulus");
+  const LevelData& lv = par->level(ct->level);
+  const ScalerDev& S = plain_scaler(e, ct->level);
+  const u32 L = lv.L, logn = par->logn;
+  const size_t words = (size_t)L << logn;
+  u64 qmin = ~0ull;
+  for (u32 j = 0; j < L; j++) qmin = std::min(qmin, par->moduli[j]);
+  const bool reduce = par->t_mod.t > 4 * qmin - 1;   // the lifted words are below t
+  const bool q0_context = plaintext_moduli_count(par) == 1;
+  ChunkRunner chunks(par, ct->count, (cudaStream_t)stream);
+  chunks.run([&](u32 c0, u32 m, cudaStream_t st) {
+    Workspace ws(par, st);
+    // c = c0 + sum h_i (secret_key_switch.rs:150-154), taken to the power basis and scaled by t / Q into limb 0 of the
+    // plaintext context; only that row is needed because the scaled value v has |v| <= t / 2 < q_0 / 2
+    u64* c = ws.secret_words(m * words);
+    sum_shares(shares, n, 0, words, ct->d + 2 * (size_t)c0 * words, 2 * words, c, words, c0, m, lv, st);
+    launch_ntt(c, c, m * L, lv.ctx_ids, par->d_limbs, logn, true, 1, false, st);
+    u64* w = ws.secret_words((size_t)m << logn);
+    launch_scale(S, par->d_limbs, c, w, nullptr, m, 1, 0, 1, 0, logn, st);
+    // w = ((v + t) mod Q_p) mod t over the plaintext context Q_p (:164-173).  With one plaintext modulus Q_p = q_0 and
+    // this is try_decrypt's lift; with more, (v + t) mod Q_p = v + t and w = v mod t.
+    const LimbDev& q0 = par->h_limbs[0];
+    if (q0_context) launch_decrypt_epilogue(w, (size_t)m << logn, PlainMod{q0.p, q0.bhi, q0.blo}, par->t_mod, st);
+    else launch_from_shares_epilogue(w, (size_t)m << logn, q0.p, par->t_mod, st);
+    launch_ntt(w, pts_out->d + (size_t)c0 * words, m * L, lv.ctx_ids, par->d_limbs, logn, false, L, reduce, st);
+  });
+  FHE_CUDA(cudaGetLastError());
+  pts_out->repr = FHE_B200_NTT;
   API_END
 }
 

@@ -199,6 +199,8 @@ void launch_phase(const u64* ct, const u64* s, u64* out, u32 cts, u32 parts, con
                   u32 logn, cudaStream_t st);
 // in place: v <- ((v + t) mod q_0) mod t   (Q0 = {q_0, Barrett constants})
 void launch_decrypt_epilogue(u64* v, size_t n_words, const PlainMod& Q0, const PlainMod& T, cudaStream_t st);
+// in place: the lift of Plaintext::from_shares over two or more plaintext moduli from limb 0 of the scaled value (t < q_0)
+void launch_from_shares_epilogue(u64* v, size_t n_words, u64 q0, const PlainMod& T, cudaStream_t st);
 // in place: Modulus::center, a - t when a >= t >> 1 (the words are read back as i64)
 void launch_center(u64* x, size_t n_words, u64 t, cudaStream_t st);
 // out[ct] = max(out[ct], max over the N coefficients of min(bits(x), bits(Q - x))), x the CRT lift of the L residues of
@@ -237,6 +239,24 @@ struct KskG {
 void launch_ksk_gen(const u64* s, const u64* e, const u64* x, u64* k0, u64* k1, u32 key, u32 digit0, u32 digits,
                     u32 n_dig, const KskG& G, const EncSeed& K, const RowIds& ids, const LimbDev* limbs, u32 logn,
                     cudaStream_t st);
+
+// ---- multiparty BFV (fhe::mbfv).  Experimental, incomplete, not audited, as the reference's module.
+// out [cts][L][N]: CommonRandomPoly k = ct_base + c (role 7, uniform NTT words)
+void launch_crp(u64* out, u32 cts, u32 ct_base, const EncSeed& K, const RowIds& ids, const LimbDev* limbs, u32 logn,
+                cudaStream_t st);
+// the share of one protocol per ciphertext (kernels.cu mbfv_share_kernel gives the operands of each)
+enum MbfvShare { SHARE_PK = 0, SHARE_SKS = 1, SHARE_PKS = 2, SHARE_RKG1 = 3, SHARE_RKG2 = 4 };
+void launch_mbfv_share(MbfvShare kind, const u64* s, const u64* s_out, const u64* x, const u64* pk, const u64* e,
+                       u64* out, u32 cts, const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st,
+                       const u64* u = nullptr, u64* out1 = nullptr, u32 ct_base = 0);
+// Aggregate: for items k < items, out item k = base item k (nullable) + sum_i src[i] item k, item_words words each
+// (rows of limb (row % limbs_per_poly)); sources are read once, in launches of kSumGroup sources, each output word
+// reduced once per launch.  Row r of an out item is at + r * out_row (0: N, contiguous rows; the key layout
+// [limb][digit][N] of fhe_b200_rkg_aggregate takes n_dig * N).  A source may be out.
+constexpr u32 kSumGroup = 64;
+void launch_shares_sum(const u64* const* src, u32 n_src, size_t src_stride, const u64* base, size_t base_stride,
+                       u64* out, size_t out_stride, u32 items, size_t item_words, const RowIds& ids,
+                       const LimbDev* limbs, u32 logn, cudaStream_t st, size_t out_row = 0);
 
 // bit (un)packing of power-basis rows (fhe-util/src/lib.rs:71-146): row r of `rows` uses nbits[r % limbs] bits per
 // coefficient; packed row r starts at byte  (r / limbs) * poly_bytes + offs[r % limbs]

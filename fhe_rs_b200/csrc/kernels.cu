@@ -5,6 +5,7 @@
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
+#include <vector>
 
 #include "engine.hpp"
 #include "ntt_tma.cuh"
@@ -1103,6 +1104,17 @@ __global__ void decrypt_epilogue_kernel(u64* v, size_t n_words, PlainMod Q0, Pla
   v[i] = barrett64(barrett64(v[i] + T.t, Q0.t, Q0.bhi, Q0.blo), T.t, T.bhi, T.blo);
 }
 
+// Plaintext::from_shares' lift (mbfv/secret_key_switch.rs:164-173) over a plaintext context of two or more moduli, from
+// limb 0 of the scaled value v = round(t x / Q), x the centred lift of the phase: |v| <= t / 2 < q_0 / 2, so v < 0
+// exactly when its residue r > q_0 / 2, and w = ((v + t) mod Q_p) mod t = (r + t - (v < 0 ? q_0 : 0)) mod t, as a
+// select
+__global__ void from_shares_epilogue_kernel(u64* v, size_t n_words, u64 q0, PlainMod T) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_words) return;
+  const u64 r = v[i];
+  v[i] = barrett64(r + T.t - (r > (q0 >> 1) ? q0 : 0), T.t, T.bhi, T.blo);
+}
+
 // Modulus::center (zq/mod.rs:448-457): a - t when a >= t >> 1, else a, as a select
 __global__ void center_kernel(u64* x, size_t n_words, u64 t) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1372,11 +1384,194 @@ __global__ void ksk_gen_kernel(KskGenArgs A) {
   reinterpret_cast<ulonglong2*>(A.k1 + off + c)[1] = make_ulonglong2(a[2], a[3]);
 }
 
+// ------------------------------------------------------------------ multiparty BFV (fhe::mbfv)
+struct CrpArgs {
+  u64* out;           // [cts][L][N]
+  EncSeed K;
+  u32 cts, ct_base, logn, limbs_per_poly;
+  const LimbDev* limbs;
+  unsigned short ids[kMaxPos];
+};
+// CommonRandomPoly::new_leveled (crp.rs:35-43): (hi 2^64 + lo) mod q_j of the role-7 row (crp, limb j), drawn directly
+// as NTT words.  One thread per (crp, limb, 4 coefficients).
+__global__ void crp_kernel(CrpArgs A) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const u32 g_per_row = 1u << (A.logn - 2);
+  const size_t total = (size_t)A.cts * A.limbs_per_poly * g_per_row;
+  if (idx >= total) return;
+  const u32 g = (u32)(idx % g_per_row);
+  const size_t row = idx / g_per_row;
+  const u32 j = (u32)(row % A.limbs_per_poly), ct = (u32)(row / A.limbs_per_poly);
+  const LimbDev& M = A.limbs[A.ids[j]];
+  u64 lo[4], hi[4];
+  chacha_block(A.K, g, A.ct_base + ct, (7u << 8) | j, 0, lo, hi);
+  u64 a[4];
+#pragma unroll
+  for (int m = 0; m < 4; m++) a[m] = reduce128_limb(lo[m], hi[m], M);
+  u64* dst = A.out + (row << A.logn) + (size_t)g * 4;
+  reinterpret_cast<ulonglong2*>(dst)[0] = make_ulonglong2(a[0], a[1]);
+  reinterpret_cast<ulonglong2*>(dst)[1] = make_ulonglong2(a[2], a[3]);
+}
+
+struct MbfvShareArgs {
+  const u64* s;       // row j: s modulo the j-th limb (NTT)
+  const u64* s_out;   // SHARE_SKS: the output key's rows, or null for DecryptionShare's zero key
+  const u64* x;       // SHARE_PK: crp [cts][L][N]; SHARE_SKS / SHARE_PKS: the ciphertexts [cts][2][L][N];
+                      // SHARE_RKG1: crp a_i [cts][L][N]; SHARE_RKG2: round-1 aggregate h0_i [cts][L][N]
+  const u64* pk;      // SHARE_PKS: the public key at the level, [2][L][N]; SHARE_RKG2: round-1 aggregate h1_i
+  const u64* u;       // SHARE_RKG1 / SHARE_RKG2: the generator's u, rows as s
+  const u64* e;       // SHARE_PK / SHARE_SKS: [cts][L][N]; SHARE_PKS: [cts][3][L][N] = (u, e0, e1);
+                      // SHARE_RKG1 / SHARE_RKG2: [cts][2][L][N] = (e0, e1), all NTT
+  u64* out;           // SHARE_PK / SHARE_SKS: [cts][L][N]; SHARE_PKS: [cts][2][L][N]; SHARE_RKG*: h0 [cts][L][N]
+  u64* out1;          // SHARE_RKG1 / SHARE_RKG2: h1 [cts][L][N]
+  u32 cts, ct_base, logn, limbs_per_poly;
+  const LimbDev* limbs;
+  unsigned short ids[kMaxPos];
+};
+// The share of one protocol in one pass, one coefficient per thread, every term a canonical residue:
+//  SHARE_PK  (public_key_gen.rs:32-58):    p0 = -crp s + e
+//  SHARE_SKS (secret_key_switch.rs:38-96): h = (s_in - s_out) c1 + e
+//  SHARE_PKS (public_key_switch.rs:33-93): (h0, h1) = (u pk0 + s c1 + e0, u pk1 + e1)
+//  SHARE_RKG1 (relin_key_gen.rs:112-198), item i = ct_base + ct: (h0_i, h1_i) = (-a_i u + w_i s + e0, a_i s + e1), w_i
+//    the Garner coefficient of the level-0 basis: w_i s is s on limb i and 0 on the others (a select on the indices)
+//  SHARE_RKG2 (relin_key_gen.rs:224-297): (h0'_i, h1'_i) = (h0_i s + e0, h1_i (u - s) + e1)
+// No branch depends on the data (s_out == null is a property of the call).
+template <int P>
+__global__ void mbfv_share_kernel(MbfvShareArgs A) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t stride = (size_t)A.limbs_per_poly << A.logn;
+  if (idx >= (size_t)A.cts * stride) return;
+  const size_t ct = idx / stride, in_ct = idx % stride;
+  const u32 j = (u32)(in_ct >> A.logn);
+  const LimbDev& M = A.limbs[A.ids[j]];
+  const u64 s = A.s[in_ct];
+  if (P == SHARE_PK) {
+    A.out[idx] = csub(A.e[idx] + M.p - mulmod_limb(A.x[idx], s, M), M.p);
+  } else if (P == SHARE_SKS) {
+    const u64 so = A.s_out ? A.s_out[in_ct] : 0;
+    const u64 c1 = A.x[(2 * ct + 1) * stride + in_ct];
+    A.out[idx] = csub(mulmod_limb(csub(s + M.p - so, M.p), c1, M) + A.e[idx], M.p);
+  } else if (P == SHARE_RKG1) {
+    const u64 a = A.x[idx], u = A.u[in_ct];
+    const u64 ws = (j == A.ct_base + (u32)ct) ? s : 0;
+    const u64* ee = A.e + ct * 2 * stride + in_ct;
+    A.out[idx] = csub(csub(ee[0] + M.p - mulmod_limb(a, u, M), M.p) + ws, M.p);
+    A.out1[idx] = csub(mulmod_limb(a, s, M) + ee[stride], M.p);
+  } else if (P == SHARE_RKG2) {
+    const u64 u = A.u[in_ct];
+    const u64* ee = A.e + ct * 2 * stride + in_ct;
+    A.out[idx] = csub(mulmod_limb(A.x[idx], s, M) + ee[0], M.p);
+    A.out1[idx] = csub(mulmod_limb(A.pk[idx], csub(u + M.p - s, M.p), M) + ee[stride], M.p);
+  } else {
+    const u64* uee = A.e + ct * 3 * stride + in_ct;
+    const u64 u = uee[0], e0 = uee[stride], e1 = uee[2 * stride];
+    const u64 c1 = A.x[(2 * ct + 1) * stride + in_ct];
+    u64* dst = A.out + ct * 2 * stride + in_ct;
+    dst[0] = csub(csub(mulmod_limb(u, A.pk[in_ct], M) + mulmod_limb(s, c1, M), M.p) + e0, M.p);
+    dst[stride] = csub(mulmod_limb(u, A.pk[stride + in_ct], M) + e1, M.p);
+  }
+}
+
+struct SumArgs {
+  const u64* src[kSumGroup];   // item k of source i at src[i] + k * src_stride
+  const u64* base;             // nullable, item k at base + k * base_stride
+  u64* out;                    // item k at out + k * out_stride
+  size_t src_stride, base_stride, out_stride, item_words;
+  size_t base_row, out_row;    // row r of a base / out item at + r * base_row / out_row (N: contiguous rows)
+  u32 n_src, items, logn, limbs_per_poly;
+  const LimbDev* limbs;
+  unsigned short ids[kMaxPos];
+};
+// out = base + sum_i src_i, two words per thread.  The words are canonical (< 2^62): the sum is accumulated in 128 bits
+// with a carry count and reduced once per word, so every source word is read once and the reduction count does not grow
+// with the number of sources.
+__global__ void shares_sum_kernel(SumArgs A) {
+  const size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 2;
+  if (i >= (size_t)A.items * A.item_words) return;
+  const size_t item = i / A.item_words, w = i % A.item_words;
+  const size_t r = w >> A.logn, c = w & ((1u << A.logn) - 1);
+  const LimbDev& M = A.limbs[A.ids[(u32)r % A.limbs_per_poly]];
+  u64 lo0 = 0, lo1 = 0, hi0 = 0, hi1 = 0;
+  if (A.base) {
+    const ulonglong2 b = *reinterpret_cast<const ulonglong2*>(A.base + item * A.base_stride + r * A.base_row + c);
+    lo0 = b.x;
+    lo1 = b.y;
+  }
+  const size_t off = item * A.src_stride + w;
+  for (u32 k = 0; k < A.n_src; k++) {
+    const ulonglong2 v = *reinterpret_cast<const ulonglong2*>(A.src[k] + off);
+    lo0 += v.x;
+    hi0 += lo0 < v.x;
+    lo1 += v.y;
+    hi1 += lo1 < v.y;
+  }
+  *reinterpret_cast<ulonglong2*>(A.out + item * A.out_stride + r * A.out_row + c) =
+      make_ulonglong2(reduce128_limb(lo0, hi0, M), reduce128_limb(lo1, hi1, M));
+}
+
 void copy_ids(unsigned short* dst, const RowIds& ids) {
   for (int i = 0; i < kMaxPos; i++) dst[i] = ids.ids[i];
 }
 
 }  // namespace
+
+void launch_crp(u64* out, u32 cts, u32 ct_base, const EncSeed& K, const RowIds& ids, const LimbDev* limbs, u32 logn,
+                cudaStream_t st) {
+  CrpArgs A;
+  A.out = out; A.K = K; A.cts = cts; A.ct_base = ct_base; A.logn = logn; A.limbs_per_poly = ids.limbs_per_poly;
+  A.limbs = limbs;
+  copy_ids(A.ids, ids);
+  const size_t total = ((size_t)cts * ids.limbs_per_poly) << (logn - 2);
+  if (!total) return;
+  crp_kernel<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(A);
+  g_launches++;
+}
+
+void launch_mbfv_share(MbfvShare kind, const u64* s, const u64* s_out, const u64* x, const u64* pk, const u64* e,
+                       u64* out, u32 cts, const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st,
+                       const u64* u, u64* out1, u32 ct_base) {
+  MbfvShareArgs A;
+  A.s = s; A.s_out = s_out; A.x = x; A.pk = pk; A.u = u; A.e = e; A.out = out; A.out1 = out1; A.cts = cts;
+  A.ct_base = ct_base; A.logn = logn;
+  A.limbs_per_poly = ids.limbs_per_poly; A.limbs = limbs;
+  copy_ids(A.ids, ids);
+  const size_t total = ((size_t)cts * ids.limbs_per_poly) << logn;
+  if (!total) return;
+  const unsigned blocks = (unsigned)((total + 255) / 256);
+  if (kind == SHARE_PK) mbfv_share_kernel<SHARE_PK><<<blocks, 256, 0, st>>>(A);
+  else if (kind == SHARE_SKS) mbfv_share_kernel<SHARE_SKS><<<blocks, 256, 0, st>>>(A);
+  else if (kind == SHARE_PKS) mbfv_share_kernel<SHARE_PKS><<<blocks, 256, 0, st>>>(A);
+  else if (kind == SHARE_RKG1) mbfv_share_kernel<SHARE_RKG1><<<blocks, 256, 0, st>>>(A);
+  else mbfv_share_kernel<SHARE_RKG2><<<blocks, 256, 0, st>>>(A);
+  g_launches++;
+}
+
+void launch_shares_sum(const u64* const* src, u32 n_src, size_t src_stride, const u64* base, size_t base_stride,
+                       u64* out, size_t out_stride, u32 items, size_t item_words, const RowIds& ids,
+                       const LimbDev* limbs, u32 logn, cudaStream_t st, size_t out_row) {
+  const size_t total = (size_t)items * item_words;
+  if (!total || !n_src) return;
+  const size_t N = (size_t)1 << logn;
+  SumArgs A;
+  A.out = out; A.src_stride = src_stride; A.out_stride = out_stride; A.item_words = item_words; A.items = items;
+  A.out_row = out_row ? out_row : N;
+  A.logn = logn; A.limbs_per_poly = ids.limbs_per_poly; A.limbs = limbs;
+  copy_ids(A.ids, ids);
+  // one launch per group of kSumGroup sources; every group after the first adds to what the previous one wrote.  A
+  // source that is also the output goes into the first group, which reads it before anything is written.
+  std::vector<const u64*> order(src, src + n_src);
+  for (u32 k = 0; k < n_src; k++)
+    if (order[k] == out) std::swap(order[k], order[0]);
+  for (u32 g0 = 0; g0 < n_src; g0 += kSumGroup) {
+    A.n_src = std::min(kSumGroup, n_src - g0);
+    for (u32 k = 0; k < A.n_src; k++) A.src[k] = order[g0 + k];
+    A.base = g0 ? out : base;
+    A.base_stride = g0 ? out_stride : base_stride;
+    A.base_row = g0 ? A.out_row : N;
+    shares_sum_kernel<<<(unsigned)((total / 2 + 255) / 256), 256, 0, st>>>(A);
+    g_launches++;
+  }
+}
 
 void launch_encode_load(const u64* staged, u64* coeffs, u32 n_pt, size_t n_values, const u32* inv_map, bool is_signed,
                         const PlainMod& T, u32 logn, cudaStream_t st) {
@@ -1422,6 +1617,12 @@ void launch_phase(const u64* ct, const u64* s, u64* out, u32 cts, u32 parts, con
 void launch_decrypt_epilogue(u64* v, size_t n_words, const PlainMod& Q0, const PlainMod& T, cudaStream_t st) {
   if (!n_words) return;
   decrypt_epilogue_kernel<<<(unsigned)((n_words + 255) / 256), 256, 0, st>>>(v, n_words, Q0, T);
+  g_launches++;
+}
+
+void launch_from_shares_epilogue(u64* v, size_t n_words, u64 q0, const PlainMod& T, cudaStream_t st) {
+  if (!n_words) return;
+  from_shares_epilogue_kernel<<<(unsigned)((n_words + 255) / 256), 256, 0, st>>>(v, n_words, q0, T);
   g_launches++;
 }
 

@@ -72,6 +72,7 @@ typedef struct fhe_b200_multiplicator fhe_b200_multiplicator; /* == Multiplicato
 typedef struct fhe_b200_encoder fhe_b200_encoder; /* == the plaintext side of BfvParameters: the NTT operator of t
                                                      and the SIMD slot map (parameters.rs:71-75, :713-726)      */
 typedef struct fhe_b200_secret_key fhe_b200_secret_key; /* == SecretKey (bfv/keys/secret_key.rs:25-53)               */
+typedef struct fhe_b200_rkg fhe_b200_rkg;             /* == mbfv::RelinKeyGenerator (mbfv/relin_key_gen.rs:36-96)  */
 
 /* Encoding (bfv/encoding.rs): the level comes from the output batch (Encoding::{poly,simd}_at_level). */
 typedef enum { FHE_B200_ENCODING_POLY = 0, FHE_B200_ENCODING_SIMD = 1 } fhe_b200_encoding;
@@ -253,8 +254,9 @@ int fhe_b200_measure_noise(const fhe_b200_secret_key* sk, const fhe_b200_batch* 
  *     word 12      b, the block index within the row
  *     word 13      the index of the ciphertext within the call (0 .. out.count - 1)
  *     word 14      role << 8 | limb: role 0 = a, 1 = e (secret-key encryption), 2 = u, 3 = e1, 4 = e2 (public-key
- *                  encryption), 5 = c1, 6 = e (key generation, below); the small polynomials use limb 0
- *     word 15      0 (encryption), the digit of the key (key generation)
+ *                  encryption), 5 = c1, 6 = e (key generation, below), 7, 8, 14 - 17 (multiparty BFV, below); the
+ *                  small polynomials use limb 0
+ *     word 15      0 (encryption, multiparty BFV), the digit of the key (key generation)
  * Each block is addressed only by its position, so the words do not depend on chunking or streams.  One 64-byte block
  * gives four 128-bit values: value m is u64 words 2m (low) and 2m + 1 (high) of the block, and coefficient 4b + m of
  * the row takes value m of block b.
@@ -315,6 +317,91 @@ int fhe_b200_galois_keys_generate(const fhe_b200_secret_key* sk, const uint32_t*
  * INVALID_ARGUMENT, power basis -> INVALID_REPRESENTATION. */
 int fhe_b200_rgsw_encrypt(const fhe_b200_secret_key* sk, const fhe_b200_batch* pts, uint32_t variance,
                           const uint8_t* seed, fhe_b200_ksk** out, void* stream);
+
+/* ---- multiparty BFV (fhe::mbfv, crates/fhe/src/mbfv) ----------------------------------------------
+ * WARNING: experimental, incomplete and not audited, as the reference's module.  As there, the errors of every share
+ * are the ordinary BfvParameters::variance errors, not smudging noise (the reference's own TODO): a decryption share
+ * may leak information about the secret key share.  No noise flooding is added here.
+ * A share is an ordinary batch; every call takes whole batches (one share per ciphertext or per CRP) and is only
+ * enqueued.  The random words come from the stream above with word 15 = 0 and word 13 = the index within the call
+ * (the CRP, or the ciphertext of `ct`):
+ *  - role 7: the CRP, (hi 2^64 + lo) mod q_j of limb j's row, drawn directly as NTT words (Poly::<Ntt>::random);
+ *  - role 8: e of PublicKeyShare;  role 14: e of SecretKeySwitchShare / DecryptionShare;  roles 15, 16, 17: u, e0, e1
+ *    of PublicKeySwitchShare;  role 9: u of RelinKeyGenerator::new;  roles 10, 11: the errors of round 1's h0_i, h1_i and
+ *    roles 12, 13 those of round 2's h0'_i, h1'_i, with word 13 = 0 and word 15 = i; all centred binomial samples of
+ *    limb 0's row lifted to every limb.
+ * Scratch holding errors, u, s-dependent values or the aggregated phase is zeroed before it goes back to the pool; the
+ * kernels have no branch that depends on the data.  Aggregation reads every share word once and reduces each output word
+ * once.  Errors: variance outside 1..32 (InvalidVariance), a NULL argument, n == 0 (MultipartyError::NoShares), shares
+ * whose shape (count, parts, level) differs from the one the call needs, an output of the wrong shape ->
+ * INVALID_ARGUMENT; operands of different parameter sets or over the multiplication basis (ParameterMismatch) ->
+ * CONTEXT_MISMATCH; ct not 2-part (InvalidPolynomialCount) -> BAD_POLY_COUNT; a crp or public key not at level 0 ->
+ * INVALID_LEVEL; power-basis operands -> INVALID_REPRESENTATION.  A refused call allocates nothing. */
+/* CommonRandomPoly::new / new_vec / new_leveled (crp.rs:15-43): every entry of `out` (a 1-part batch) becomes one CRP
+ * at out's level; new_vec is a batch of n_moduli entries at level 0. */
+int fhe_b200_crp_generate(const fhe_b200_params* p, const uint8_t* seed, fhe_b200_batch* out, void* stream);
+/* PublicKeyShare::new (public_key_gen.rs:32-58): out entry k = p0 = -crp_k s + e_k at level 0.  crp: a 1-part level-0
+ * batch; out: a 1-part level-0 batch of crp.count entries. */
+int fhe_b200_pk_share(const fhe_b200_secret_key* sk, const fhe_b200_batch* crp, uint32_t variance, const uint8_t* seed,
+                      fhe_b200_batch* out, void* stream);
+/* PublicKey::from_shares (public_key_gen.rs:60-77): pk entry k = (sum_i shares[i]_k, crp_k), a 2-part level-0 batch of
+ * crp.count entries; an entry is a public key fhe_b200_encrypt_pk takes as it is. */
+int fhe_b200_pk_aggregate(const fhe_b200_batch* const* shares, uint32_t n, const fhe_b200_batch* crp,
+                          fhe_b200_batch* pk, void* stream);
+/* out = sum of the n shares, word by word, for shares of out's shape (the sum inside every aggregation, and
+ * RelinKeyShare<R1Aggregated>::from_shares, relin_key_gen.rs:200-222, for h0 and h1 each).  out may be any of the
+ * shares.  Shares are summed in launches of 64: each output word is reduced once per launch. */
+int fhe_b200_shares_sum(const fhe_b200_batch* const* shares, uint32_t n, fhe_b200_batch* out, void* stream);
+/* SecretKeySwitchShare::new (secret_key_switch.rs:38-96) of every ciphertext of ct (2-part): out entry k =
+ * h = (s_in - s_out) c1_k + e_k at ct's level, a 1-part batch of ct.count entries.  sk_out NULL is the zero key of
+ * DecryptionShare::new (:133-143). */
+int fhe_b200_sks_share(const fhe_b200_secret_key* sk_in, const fhe_b200_secret_key* sk_out, const fhe_b200_batch* ct,
+                       uint32_t variance, const uint8_t* seed, fhe_b200_batch* out, void* stream);
+/* Ciphertext::from_shares of SecretKeySwitchShares (secret_key_switch.rs:98-115): out = (c0 + sum h_i, c1), a 2-part
+ * batch of ct's shape (out may be ct). */
+int fhe_b200_sks_aggregate(const fhe_b200_batch* ct, const fhe_b200_batch* const* shares, uint32_t n,
+                           fhe_b200_batch* out, void* stream);
+/* PublicKeySwitchShare::new (public_key_switch.rs:33-93) of every ciphertext of ct: out entry k = (u pk0 + s c1_k + e0,
+ * u pk1 + e1), pk (a level-0 public key, as for fhe_b200_encrypt_pk) switched down to ct's level; out has ct's shape. */
+int fhe_b200_pks_share(const fhe_b200_secret_key* sk, const fhe_b200_batch* pk, const fhe_b200_batch* ct,
+                       uint32_t variance, const uint8_t* seed, fhe_b200_batch* out, void* stream);
+/* Ciphertext::from_shares of PublicKeySwitchShares (public_key_switch.rs:95-112): out = (c0 + sum h0_i, sum h1_i). */
+int fhe_b200_pks_aggregate(const fhe_b200_batch* ct, const fhe_b200_batch* const* shares, uint32_t n,
+                           fhe_b200_batch* out, void* stream);
+/* RelinKeyGenerator::new (relin_key_gen.rs:76-96): u (role 9) is drawn and kept on the device in *out; the generator
+ * also refers to sk and to crp, a 1-part level-0 batch of the n_moduli CRPs of CommonRandomPoly::new_vec, which must
+ * outlive it (the reference borrows both).  fhe_b200_rkg_free waits for the device, erases u and releases it.
+ * Errors: a single modulus -> UNSUPPORTED (KeySwitchingNotSupported); crp.count != n_moduli ->
+ * INVALID_ARGUMENT (InvalidCommonRandomPolynomialCount); crp not at level 0 -> INVALID_LEVEL. */
+int fhe_b200_rkg_create(const fhe_b200_secret_key* sk, const fhe_b200_batch* crp, uint32_t variance,
+                        const uint8_t* seed, fhe_b200_rkg** out, void* stream);
+int fhe_b200_rkg_free(fhe_b200_rkg* r);
+/* RelinKeyGenerator::round_1 (relin_key_gen.rs:112-198): entry i of h0 / h1 (1-part level-0 batches of n_moduli
+ * entries) = -a_i u + w_i s + e, a_i s + e; w_i is the Garner coefficient of the level-0 basis (s on limb i, 0 on the
+ * others).  Aggregate the parties' h0 and h1 with fhe_b200_shares_sum (RelinKeyShare<R1Aggregated>). */
+int fhe_b200_rkg_round1(const fhe_b200_rkg* r, const uint8_t* seed, fhe_b200_batch* h0, fhe_b200_batch* h1,
+                        void* stream);
+/* RelinKeyGenerator::round_2 (relin_key_gen.rs:224-297) from the round-1 aggregate (r1_h0, r1_h1): entry i of h0 / h1
+ * = r1_h0_i s + e, r1_h1_i (u - s) + e. */
+int fhe_b200_rkg_round2(const fhe_b200_rkg* r, const fhe_b200_batch* r1_h0, const fhe_b200_batch* r1_h1,
+                        const uint8_t* seed, fhe_b200_batch* h0, fhe_b200_batch* h1, void* stream);
+/* RelinearizationKey::from_shares (relin_key_gen.rs:299-350) of the n parties' round-2 shares (h0s[k], h1s[k]) and the
+ * round-1 aggregate's r1_h1: *out = a new level-0 RNS-digit key with c0_i = sum h0'_i + sum h1'_i, c1_i = r1_h1_i,
+ * written straight into the key's device layout.  It is an ordinary key for fhe_b200_relinearize, fhe_b200_mul_relin
+ * and the multiplicator, released with fhe_b200_ksk_free. */
+int fhe_b200_rkg_aggregate(const fhe_b200_batch* const* h0s, const fhe_b200_batch* const* h1s, uint32_t n,
+                           const fhe_b200_batch* r1_h1, fhe_b200_ksk** out, void* stream);
+/* Plaintext::from_shares of DecryptionShares (secret_key_switch.rs:145-186): c = c0 + sum h_i to the power basis, scaled
+ * by t / Q (cipher_plain_context.scaler), w = ((v + t) mod Q_p) mod t with Q_p the product of the plaintext-context
+ * moduli (the first moduli whose sizes add up to bits(t) + 60, parameters.rs:579-595), lifted and transformed into
+ * pts_out (a 1-part batch of ct.count entries at ct's level, encoding None).  The scaled value v is the rounding of
+ * t x / Q for the centred lift x of the phase, |v| <= t / 2, and from_shares gives v mod t.  fhe_b200_decrypt lifts
+ * ((v + t) mod q_0) mod t instead; the two differ when the plaintext context has two or more moduli, q_0 / 2 < t < q_0
+ * and v >= q_0 - t.  The aggregator holds no secret key: the scaler tables of each level live on the encoder `e`, built
+ * on first use.  t >= q_0 or t beyond a u64 Modulus -> UNSUPPORTED. */
+int fhe_b200_decryption_aggregate(const fhe_b200_encoder* e, const fhe_b200_batch* ct,
+                                  const fhe_b200_batch* const* shares, uint32_t n, fhe_b200_batch* pts_out,
+                                  void* stream);
 
 /* &Ciphertext * &Ciphertext (bfv/ops/mod.rs:259-358): n parts x m parts -> n + m - 1 parts (out3 must have that many;
  * 2 x 2 -> 3 is the fused path) */

@@ -41,6 +41,10 @@ inline void check(int code) {
   if (code != FHE_B200_OK) throw Error(code, fhe_b200_last_error());
 }
 
+namespace mbfv {
+class PlaintextAccess;
+}
+
 namespace bfv {
 
 enum class Representation : int { PowerBasis = FHE_B200_POWER_BASIS, Ntt = FHE_B200_NTT };
@@ -333,6 +337,7 @@ class PlaintextVec {
 
  protected:
   friend class SecretKey;
+  friend class mbfv::PlaintextAccess;   // Plaintext::from_shares builds plaintexts without an encoding
   PlaintextVec(Ciphertext b, const Encoding& e) : batch_(std::move(b)), encoding_(e) {}
   explicit PlaintextVec(Ciphertext b) : batch_(std::move(b)), encoding_(Encoding::poly()), has_encoding_(false) {}
   static PlaintextVec encode(const void* values, size_t n, bool is_signed, const Encoding& e,
@@ -838,4 +843,218 @@ class Multiplicator {
 };
 
 }  // namespace bfv
+
+// fhe::mbfv (multiparty BFV, crates/fhe/src/mbfv).  WARNING: experimental, incomplete and not audited, as the
+// reference's module: the share errors are the ordinary variance errors, not smudging noise, and none is added.  Every
+// share holds device batches and covers a whole batch of ciphertexts; seeds as for SecretKey::try_encrypt.
+namespace mbfv {
+using bfv::BfvParameters;
+using bfv::Ciphertext;
+using bfv::EncryptionSeed;
+using bfv::KeySwitchingKey;
+using bfv::PlaintextVec;
+using bfv::PublicKey;
+using bfv::RelinearizationKey;
+using bfv::Representation;
+using bfv::SecretKey;
+
+inline std::vector<fhe_b200_batch*> handles(const std::vector<const Ciphertext*>& b) {
+  std::vector<fhe_b200_batch*> h;
+  for (const Ciphertext* c : b) h.push_back(c->handle());
+  return h;
+}
+inline const fhe_b200_batch* const* table(const std::vector<fhe_b200_batch*>& h) {
+  return reinterpret_cast<const fhe_b200_batch* const*>(h.data());
+}
+
+// CommonRandomPoly (crp.rs:8-44): a 1-part batch, one CRP per entry
+struct CommonRandomPoly {
+  std::shared_ptr<Ciphertext> batch;
+  static CommonRandomPoly new_leveled(const std::shared_ptr<BfvParameters>& par, uint32_t level,
+                                      const uint8_t* seed = nullptr) {
+    return {generate(par, 1, level, seed)};
+  }
+  static CommonRandomPoly new_key(const std::shared_ptr<BfvParameters>& par, const uint8_t* seed = nullptr) {
+    return new_leveled(par, 0, seed);
+  }
+  // one CRP per modulus, drawn in one call (entry k of the call is CRP k)
+  static std::vector<CommonRandomPoly> new_vec(const std::shared_ptr<BfvParameters>& par, const uint8_t* seed = nullptr) {
+    const auto b = generate(par, (uint32_t)par->moduli().size(), 0, seed);
+    std::vector<CommonRandomPoly> v;
+    for (uint32_t k = 0; k < b->count(); k++) v.push_back({std::make_shared<Ciphertext>(b->take(k, 1))});
+    return v;
+  }
+  static std::shared_ptr<Ciphertext> generate(const std::shared_ptr<BfvParameters>& par, uint32_t count, uint32_t level,
+                                              const uint8_t* seed) {
+    const EncryptionSeed s(seed);
+    auto b = std::make_shared<Ciphertext>(par, count, 1, level);
+    check(fhe_b200_crp_generate(par->handle(), s.bytes, b->handle(), b->stream()));
+    return b;
+  }
+};
+
+// PublicKeyShare (public_key_gen.rs:11-58): p0 = -crp s + e
+struct PublicKeyShare {
+  CommonRandomPoly crp;
+  Ciphertext p0_share;
+  PublicKeyShare(const SecretKey& sk, CommonRandomPoly c, const uint8_t* seed = nullptr)
+      : crp(std::move(c)), p0_share(sk.par(), crp.batch->count(), 1, 0) {
+    const EncryptionSeed s(seed);
+    check(fhe_b200_pk_share(sk.handle(), crp.batch->handle(), sk.par()->variance(), s.bytes, p0_share.handle(),
+                            p0_share.stream()));
+  }
+};
+
+// SecretKeySwitchShare (secret_key_switch.rs:14-96): h = (s_in - s_out) c1 + e for every ciphertext of ct; a null
+// output key is DecryptionShare's zero key (:117-143)
+struct SecretKeySwitchShare {
+  const Ciphertext* ct;
+  Ciphertext h_share;
+  SecretKeySwitchShare(const SecretKey& sk_in, const SecretKey* sk_out, const Ciphertext& c, const uint8_t* seed = nullptr)
+      : ct(&c), h_share(sk_in.par(), c.count(), 1, c.level(), Representation::Ntt, c.stream()) {
+    const EncryptionSeed s(seed);
+    check(fhe_b200_sks_share(sk_in.handle(), sk_out ? sk_out->handle() : nullptr, c.handle(), sk_in.par()->variance(),
+                             s.bytes, h_share.handle(), c.stream()));
+  }
+};
+struct DecryptionShare : SecretKeySwitchShare {
+  DecryptionShare(const SecretKey& sk, const Ciphertext& c, const uint8_t* seed = nullptr)
+      : SecretKeySwitchShare(sk, nullptr, c, seed) {}
+};
+
+// PublicKeySwitchShare (public_key_switch.rs:13-93): (u pk0 + s c1 + e0, u pk1 + e1), a 2-part batch
+struct PublicKeySwitchShare {
+  const Ciphertext* ct;
+  Ciphertext h_share;
+  PublicKeySwitchShare(const SecretKey& sk, const PublicKey& pk, const Ciphertext& c, const uint8_t* seed = nullptr)
+      : ct(&c), h_share(sk.par(), c.count(), 2, c.level(), Representation::Ntt, c.stream()) {
+    const EncryptionSeed s(seed);
+    check(fhe_b200_pks_share(sk.handle(), pk.c().handle(), c.handle(), sk.par()->variance(), s.bytes, h_share.handle(),
+                             c.stream()));
+  }
+};
+
+// RelinKeyShare<R> (relin_key_gen.rs:14-34): h0, h1, one polynomial per level-0 modulus each; a round-2 share keeps
+// the round-1 aggregate it was made from
+enum class Round { R1, R1Aggregated, R2 };
+struct RelinKeyShare {
+  Round round;
+  std::shared_ptr<Ciphertext> h0, h1;
+  std::shared_ptr<const RelinKeyShare> last_round;
+};
+
+// RelinKeyGenerator (relin_key_gen.rs:36-110): u lives on the device and is erased when the generator is destroyed
+class RelinKeyGenerator {
+ public:
+  RelinKeyGenerator(const SecretKey& sk, const std::vector<CommonRandomPoly>& crp, const uint8_t* seed = nullptr)
+      : par_(sk.par()), crp_(par_, (uint32_t)par_->moduli().size(), 1, 0) {
+    if (crp.size() != par_->moduli().size())
+      throw Error(FHE_B200_INVALID_ARGUMENT, "MultipartyError::InvalidCommonRandomPolynomialCount");
+    for (uint32_t i = 0; i < crp.size(); i++)
+      check(fhe_b200_batch_copy_range(crp_.handle(), i, crp[i].batch->handle(), 0, 1, 1, crp_.stream()));
+    const EncryptionSeed s(seed);
+    check(fhe_b200_rkg_create(sk.handle(), crp_.handle(), par_->variance(), s.bytes, &h_, crp_.stream()));
+  }
+  RelinKeyGenerator(const RelinKeyGenerator&) = delete;
+  RelinKeyGenerator& operator=(const RelinKeyGenerator&) = delete;
+  ~RelinKeyGenerator() { fhe_b200_rkg_free(h_); }
+  RelinKeyShare round_1(const uint8_t* seed = nullptr) const {
+    const EncryptionSeed s(seed);
+    RelinKeyShare r = pair(Round::R1);
+    check(fhe_b200_rkg_round1(h_, s.bytes, r.h0->handle(), r.h1->handle(), r.h0->stream()));
+    return r;
+  }
+  RelinKeyShare round_2(const std::shared_ptr<const RelinKeyShare>& r1, const uint8_t* seed = nullptr) const {
+    if (r1->round != Round::R1Aggregated) throw Error(FHE_B200_INVALID_ARGUMENT, "round 2 takes the round-1 aggregate");
+    const EncryptionSeed s(seed);
+    RelinKeyShare r = pair(Round::R2);
+    r.last_round = r1;
+    check(fhe_b200_rkg_round2(h_, r1->h0->handle(), r1->h1->handle(), s.bytes, r.h0->handle(), r.h1->handle(),
+                              r.h0->stream()));
+    return r;
+  }
+
+ private:
+  RelinKeyShare pair(Round round) const {
+    const uint32_t L = (uint32_t)par_->moduli().size();
+    return {round, std::make_shared<Ciphertext>(par_, L, 1, 0), std::make_shared<Ciphertext>(par_, L, 1, 0), nullptr};
+  }
+  std::shared_ptr<BfvParameters> par_;
+  Ciphertext crp_;   // the CRPs side by side, as long as the generator
+  fhe_b200_rkg* h_ = nullptr;
+};
+
+// Aggregate::from_shares (aggregate.rs and the impls beside each share); the first share supplies the CRP / ciphertext
+inline PublicKey public_key_from_shares(const std::vector<PublicKeyShare>& shares) {
+  if (shares.empty()) throw Error(FHE_B200_INVALID_ARGUMENT, "MultipartyError::NoShares");
+  std::vector<const Ciphertext*> b;
+  for (const auto& s : shares) b.push_back(&s.p0_share);
+  const auto h = handles(b);
+  const Ciphertext& crp = *shares[0].crp.batch;
+  Ciphertext pk(crp.par(), crp.count(), 2, 0, Representation::Ntt, crp.stream());
+  check(fhe_b200_pk_aggregate(table(h), (uint32_t)h.size(), crp.handle(), pk.handle(), pk.stream()));
+  return PublicKey(crp.par(), std::move(pk));
+}
+template <class Share>
+inline Ciphertext ciphertext_from_shares(const std::vector<Share>& shares) {
+  if (shares.empty()) throw Error(FHE_B200_INVALID_ARGUMENT, "MultipartyError::NoShares");
+  std::vector<const Ciphertext*> b;
+  for (const auto& s : shares) b.push_back(&s.h_share);
+  const auto h = handles(b);
+  const Ciphertext& ct = *shares[0].ct;
+  Ciphertext out(ct.par(), ct.count(), 2, ct.level(), Representation::Ntt, ct.stream());
+  const bool sks = std::is_base_of<SecretKeySwitchShare, Share>::value;
+  check((sks ? fhe_b200_sks_aggregate : fhe_b200_pks_aggregate)(ct.handle(), table(h), (uint32_t)h.size(), out.handle(),
+                                                                out.stream()));
+  return out;
+}
+class PlaintextAccess {
+ public:
+  static PlaintextVec without_encoding(Ciphertext b) { return PlaintextVec(std::move(b)); }
+};
+// Plaintext::from_shares: one plaintext per ciphertext, no encoding
+inline PlaintextVec plaintext_from_shares(const std::vector<DecryptionShare>& shares) {
+  if (shares.empty()) throw Error(FHE_B200_INVALID_ARGUMENT, "MultipartyError::NoShares");
+  std::vector<const Ciphertext*> b;
+  for (const auto& s : shares) b.push_back(&s.h_share);
+  const auto h = handles(b);
+  const Ciphertext& ct = *shares[0].ct;
+  Ciphertext out(ct.par(), ct.count(), 1, ct.level(), Representation::Ntt, ct.stream());
+  check(fhe_b200_decryption_aggregate(ct.par()->encoder(), ct.handle(), table(h), (uint32_t)h.size(), out.handle(),
+                                      out.stream()));
+  return PlaintextAccess::without_encoding(std::move(out));
+}
+// RelinKeyShare<R1Aggregated>::from_shares (round-1 shares) or RelinearizationKey::from_shares (round-2 shares)
+inline RelinKeyShare r1_from_shares(const std::vector<RelinKeyShare>& shares) {
+  if (shares.empty()) throw Error(FHE_B200_INVALID_ARGUMENT, "MultipartyError::NoShares");
+  std::vector<const Ciphertext*> b0, b1;
+  for (const auto& s : shares) {
+    if (s.round != Round::R1) throw Error(FHE_B200_INVALID_ARGUMENT, "round-1 shares expected");
+    b0.push_back(s.h0.get());
+    b1.push_back(s.h1.get());
+  }
+  const Ciphertext& f = *shares[0].h0;
+  RelinKeyShare r{Round::R1Aggregated, std::make_shared<Ciphertext>(f.par(), f.count(), 1, 0),
+                  std::make_shared<Ciphertext>(f.par(), f.count(), 1, 0), nullptr};
+  const auto h0 = handles(b0), h1 = handles(b1);
+  check(fhe_b200_shares_sum(table(h0), (uint32_t)h0.size(), r.h0->handle(), r.h0->stream()));
+  check(fhe_b200_shares_sum(table(h1), (uint32_t)h1.size(), r.h1->handle(), r.h1->stream()));
+  return r;
+}
+inline RelinearizationKey relin_key_from_shares(const std::vector<RelinKeyShare>& shares) {
+  if (shares.empty()) throw Error(FHE_B200_INVALID_ARGUMENT, "MultipartyError::NoShares");
+  std::vector<const Ciphertext*> b0, b1;
+  for (const auto& s : shares) {
+    if (s.round != Round::R2) throw Error(FHE_B200_INVALID_ARGUMENT, "round-2 shares expected");
+    b0.push_back(s.h0.get());
+    b1.push_back(s.h1.get());
+  }
+  const auto h0 = handles(b0), h1 = handles(b1);
+  const Ciphertext& f = *shares[0].h0;
+  fhe_b200_ksk* k = nullptr;
+  check(fhe_b200_rkg_aggregate(table(h0), table(h1), (uint32_t)h0.size(), shares[0].last_round->h1->handle(), &k,
+                               f.stream()));
+  return RelinearizationKey(std::make_shared<KeySwitchingKey>(f.par(), k, 0, 0, f.stream()));
+}
+}  // namespace mbfv
 }  // namespace fhe_b200
