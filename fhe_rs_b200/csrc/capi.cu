@@ -29,33 +29,105 @@ struct ScalerData {
 struct LevelData {
   u32 level = 0, L = 0, E = 0, K = 0;
   RowIds ctx_ids, mul_ids;
+  RowIds ext_ids;                       // the E extension limbs of the multiplication basis
   std::vector<u64> mul_moduli;
+  u64 q_min = 0, q_max = 0;             // of the level's moduli
+  // a lift of plaintext words (< t) onto the level's limbs needs the reduction on load of the forward transform,
+  // whose butterflies take inputs below 4 q_j: t > 4 q_min - 1
+  bool lift_reduce = false;
   ScalerData ext, down;
   bool has_sd = false;
   SwitchDownDev sd;
-  // CipherPlainContext (parameters.rs:604-633): Q_level mod t (when t fits a Modulus) and delta = (-t)^-1 mod q_i
+  // CipherPlainContext (parameters.rs:604-643): Q_level mod t (when t fits a Modulus), delta = (-t)^-1 mod q_i and
+  // the scaler from the level's basis to the plaintext context by t / Q_level
   u64 q_mod_t = 0;
   std::vector<u64> delta;
   const u64 *d_delta = nullptr, *d_delta_s = nullptr;
+  ScalerData plain;
+  // noise measurement: garner [L][L] with (i, j < i) = q_j^-1 mod q_i, and Q_level as W little-endian 64-bit words
+  const u64* garner = nullptr;
+  const u64* q_words = nullptr;
+  u32 W = 0;
 };
 
-// Device copy of one RnsScaler's tables (rns/scaler.rs:79-175).  `to_dev` uploads a vector and keeps ownership of the
-// allocation, `index_of` maps a modulus of the `to` basis to its slot in the limb table the kernels will be given.
-template <typename ToDev, typename IndexOf>
-void upload_scaler_tables(ScalerData& s, const std::vector<u64>& to_moduli, ToDev&& to_dev, IndexOf&& index_of) {
+// Selects a device for the lifetime of the guard and puts the caller's device back afterwards.  Create and compute
+// paths check (`check`): a failed cudaSetDevice throws, and the guard of a parameter set refuses one made without a
+// device with NO_DEVICE before it selects anything.  Release paths never throw and leave no error behind.
+struct DeviceGuard {
+  int prev = -1;
+  const bool check;
+  DeviceGuard(int device, bool check_) : check(check_) {
+    if (device < 0) return;
+    if (cudaGetDevice(&prev) != cudaSuccess) { cudaGetLastError(); prev = -1; }
+    if (prev == device) prev = -1;
+    else if (check) FHE_CUDA(cudaSetDevice(device));
+    else cudaSetDevice(device);
+    if (!check) cudaGetLastError();
+  }
+  explicit DeviceGuard(const fhe_b200_params* p);
+  ~DeviceGuard() {
+    if (prev >= 0) cudaSetDevice(prev);
+    if (!check) cudaGetLastError();
+  }
+  DeviceGuard(const DeviceGuard&) = delete;
+  DeviceGuard& operator=(const DeviceGuard&) = delete;
+};
+
+// The owner of a handle's immutable device tables: `put` uploads a vector on the owner's device and keeps the
+// allocation until the owner goes.  Not thread-safe: the parameter set calls put only while it holds its mutex (the
+// lazy tables of level(), perm() and expansion_monomial_dev()); the other owners fill theirs before their handle is
+// handed out.
+class DeviceTables {
+ public:
+  explicit DeviceTables(int device) : device_(device) {}
+  DeviceTables(const DeviceTables&) = delete;
+  DeviceTables& operator=(const DeviceTables&) = delete;
+  ~DeviceTables() {
+    if (allocs_.empty()) return;
+    DeviceGuard g(device_, false);
+    for (void* d : allocs_) cudaFree(d);
+  }
+  // nullptr for an empty vector or a host-only parameter set (device < 0)
+  template <typename T>
+  T* put(const std::vector<T>& v) {
+    if (device_ < 0 || v.empty()) return nullptr;
+    DeviceGuard g(device_, true);   // tables are built lazily, possibly from a thread on another device
+    T* d = nullptr;
+    FHE_CUDA(cudaMalloc(&d, v.size() * sizeof(T)));
+    allocs_.push_back(d);
+    FHE_CUDA(cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+    return d;
+  }
+
+ private:
+  const int device_;
+  std::vector<void*> allocs_;
+};
+
+// the slot of prime q in a limb table, -1 when it has none
+int prime_index(const std::vector<u64>& primes, u64 q) {
+  for (size_t i = 0; i < primes.size(); i++)
+    if (primes[i] == q) return (int)i;
+  return -1;
+}
+
+// Device copy of one RnsScaler's tables (rns/scaler.rs:79-175), owned by `tables`.  `limb_primes` are the primes of the
+// limb table the kernels will be given, in which every modulus of the `to` basis has its slot.
+void upload_scaler_tables(ScalerData& s, const std::vector<u64>& to_moduli, const std::vector<u64>& limb_primes,
+                          DeviceTables& tables) {
   ScalerDev& d = s.dev;
   std::memset(&d, 0, sizeof(d));
   d.n_from = s.h.n_from; d.n_to = s.h.n_to; d.is_one = s.h.is_one; d.shift = s.h.shift;
   d.tg_lo = s.h.theta_gamma_lo; d.tg_hi = s.h.theta_gamma_hi; d.tg_sign = s.h.theta_gamma_sign;
-  for (size_t j = 0; j < to_moduli.size(); j++) d.to_ids[j] = (unsigned short)index_of(to_moduli[j]);
+  for (size_t j = 0; j < to_moduli.size(); j++) d.to_ids[j] = (unsigned short)prime_index(limb_primes, to_moduli[j]);
   d.all_solinas = switches().no_solinas ? 0 : 1;
   for (u64 q : to_moduli)
     if ((q >> 61) != 1 || ((1ull << 62) - q) >= (1ull << 28)) d.all_solinas = 0;
-  d.gamma = to_dev(s.h.gamma);
-  d.omega = to_dev(s.h.omega);
-  d.to_lo = to_dev(s.h.theta_omega_lo);
-  d.to_hi = to_dev(s.h.theta_omega_hi);
-  d.to_sign = to_dev(s.h.theta_omega_sign);
+  d.gamma = tables.put(s.h.gamma);
+  d.omega = tables.put(s.h.omega);
+  d.to_lo = tables.put(s.h.theta_omega_lo);
+  d.to_hi = tables.put(s.h.theta_omega_hi);
+  d.to_sign = tables.put(s.h.theta_omega_sign);
   // source indices of the theta_omega terms, positive sign first (the kernel makes one pass per sign).  Terms whose
   // fractional part is exactly zero add nothing (rns/scaler.rs:282-298 multiplies them by zero) and are left out:
   // in the down scaler of the multiplication basis that is every extension limb (garner_i * t / Q is an integer).
@@ -69,9 +141,39 @@ void upload_scaler_tables(ScalerData& s, const std::vector<u64>& to_moduli, ToDe
       }
   d.n_terms = (u32)order.size();
   if (order.empty()) order.push_back(0);   // keep the table non-empty (never read: n_terms == 0)
-  d.to_order = to_dev(order);
-  d.tgar_lo = to_dev(s.h.theta_garner_lo);
-  d.tgar_hi = to_dev(s.h.theta_garner_hi);
+  d.to_order = tables.put(order);
+  d.tgar_lo = tables.put(s.h.theta_garner_lo);
+  d.tgar_hi = tables.put(s.h.theta_garner_hi);
+}
+
+// Per-prime device constants and twiddle tables (NttOperator::new, ntt/native.rs:35-73, as (value, companion) pairs).
+LimbDev make_limb_dev(u64 q, const NttTablesH& t, DeviceTables& tables) {
+  ModulusH m(q);
+  LimbDev d;
+  std::memset(&d, 0, sizeof(d));
+  d.p = q; d.p2 = 2 * q; d.bhi = m.bhi; d.blo = m.blo; d.c128 = m.c128;
+  d.ninv = t.ninv; d.zn = t.zn;
+  // limb mode: p = 2^62 - c with c < 2^28 takes the Solinas constant-multiplication form
+  const u64 cc = (1ull << 62) - q;
+  const bool sol = (q >> 61) == 1 && cc < (1ull << 28) && !switches().no_solinas;
+  // NTT butterflies: Shoup pairs by default (no Solinas instruction selection timed in bench_micro/bf_bench.cu beat
+  // them); FHE_B200_SOLINAS_NTT=1 selects the (w, w*2^32 mod p) pairs instead
+  const bool sol_ntt = switches().solinas_ntt;
+  auto pairs = [&](const std::vector<u64>& v, const std::vector<u64>& shoup) {
+    std::vector<ulonglong2> o(v.size());
+    for (size_t k = 0; k < v.size(); k++) {
+      o[k].x = v[k];
+      o[k].y = (sol && sol_ntt) ? (u64)((((u128)v[k]) << 32) % q) : shoup[k];
+    }
+    return o;
+  };
+  d.sol_c = sol ? cc : 0;
+  d.sol_ntt = (sol && sol_ntt) ? 1 : 0;
+  d.ninv_s = (sol && sol_ntt) ? (u64)((((u128)t.ninv) << 32) % q) : t.ninv_s;
+  d.zn_s = (sol && sol_ntt) ? (u64)((((u128)t.zn) << 32) % q) : t.zn_s;
+  d.om = tables.put(pairs(t.om, t.om_s));
+  d.zi = tables.put(pairs(t.zi, t.zi_s));
+  return d;
 }
 
 }  // namespace
@@ -81,7 +183,7 @@ struct fhe_b200_params {
   // reference, so the tables outlive every handle that points at them regardless of the order
   // in which a garbage-collected host releases its objects.
   std::atomic<int> refs{1};
-  int device = -1;
+  const int device;
   u32 N = 0, logn = 0, Lmax = 0;
   std::vector<u64> moduli, ext, primes, psi;
   std::vector<u32> moduli_sizes;
@@ -91,7 +193,7 @@ struct fhe_b200_params {
   std::vector<NttTablesH> tables;  // host copies (kept for inspection / host-only handles)
   std::vector<LimbDev> h_limbs;
   LimbDev* d_limbs = nullptr;
-  std::vector<void*> d_allocs;
+  mutable DeviceTables uploads;
   // scratch of the batched operations comes from a stream-ordered pool this parameter set owns (the device's default
   // pool, which a host application may be using for its own cudaMallocAsync calls, is left untouched)
   cudaMemPool_t pool = nullptr;
@@ -101,30 +203,18 @@ struct fhe_b200_params {
   mutable std::map<u32, std::unique_ptr<LevelData>> levels;
   mutable std::map<u32, int*> perms;
 
-  template <typename T>
-  T* to_dev(const std::vector<T>& v) const {
-    if (device < 0 || v.empty()) return nullptr;
-    T* d = nullptr;
-    // tables are built lazily, possibly from a thread whose current device differs: select ours, put theirs back
-    struct Restore {
-      int prev = -1;
-      ~Restore() { if (prev >= 0) cudaSetDevice(prev); }
-    } restore;
-    if (cudaGetDevice(&restore.prev) != cudaSuccess) { cudaGetLastError(); restore.prev = -1; }
-    if (restore.prev == device) restore.prev = -1;
-    else FHE_CUDA(cudaSetDevice(device));
-    FHE_CUDA(cudaMalloc(&d, v.size() * sizeof(T)));
-    const_cast<fhe_b200_params*>(this)->d_allocs.push_back(d);   // owned from here on (freed with the set)
-    FHE_CUDA(cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-    return d;
-  }
-  int prime_index(u64 q) const {
-    for (size_t i = 0; i < primes.size(); i++)
-      if (primes[i] == q) return (int)i;
-    return -1;
-  }
-  void upload_scaler(ScalerData& s, const std::vector<u64>& to_moduli) const {
-    upload_scaler_tables(s, to_moduli, [&](const auto& v) { return to_dev(v); }, [&](u64 q) { return prime_index(q); });
+  explicit fhe_b200_params(int dev) : device(dev), uploads(dev) {}
+
+  // the plaintext context: the first moduli whose sizes add up to bits(t) + 60 (parameters.rs:579-595)
+  u32 plaintext_moduli_count() const {
+    const size_t t_bits = t.bits();
+    u32 pc = 0, acc = 0;
+    for (u32 sz : moduli_sizes) {
+      acc += sz;
+      pc++;
+      if (acc >= t_bits + 60) break;
+    }
+    return std::min(std::max(pc, 1u), Lmax);
   }
 
   // ContextLevel + MultiplicationParameters of one level (bfv/parameters.rs:600-700, :793-813)
@@ -146,15 +236,20 @@ struct fhe_b200_params {
     d->mul_moduli.insert(d->mul_moduli.end(), ext.begin(), ext.begin() + d->E);
     std::memset(&d->ctx_ids, 0, sizeof(RowIds));
     std::memset(&d->mul_ids, 0, sizeof(RowIds));
+    std::memset(&d->ext_ids, 0, sizeof(RowIds));
     d->ctx_ids.limbs_per_poly = d->L;
     d->mul_ids.limbs_per_poly = d->K;
+    d->ext_ids.limbs_per_poly = d->E;
     for (u32 i = 0; i < d->L; i++) d->ctx_ids.ids[i] = d->mul_ids.ids[i] = (unsigned short)i;
-    for (u32 j = 0; j < d->E; j++) d->mul_ids.ids[d->L + j] = (unsigned short)(Lmax + j);
+    for (u32 j = 0; j < d->E; j++) d->mul_ids.ids[d->L + j] = d->ext_ids.ids[j] = (unsigned short)(Lmax + j);
+    d->q_min = *std::min_element(ctx.begin(), ctx.end());
+    d->q_max = *std::max_element(ctx.begin(), ctx.end());
+    d->lift_reduce = t_mod.t > 4 * d->q_min - 1;
     RnsContextH from(ctx), to(d->mul_moduli);
     d->ext.h = make_scaler_tables(from, to, BigUint(1), BigUint(1));
     d->down.h = make_scaler_tables(to, from, t, from.product);
-    upload_scaler(d->ext, d->mul_moduli);
-    upload_scaler(d->down, ctx);
+    upload_scaler_tables(d->ext, d->mul_moduli, primes, uploads);
+    upload_scaler_tables(d->down, ctx, primes, uploads);
     if (d->L >= 2) {  // rq/context.rs:65-71 and rq/mod.rs:444-468
       d->has_sd = true;
       u64 ql = ctx.back();
@@ -168,9 +263,9 @@ struct fhe_b200_params {
       }
       d->sd.q_last = ql;
       d->sd.q_last_half = ql / 2;
-      d->sd.half_mod = to_dev(half_mod);
-      d->sd.inv = to_dev(inv);
-      d->sd.inv_s = to_dev(inv_s);
+      d->sd.half_mod = uploads.put(half_mod);
+      d->sd.inv = uploads.put(inv);
+      d->sd.inv_s = uploads.put(inv_s);
     }
     if (t_small) d->q_mod_t = from.product.mod_u64(t_mod.t);
     std::vector<u64> delta_s;
@@ -180,8 +275,23 @@ struct fhe_b200_params {
       d->delta.push_back(iv);
       delta_s.push_back(ModulusH(qi).shoup(iv));
     }
-    d->d_delta = to_dev(d->delta);
-    d->d_delta_s = to_dev(delta_s);
+    d->d_delta = uploads.put(d->delta);
+    d->d_delta_s = uploads.put(delta_s);
+    const std::vector<u64> plain(moduli.begin(), moduli.begin() + plaintext_moduli_count());
+    d->plain.h = make_scaler_tables(from, RnsContextH(plain), t, from.product);   // parameters.rs:638-643
+    upload_scaler_tables(d->plain, plain, primes, uploads);
+    std::vector<u64> garner((size_t)d->L * d->L, 0);
+    for (u32 i = 0; i < d->L; i++)
+      for (u32 j = 0; j < i; j++)
+        if (!invmod_h(ctx[j] % ctx[i], ctx[i], &garner[(size_t)i * d->L + j]))
+          throw FheError(FHE_B200_INVALID_MODULUS, "NonCoprimeModuli");
+    d->garner = uploads.put(garner);
+    std::vector<u64> qw;
+    const BigUint& Q = from.product;
+    for (size_t k = 0; k < Q.w.size(); k += 2)
+      qw.push_back((u64)Q.w[k] | (k + 1 < Q.w.size() ? (u64)Q.w[k + 1] << 32 : 0));
+    d->W = (u32)qw.size();
+    d->q_words = uploads.put(qw);
     auto* raw = d.get();
     levels[lv] = std::move(d);
     return *raw;
@@ -204,7 +314,7 @@ struct fhe_b200_params {
       p[brev(j)] = (int)brev((u32)(power & (N - 1)));
       power += exponent;
     }
-    int* d = to_dev(p);
+    int* d = uploads.put(p);
     perms[exponent] = d;
     return d;
   }
@@ -248,32 +358,107 @@ struct fhe_b200_params {
         pairs[k].y = mq.shoup(w[k]);
       }
     }
-    const ulonglong2* d = to_dev(pairs);
+    const ulonglong2* d = uploads.put(pairs);
     monos[{lv, l}] = d;
     return d;
   }
   mutable std::map<std::pair<u32, u32>, const ulonglong2*> monos;
 };
 
+namespace {
+
+void params_release(const fhe_b200_params* cp) {
+  fhe_b200_params* p = const_cast<fhe_b200_params*>(cp);
+  if (!p || p->refs.fetch_sub(1) != 1) return;
+  if (p->device >= 0) {
+    DeviceGuard g(p->device, false);
+    for (cudaStream_t ss : p->side)
+      if (ss) cudaStreamDestroy(ss);
+    if (p->pool) {
+      cudaDeviceSynchronize();   // scratch freed with cudaFreeAsync must have retired before its pool goes away
+      cudaMemPoolDestroy(p->pool);
+    }
+  }
+  delete p;   // its device tables go with it
+}
+const fhe_b200_params* params_retain(const fhe_b200_params* p) {
+  const_cast<fhe_b200_params*>(p)->refs.fetch_add(1);
+  return p;
+}
+
+// A handle's reference on its parameter set (fhe_b200_params::refs): retained when the handle is made, released when
+// it goes.  Every handle declares it first, so that its other members, device memory included, are released while the
+// set and its device are still there.
+class ParamsRef {
+ public:
+  explicit ParamsRef(const fhe_b200_params* p) : p_(params_retain(p)) {}
+  ~ParamsRef() { params_release(p_); }
+  ParamsRef(const ParamsRef&) = delete;
+  ParamsRef& operator=(const ParamsRef&) = delete;
+  operator const fhe_b200_params*() const { return p_; }
+  const fhe_b200_params* operator->() const { return p_; }
+
+ private:
+  const fhe_b200_params* const p_;
+};
+
+// Device words derived from a secret (SecretKey's s, the relinearization-key generator's u), erased before they are
+// freed as SecretKey's Zeroize erases s (secret_key.rs:28-40).  Work that reads the words may still be queued on
+// streams that do not order against the legacy stream the memset runs on (the chunk runner's side streams, a caller's
+// non-blocking stream): the release waits for the device first, as cudaFree would, so that releasing the handle right
+// after an enqueue-only call is as safe as releasing any other handle.
+struct SecretBuffer {
+  const int device;
+  const size_t bytes;
+  u64* d = nullptr;
+  SecretBuffer(int dev, size_t words) : device(dev), bytes(words * sizeof(u64)) { FHE_CUDA(cudaMalloc(&d, bytes)); }
+  ~SecretBuffer() {
+    DeviceGuard g(device, false);
+    cudaDeviceSynchronize();
+    cudaMemset(d, 0, bytes);
+    cudaDeviceSynchronize();
+    cudaFree(d);
+  }
+  SecretBuffer(const SecretBuffer&) = delete;
+  SecretBuffer& operator=(const SecretBuffer&) = delete;
+};
+
+}  // namespace
+
+DeviceGuard::DeviceGuard(const fhe_b200_params* p) : DeviceGuard(p->device, true) {
+  if (p->device < 0) throw FheError(FHE_B200_NO_DEVICE, "parameter set was created without a CUDA device");
+}
+
 struct fhe_b200_batch {
-  const fhe_b200_params* par;
-  u32 count, parts, level, limbs;
-  int repr;
-  bool mul_basis;
-  u64* d;
+  ParamsRef par;
+  u32 count = 0, parts = 0, level = 0, limbs = 0;
+  int repr = 0;
+  bool mul_basis = false;
+  u64* d = nullptr;
+  explicit fhe_b200_batch(const fhe_b200_params* p) : par(p) {}
+  ~fhe_b200_batch() {
+    DeviceGuard g(par->device, false);
+    cudaFree(d);
+  }
   size_t words_per_ct() const { return ((size_t)parts * limbs) << par->logn; }
 };
 
 struct fhe_b200_ksk {
-  const fhe_b200_params* par;
-  u32 ct_level, ksk_level, n_dig, Lk;
-  u32 log_base;   // 0: RNS-digit variant; else base-2^log_base decomposition (single-modulus key level)
-  u64 *k0, *k1;
+  ParamsRef par;
+  u32 ct_level = 0, ksk_level = 0, n_dig = 0, Lk = 0;
+  u32 log_base = 0;   // 0: RNS-digit variant; else base-2^log_base decomposition (single-modulus key level)
+  u64 *k0 = nullptr, *k1 = nullptr;
+  explicit fhe_b200_ksk(const fhe_b200_params* p) : par(p) {}
+  ~fhe_b200_ksk() {
+    DeviceGuard g(par->device, false);
+    cudaFree(k0);
+    cudaFree(k1);
+  }
 };
 
 // Multiplicator::new / new_leveled (bfv/ops/mul.rs:37-98): custom scaling factors and extended basis.
 struct fhe_b200_multiplicator {
-  const fhe_b200_params* par;
+  ParamsRef par;
   u32 level = 0, L = 0, K = 0;
   u32 nc_l = 0, nc_r = 0, nc_d = 0;     // Scaler::number_common_moduli of the two extenders and the down scaler
   std::vector<u64> mul_moduli, plan_primes;
@@ -281,31 +466,15 @@ struct fhe_b200_multiplicator {
   std::vector<LimbDev> h_limbs;          // the parameter set's limbs followed by the primes only this basis has
   LimbDev* d_limbs = nullptr;
   ScalerData ext_l, ext_r, down;
-  std::vector<void*> d_allocs;
-  template <typename T>
-  T* to_dev(const std::vector<T>& v) {
-    if (v.empty()) return nullptr;
-    T* d = nullptr;
-    FHE_CUDA(cudaMalloc(&d, v.size() * sizeof(T)));
-    d_allocs.push_back(d);
-    FHE_CUDA(cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-    return d;
-  }
-  int prime_index(u64 q) const {
-    for (size_t i = 0; i < plan_primes.size(); i++)
-      if (plan_primes[i] == q) return (int)i;
-    return -1;
-  }
-  void upload_scaler(ScalerData& sd, const std::vector<u64>& to_moduli) {
-    upload_scaler_tables(sd, to_moduli, [&](const auto& v) { return to_dev(v); }, [&](u64 q) { return prime_index(q); });
-  }
+  DeviceTables uploads;
+  explicit fhe_b200_multiplicator(const fhe_b200_params* p) : par(p), uploads(p->device) {}
 };
 
 // The plaintext side of BfvParameters: the NTT operator of t (parameters.rs:71-75, :598) and the SIMD slot map
 // (matrix_reps_index_map, :713-726).  Its limb table is the parameter set's followed by t, so the level RowIds of
 // the parameter set index it unchanged.
 struct fhe_b200_encoder {
-  const fhe_b200_params* par;
+  ParamsRef par;
   bool has_ntt = false;                 // NttOperator::new(t) is Some (ntt/native.rs:35-73)
   u64 psi_t = 0;
   NttTablesH tables;                    // of t, when has_ntt
@@ -315,142 +484,20 @@ struct fhe_b200_encoder {
   u32* d_inv_map = nullptr;             // coefficient index -> slot
   int* d_index_map = nullptr;           // index_map on the device (the decoders' gather)
   RowIds t_ids;                         // one row per plaintext, all modulo t
-  // cipher_plain_context.scaler of each level (parameters.rs:638-643), built on first use by
-  // fhe_b200_decryption_aggregate: the aggregator of a collective decryption holds no secret key
-  std::mutex mu;
-  std::map<u32, std::unique_ptr<ScalerData>> plain_scalers;
-  std::vector<void*> d_allocs;
-  template <typename T>
-  T* to_dev(const std::vector<T>& v) {
-    if (par->device < 0 || v.empty()) return nullptr;
-    T* d = nullptr;
-    FHE_CUDA(cudaMalloc(&d, v.size() * sizeof(T)));
-    d_allocs.push_back(d);
-    FHE_CUDA(cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-    return d;
-  }
+  DeviceTables uploads;
+  explicit fhe_b200_encoder(const fhe_b200_params* p) : par(p), uploads(p->device) {}
 };
 
 // SecretKey (keys/secret_key.rs:25-53) on the device: s as NTT words modulo every modulus of the parameter set (the
-// context of level l is the prefix moduli[..L-l], so every level reads a prefix of the same rows), and per level the
-// tables decryption and noise measurement need.  The words of s are erased before they are freed.
+// context of level l is the prefix moduli[..L-l], so every level reads a prefix of the same rows).  The tables that
+// decryption and noise measurement read are the level's (LevelData).
 struct fhe_b200_secret_key {
-  const fhe_b200_params* par;
-  u64* s = nullptr;                     // [n_moduli][N]
-  struct Level {
-    ScalerData scaler;                  // cipher_plain_context.scaler: level basis -> plaintext context, t / Q_level
-    const u64* garner = nullptr;        // [L][L]: (i, j < i) = q_j^-1 mod q_i
-    const u64* q_words = nullptr;       // Q_level as little-endian 64-bit words
-    u32 W = 0;
-  };
-  std::vector<Level> levels;
-  std::vector<void*> d_allocs;
-  template <typename T>
-  T* to_dev(const std::vector<T>& v) {
-    if (v.empty()) return nullptr;
-    T* d = nullptr;
-    FHE_CUDA(cudaMalloc(&d, v.size() * sizeof(T)));
-    d_allocs.push_back(d);
-    FHE_CUDA(cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-    return d;
-  }
+  ParamsRef par;
+  SecretBuffer s;                       // [n_moduli][N]
+  explicit fhe_b200_secret_key(const fhe_b200_params* p) : par(p), s(p->device, (size_t)p->Lmax * p->N) {}
 };
 
 namespace {
-
-void params_release(const fhe_b200_params* cp) {
-  fhe_b200_params* p = const_cast<fhe_b200_params*>(cp);
-  if (!p || p->refs.fetch_sub(1) != 1) return;
-  if (p->device >= 0) {
-    int prev = -1;
-    cudaGetDevice(&prev);
-    cudaSetDevice(p->device);
-    for (void* d : p->d_allocs) cudaFree(d);
-    for (cudaStream_t ss : p->side)
-      if (ss) cudaStreamDestroy(ss);
-    if (p->pool) {
-      cudaDeviceSynchronize();   // scratch freed with cudaFreeAsync must have retired before its pool goes away
-      cudaMemPoolDestroy(p->pool);
-    }
-    if (prev >= 0) cudaSetDevice(prev);
-    cudaGetLastError();
-  }
-  delete p;
-}
-const fhe_b200_params* params_retain(const fhe_b200_params* p) {
-  const_cast<fhe_b200_params*>(p)->refs.fetch_add(1);
-  return p;
-}
-
-// Per-prime device constants and twiddle tables (NttOperator::new, ntt/native.rs:35-73, as (value, companion) pairs).
-template <typename ToDev>
-LimbDev make_limb_dev(u64 q, const NttTablesH& t, ToDev&& to_dev) {
-  ModulusH m(q);
-  LimbDev d;
-  std::memset(&d, 0, sizeof(d));
-  d.p = q; d.p2 = 2 * q; d.bhi = m.bhi; d.blo = m.blo; d.c128 = m.c128;
-  d.ninv = t.ninv; d.zn = t.zn;
-  // limb mode: p = 2^62 - c with c < 2^28 takes the Solinas constant-multiplication form
-  const u64 cc = (1ull << 62) - q;
-  const bool sol = (q >> 61) == 1 && cc < (1ull << 28) && !switches().no_solinas;
-  // NTT butterflies: Shoup pairs by default (no Solinas instruction selection timed in bench_micro/bf_bench.cu beat
-  // them); FHE_B200_SOLINAS_NTT=1 selects the (w, w*2^32 mod p) pairs instead
-  const bool sol_ntt = switches().solinas_ntt;
-  auto pairs = [&](const std::vector<u64>& v, const std::vector<u64>& shoup) {
-    std::vector<ulonglong2> o(v.size());
-    for (size_t k = 0; k < v.size(); k++) {
-      o[k].x = v[k];
-      o[k].y = (sol && sol_ntt) ? (u64)((((u128)v[k]) << 32) % q) : shoup[k];
-    }
-    return o;
-  };
-  d.sol_c = sol ? cc : 0;
-  d.sol_ntt = (sol && sol_ntt) ? 1 : 0;
-  d.ninv_s = (sol && sol_ntt) ? (u64)((((u128)t.ninv) << 32) % q) : t.ninv_s;
-  d.zn_s = (sol && sol_ntt) ? (u64)((((u128)t.zn) << 32) % q) : t.zn_s;
-  d.om = to_dev(pairs(t.om, t.om_s));
-  d.zi = to_dev(pairs(t.zi, t.zi_s));
-  return d;
-}
-
-// selects the parameter set's device for the duration of an API call and puts the caller's device back afterwards
-struct DeviceGuard {
-  int prev = -1;
-  explicit DeviceGuard(const fhe_b200_params* p) {
-    if (p->device < 0) throw FheError(FHE_B200_NO_DEVICE, "parameter set was created without a CUDA device");
-    if (cudaGetDevice(&prev) != cudaSuccess) { cudaGetLastError(); prev = -1; }
-    if (prev != p->device) FHE_CUDA(cudaSetDevice(p->device));
-    else prev = -1;
-  }
-  ~DeviceGuard() {
-    if (prev >= 0) cudaSetDevice(prev);
-  }
-  DeviceGuard(const DeviceGuard&) = delete;
-  DeviceGuard& operator=(const DeviceGuard&) = delete;
-};
-
-// the same for the release paths: never throws, puts the caller's device back
-struct ScopedDevice {
-  int prev = -1;
-  explicit ScopedDevice(int device) {
-    if (device < 0) return;
-    if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
-    if (prev == device) prev = -1;
-    else cudaSetDevice(device);
-    cudaGetLastError();
-  }
-  ~ScopedDevice() {
-    if (prev >= 0) cudaSetDevice(prev);
-    cudaGetLastError();
-  }
-};
-
-// owning device pointer for the construction of handles (released on commit)
-struct DevPtr {
-  void* p = nullptr;
-  ~DevPtr() { if (p) { cudaFree(p); cudaGetLastError(); } }
-  void* release() { void* r = p; p = nullptr; return r; }
-};
 
 // stream-ordered scratch memory from the parameter set's own pool
 struct Workspace {
@@ -571,13 +618,12 @@ void key_switch_core(const fhe_b200_params* par, const fhe_b200_ksk* k, const u6
   } else {
   // digit broadcast (rq/mod.rs:563-586), then NTT of every (digit, limb) row.  The reference lazily reduces the
   // digit modulo q_j before its lazy transform; the forward butterflies accept any input below 4*q_j, so the
-  // reduction on load is only needed when a digit (< max q_i) can reach 4 * min q_j (mixed modulus sizes).
-  u64 qmax = 0, qmin = ~0ull;
-  for (u32 i = 0; i < L; i++) qmax = std::max(qmax, par->moduli[i]);
-  for (u32 j = 0; j < Lk; j++) qmin = std::min(qmin, par->moduli[j]);
-  // The lifts of plaintext words (encode, to_poly_from_coefficients, decrypt) test only t > 4 * q_min - 1: the
-  // butterflies take [0, 4p) for any modulus, down to q_min = 193 < 2^8 (tests/test_gpu_client_edges.py).  The extra
-  // clause here changes the choice only when every modulus of the key level is below 2^10, which needs N <= 64.
+  // reduction on load is only needed when a digit (< max q_i) can reach 4 * min q_j (mixed modulus sizes).  The
+  // digits are those of the ciphertext level (n_dig = its L), the rows those of the key level.
+  const u64 qmax = par->level(k->ct_level).q_max, qmin = kl.q_min;
+  // The lifts of plaintext words (LevelData::lift_reduce) test only t > 4 * q_min - 1: the butterflies take [0, 4p)
+  // for any modulus, down to q_min = 193 < 2^8 (tests/test_gpu_client_edges.py).  The extra clause here changes the
+  // choice only when every modulus of the key level is below 2^10, which needs N <= 64.
   const bool reduce = qmax > 4 * qmin - 1 || qmin < (1ull << 8);
   // forward_vt_lazy (rq/mod.rs:580): the digits stay in [0,4q_j); the lazy accumulator of the inner product takes
   // any 64-bit operand and reduces once
@@ -664,10 +710,6 @@ void mul_core(const fhe_b200_params* par, const LevelData& lv, const u64* a, con
   u64* X_l = ws.words((size_t)cts * 2 * E * row);
   u64* X_r = ws.words((size_t)cts * 2 * E * row);
   u64* T = ws.words((size_t)cts * 3 * K * row);
-  RowIds ext_ids;
-  std::memset(&ext_ids, 0, sizeof(ext_ids));
-  ext_ids.limbs_per_poly = E;
-  for (u32 j = 0; j < E; j++) ext_ids.ids[j] = lv.mul_ids.ids[L + j];
   // rq/scaler.rs:69-79: backward NTT of the source rows
   launch_ntt(a, A_l, cts * 2 * L, lv.ctx_ids, par->d_limbs, logn, true, 1, false, st);
   launch_ntt(b, A_r, cts * 2 * L, lv.ctx_ids, par->d_limbs, logn, true, 1, false, st);
@@ -675,8 +717,8 @@ void mul_core(const fhe_b200_params* par, const LevelData& lv, const u64* a, con
   launch_scale(lv.ext.dev, par->d_limbs, A_l, X_l, nullptr, cts * 2, E, L, E, 0, logn, st);
   launch_scale(lv.ext.dev, par->d_limbs, A_r, X_r, nullptr, cts * 2, E, L, E, 0, logn, st);
   // rq/scaler.rs:97-115: forward NTT of the new rows
-  launch_ntt(X_l, X_l, cts * 2 * E, ext_ids, par->d_limbs, logn, false, 1, false, st);
-  launch_ntt(X_r, X_r, cts * 2 * E, ext_ids, par->d_limbs, logn, false, 1, false, st);
+  launch_ntt(X_l, X_l, cts * 2 * E, lv.ext_ids, par->d_limbs, logn, false, 1, false, st);
+  launch_ntt(X_r, X_r, cts * 2 * E, lv.ext_ids, par->d_limbs, logn, false, 1, false, st);
   // mul.rs:198-201 tensor product, then mul.rs:204-206 scale down by t/Q (backward NTT of the 3K rows, exact scaling
   // K -> L); product and first inverse pass run as one kernel where the TMA kernels serve the shape
   if (!launch_tensor_inverse_ntt(a, b, X_l, X_r, T, cts, L, K, lv.mul_ids, par->d_limbs, logn, st)) {
@@ -691,10 +733,6 @@ void mul_core_parts(const fhe_b200_params* par, const LevelData& lv, const u64* 
                     u64* out, Workspace& ws, cudaStream_t st) {
   const u32 L = lv.L, E = lv.E, K = lv.K, logn = par->logn, nc = na + nb - 1;
   const size_t row = (size_t)1 << logn;
-  RowIds ext_ids;
-  std::memset(&ext_ids, 0, sizeof(ext_ids));
-  ext_ids.limbs_per_poly = E;
-  for (u32 j = 0; j < E; j++) ext_ids.ids[j] = lv.mul_ids.ids[L + j];
   const u64* src[2] = {a, b};
   const u32 np[2] = {na, nb};
   u64* X[2];
@@ -703,7 +741,7 @@ void mul_core_parts(const fhe_b200_params* par, const LevelData& lv, const u64* 
     X[s] = ws.words((size_t)cts * np[s] * E * row);
     launch_ntt(src[s], pb, cts * np[s] * L, lv.ctx_ids, par->d_limbs, logn, true, 1, false, st);
     launch_scale(lv.ext.dev, par->d_limbs, pb, X[s], nullptr, cts * np[s], E, L, E, 0, logn, st);
-    launch_ntt(X[s], X[s], cts * np[s] * E, ext_ids, par->d_limbs, logn, false, 1, false, st);
+    launch_ntt(X[s], X[s], cts * np[s] * E, lv.ext_ids, par->d_limbs, logn, false, 1, false, st);
   }
   u64* T = ws.words((size_t)cts * nc * K * row);
   launch_tensor_nm(a, b, X[0], X[1], T, cts, L, E, na, nb, lv.mul_ids, par->d_limbs, logn, st);
@@ -778,13 +816,7 @@ static int params_build(int device, uint32_t degree, const std::vector<u64>& mod
           "InvalidPolynomialDegree: " + std::to_string(degree));
   REQUIRE(!moduli.empty() && moduli.size() < 32, FHE_B200_INVALID_ARGUMENT, "MissingCiphertextModulusSpecification");
   // released through params_release on every exit path (frees the device tables and the pool of a half-built set)
-  std::unique_ptr<fhe_b200_params, void (*)(const fhe_b200_params*)> p(new fhe_b200_params(), params_release);
-  struct Restore {   // the caller's current device is left as it was
-    int prev = -1;
-    ~Restore() { if (prev >= 0) cudaSetDevice(prev); }
-  } restore;
-  if (device >= 0 && cudaGetDevice(&restore.prev) != cudaSuccess) { cudaGetLastError(); restore.prev = -1; }
-  p->device = device;
+  std::unique_ptr<fhe_b200_params, void (*)(const fhe_b200_params*)> p(new fhe_b200_params(device), params_release);
   p->N = degree;
   p->logn = (u32)__builtin_ctz(degree);
   p->Lmax = (u32)moduli.size();
@@ -826,7 +858,9 @@ static int params_build(int device, uint32_t degree, const std::vector<u64>& mod
       cudaGetLastError();
       throw FheError(FHE_B200_NO_DEVICE, "CUDA device " + std::to_string(device) + " not available");
     }
-    FHE_CUDA(cudaSetDevice(device));
+  }
+  DeviceGuard g(device, true);   // selects nothing for a host-only set
+  if (device >= 0) {
     cudaMemPoolProps props;
     std::memset(&props, 0, sizeof(props));
     props.allocType = cudaMemAllocationTypePinned;
@@ -846,9 +880,9 @@ static int params_build(int device, uint32_t degree, const std::vector<u64>& mod
     u64 r = psi ? psi[i] : default_psi(q, degree);
     p->psi.push_back(r);
     p->tables.push_back(make_ntt_tables(q, degree, r));
-    p->h_limbs.push_back(make_limb_dev(q, p->tables.back(), [&](const std::vector<ulonglong2>& v) { return p->to_dev(v); }));
+    p->h_limbs.push_back(make_limb_dev(q, p->tables.back(), p->uploads));
   }
-  p->d_limbs = p->to_dev(p->h_limbs);
+  p->d_limbs = p->uploads.put(p->h_limbs);
   *out = p.release();
   API_END
 }
@@ -903,7 +937,7 @@ int fhe_b200_params_mul_basis(const fhe_b200_params* p, uint32_t level, uint64_t
 }
 int fhe_b200_params_psi(const fhe_b200_params* p, uint64_t q, uint64_t* psi) {
   if (!p || !psi) return FHE_B200_INVALID_ARGUMENT;
-  int i = p->prime_index(q);
+  int i = prime_index(p->primes, q);
   if (i < 0) { g_last_error = "prime not in parameter set"; return FHE_B200_INVALID_MODULUS; }
   *psi = p->psi[i];
   return FHE_B200_OK;
@@ -918,13 +952,11 @@ static int batch_alloc(const fhe_b200_params* p, uint32_t count, uint32_t parts,
   REQUIRE(repr == FHE_B200_POWER_BASIS || repr == FHE_B200_NTT, FHE_B200_INVALID_REPRESENTATION, "bad representation");
   DeviceGuard g(p);
   const LevelData& lv = p->level(level);
-  std::unique_ptr<fhe_b200_batch> b(new fhe_b200_batch());
-  b->par = p; b->count = count; b->parts = parts; b->level = level; b->repr = repr;
+  std::unique_ptr<fhe_b200_batch> b(new fhe_b200_batch(p));
+  b->count = count; b->parts = parts; b->level = level; b->repr = repr;
   b->mul_basis = mul_basis;
   b->limbs = mul_basis ? lv.K : lv.L;
-  b->d = nullptr;
   FHE_CUDA(cudaMalloc(&b->d, b->words_per_ct() * count * sizeof(u64)));
-  params_retain(p);
   *out = b.release();
   API_END
 }
@@ -937,13 +969,6 @@ int fhe_b200_batch_alloc_mul_basis(const fhe_b200_params* p, uint32_t count, uin
   return batch_alloc(p, count, parts, level, repr, true, out);
 }
 int fhe_b200_batch_free(fhe_b200_batch* b) {
-  if (!b) return FHE_B200_OK;
-  {
-    ScopedDevice g(b->par->device);
-    cudaFree(b->d);
-    cudaGetLastError();
-  }
-  params_release(b->par);
   delete b;
   return FHE_B200_OK;
 }
@@ -1047,6 +1072,18 @@ static u32 ksk_digits(const fhe_b200_params* p, const LevelData& cl, const Level
   return (log_modulus + log_base - 1) / log_base;
 }
 
+// A key handle with room for its words: both parts in the device layout [limb][digit][N] of n_dig digits over the Lk
+// limbs of the key level
+static std::unique_ptr<fhe_b200_ksk> make_ksk(const fhe_b200_params* p, u32 ct_level, u32 ksk_level, u32 n_dig, u32 Lk,
+                                              u32 log_base) {
+  std::unique_ptr<fhe_b200_ksk> k(new fhe_b200_ksk(p));
+  k->ct_level = ct_level; k->ksk_level = ksk_level; k->n_dig = n_dig; k->Lk = Lk; k->log_base = log_base;
+  const size_t bytes = ((size_t)n_dig * Lk << p->logn) * sizeof(u64);
+  FHE_CUDA(cudaMalloc(&k->k0, bytes));
+  FHE_CUDA(cudaMalloc(&k->k1, bytes));
+  return k;
+}
+
 int fhe_b200_ksk_upload(const fhe_b200_params* p, uint32_t ciphertext_level, uint32_t ksk_level, const uint64_t* c0,
                         const uint64_t* c1, uint32_t n_digits, fhe_b200_ksk** out) {
   API_BEGIN
@@ -1060,24 +1097,15 @@ int fhe_b200_ksk_upload(const fhe_b200_params* p, uint32_t ciphertext_level, uin
   REQUIRE(n_digits == want, FHE_B200_CONTEXT_MISMATCH,
           log_base ? "n_digits must be ceil(log_modulus / log_base) for a single-modulus key"
                    : "n_digits must equal the ciphertext level's limb count");
-  std::unique_ptr<fhe_b200_ksk> k(new fhe_b200_ksk());
-  k->par = p; k->ct_level = ciphertext_level; k->ksk_level = ksk_level; k->n_dig = n_digits; k->Lk = kl.L;
-  k->log_base = log_base;
-  size_t bytes = ((size_t)n_digits * kl.L << p->logn) * sizeof(u64);
-  DevPtr g0, g1;   // freed again if anything below fails
-  FHE_CUDA(cudaMalloc(&g0.p, bytes));
-  FHE_CUDA(cudaMalloc(&g1.p, bytes));
+  std::unique_ptr<fhe_b200_ksk> k = make_ksk(p, ciphertext_level, ksk_level, n_digits, kl.L, log_base);
   // host layout [digit][limb][N] -> device layout [limb][digit][N]: the inner product walks the digits of one limb
   const size_t rowb = sizeof(u64) << p->logn;
   for (u32 i = 0; i < n_digits; i++) {
-    FHE_CUDA(cudaMemcpy2D((char*)g0.p + i * rowb, n_digits * rowb, (const char*)c0 + (size_t)i * kl.L * rowb, rowb, rowb,
-                          kl.L, cudaMemcpyHostToDevice));
-    FHE_CUDA(cudaMemcpy2D((char*)g1.p + i * rowb, n_digits * rowb, (const char*)c1 + (size_t)i * kl.L * rowb, rowb, rowb,
-                          kl.L, cudaMemcpyHostToDevice));
+    FHE_CUDA(cudaMemcpy2D((char*)k->k0 + i * rowb, n_digits * rowb, (const char*)c0 + (size_t)i * kl.L * rowb, rowb,
+                          rowb, kl.L, cudaMemcpyHostToDevice));
+    FHE_CUDA(cudaMemcpy2D((char*)k->k1 + i * rowb, n_digits * rowb, (const char*)c1 + (size_t)i * kl.L * rowb, rowb,
+                          rowb, kl.L, cudaMemcpyHostToDevice));
   }
-  k->k0 = (u64*)g0.release();
-  k->k1 = (u64*)g1.release();
-  params_retain(p);
   *out = k.release();
   API_END
 }
@@ -1098,14 +1126,6 @@ int fhe_b200_ksk_download(const fhe_b200_ksk* k, uint64_t* c0, uint64_t* c1, voi
   API_END
 }
 int fhe_b200_ksk_free(fhe_b200_ksk* k) {
-  if (!k) return FHE_B200_OK;
-  {
-    ScopedDevice g(k->par->device);
-    cudaFree(k->k0);
-    cudaFree(k->k1);
-    cudaGetLastError();
-  }
-  params_release(k->par);
   delete k;
   return FHE_B200_OK;
 }
@@ -1195,13 +1215,7 @@ int fhe_b200_dot_product_scalar(const fhe_b200_batch* cts, const fhe_b200_batch*
 int fhe_b200_encoder_create(const fhe_b200_params* p, const uint64_t* psi_t, fhe_b200_encoder** out) {
   API_BEGIN
   REQUIRE(p && out, FHE_B200_INVALID_ARGUMENT, "null argument");
-  ScopedDevice g(p->device);
-  std::unique_ptr<fhe_b200_encoder> e(new fhe_b200_encoder());
-  struct Cleanup {   // frees the device tables if construction throws
-    fhe_b200_encoder* e;
-    ~Cleanup() { if (e) { for (void* d : e->d_allocs) cudaFree(d); cudaGetLastError(); } }
-  } cleanup{e.get()};
-  e->par = p;
+  std::unique_ptr<fhe_b200_encoder> e(new fhe_b200_encoder(p));
   const u32 N = p->N;
   // parameters.rs:713-726
   e->index_map.resize(N);
@@ -1229,25 +1243,16 @@ int fhe_b200_encoder_create(const fhe_b200_params* p, const uint64_t* psi_t, fhe
   if (e->has_ntt) {
     e->psi_t = psi_t ? *psi_t : default_psi(t, N);
     e->tables = make_ntt_tables(t, N, e->psi_t);
-    e->h_limbs.push_back(make_limb_dev(t, e->tables, [&](const std::vector<ulonglong2>& v) { return e->to_dev(v); }));
+    e->h_limbs.push_back(make_limb_dev(t, e->tables, e->uploads));
   }
-  e->d_limbs = e->to_dev(e->h_limbs);
-  e->d_inv_map = e->to_dev(inv);
-  e->d_index_map = e->to_dev(std::vector<int>(e->index_map.begin(), e->index_map.end()));
-  params_retain(p);
-  cleanup.e = nullptr;
+  e->d_limbs = e->uploads.put(e->h_limbs);
+  e->d_inv_map = e->uploads.put(inv);
+  e->d_index_map = e->uploads.put(std::vector<int>(e->index_map.begin(), e->index_map.end()));
   *out = e.release();
   API_END
 }
 
 int fhe_b200_encoder_free(fhe_b200_encoder* e) {
-  if (!e) return FHE_B200_OK;
-  if (e->par->device >= 0) {
-    ScopedDevice g(e->par->device);
-    for (void* d : e->d_allocs) cudaFree(d);
-    cudaGetLastError();
-  }
-  params_release(e->par);
   delete e;
   return FHE_B200_OK;
 }
@@ -1275,9 +1280,7 @@ int fhe_b200_encode(const fhe_b200_encoder* e, int encoding, int is_signed, cons
   const u32 L = lv.L, logn = par->logn;
   const bool poly_u64 = !simd && !is_signed;
   // forward butterflies take inputs below 4 q_j: Poly u64 words are arbitrary, the other words are below t
-  u64 qmin = ~0ull;
-  for (u32 j = 0; j < L; j++) qmin = std::min(qmin, par->moduli[j]);
-  const bool reduce = poly_u64 || par->t_mod.t > 4 * qmin - 1;
+  const bool reduce = poly_u64 || lv.lift_reduce;
   const char* src = (const char*)values;
   ChunkRunner chunks(par, (u32)count, (cudaStream_t)stream);
   chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
@@ -1333,11 +1336,8 @@ static RowIds q0_row_ids() {
 // transformed into m [n][L][N]
 static void to_poly_from_coefficients(const fhe_b200_params* par, const LevelData& lv, u64* x, u32 n, u64* m,
                                       cudaStream_t st) {
-  u64 qmin = ~0ull;
-  for (u32 j = 0; j < lv.L; j++) qmin = std::min(qmin, par->moduli[j]);
-  const bool reduce = par->t_mod.t > 4 * qmin - 1;
   launch_to_poly_load(x, (size_t)n << par->logn, par->t_mod, lv.q_mod_t, st);
-  launch_ntt(x, m, n * lv.L, lv.ctx_ids, par->d_limbs, par->logn, false, lv.L, reduce, st);
+  launch_ntt(x, m, n * lv.L, lv.ctx_ids, par->d_limbs, par->logn, false, lv.L, lv.lift_reduce, st);
 }
 
 // Plaintext::to_poly (plaintext.rs:172-197) of plaintexts [p0, p0 + n) of the 1-part NTT batch pts into m [n][L][N],
@@ -1386,35 +1386,12 @@ int fhe_b200_add_plain_batch(fhe_b200_batch* a, const fhe_b200_batch* pts, int s
 }
 
 // ---- decryption, decoding and noise measurement
-// the plaintext context: the first moduli whose sizes add up to bits(t) + 60 (parameters.rs:579-595)
-static u32 plaintext_moduli_count(const fhe_b200_params* p) {
-  const size_t t_bits = p->t.bits();
-  u32 pc = 0, acc = 0;
-  for (u32 sz : p->moduli_sizes) {
-    acc += sz;
-    pc++;
-    if (acc >= t_bits + 60) break;
-  }
-  return std::min(std::max(pc, 1u), p->Lmax);
-}
-
 int fhe_b200_secret_key_create(const fhe_b200_params* p, const int64_t* coeffs, fhe_b200_secret_key** out) {
   API_BEGIN
   REQUIRE(p && coeffs && out, FHE_B200_INVALID_ARGUMENT, "null argument");
   REQUIRE(p->t_small, FHE_B200_UNSUPPORTED, "the plaintext modulus does not fit a u64 Modulus");
   DeviceGuard g(p);
-  std::unique_ptr<fhe_b200_secret_key> sk(new fhe_b200_secret_key());
-  struct Cleanup {   // frees the device tables (and erases s) if construction throws
-    fhe_b200_secret_key* k;
-    size_t s_bytes;
-    ~Cleanup() {
-      if (!k) return;
-      if (k->s) cudaMemset(k->s, 0, s_bytes);
-      for (void* d : k->d_allocs) cudaFree(d);
-      cudaGetLastError();
-    }
-  } cleanup{sk.get(), ((size_t)p->Lmax * p->N) * sizeof(u64)};
-  sk->par = p;
+  std::unique_ptr<fhe_b200_secret_key> sk(new fhe_b200_secret_key(p));
   const u32 N = p->N, Lmax = p->Lmax;
   // Poly::try_convert_from(&[i64], ctx, false) (rq/convert.rs:194-230): the canonical residue of every signed word
   std::vector<u64> res((size_t)Lmax * N);
@@ -1425,58 +1402,18 @@ int fhe_b200_secret_key_create(const fhe_b200_params* p, const int64_t* coeffs, 
       res[(size_t)j * N + i] = (coeffs[i] < 0 && r) ? q - r : r;
     }
   }
-  sk->s = sk->to_dev(res);
+  FHE_CUDA(cudaMemcpy(sk->s.d, res.data(), res.size() * sizeof(u64), cudaMemcpyHostToDevice));
   volatile u64* wipe = res.data();   // erase the host copy (volatile: the stores are not elided)
   for (size_t i = 0; i < res.size(); i++) wipe[i] = 0;
   const LevelData& l0 = p->level(0);
-  launch_ntt(sk->s, sk->s, Lmax, l0.ctx_ids, p->d_limbs, p->logn, false, 1, false, nullptr);   // into_ntt
+  launch_ntt(sk->s.d, sk->s.d, Lmax, l0.ctx_ids, p->d_limbs, p->logn, false, 1, false, nullptr);   // into_ntt
   FHE_CUDA(cudaGetLastError());
   FHE_CUDA(cudaStreamSynchronize(nullptr));
-  const std::vector<u64> plain(p->moduli.begin(), p->moduli.begin() + plaintext_moduli_count(p));
-  const RnsContextH to(plain);
-  sk->levels.resize(Lmax);
-  for (u32 lv = 0; lv < Lmax; lv++) {
-    const u32 L = Lmax - lv;
-    const std::vector<u64> ctx(p->moduli.begin(), p->moduli.begin() + L);
-    const RnsContextH from(ctx);
-    fhe_b200_secret_key::Level& d = sk->levels[lv];
-    d.scaler.h = make_scaler_tables(from, to, p->t, from.product);   // parameters.rs:638-643
-    upload_scaler_tables(d.scaler, plain, [&](const auto& v) { return sk->to_dev(v); },
-                         [&](u64 q) { return p->prime_index(q); });
-    std::vector<u64> garner((size_t)L * L, 0);
-    for (u32 i = 0; i < L; i++)
-      for (u32 j = 0; j < i; j++)
-        if (!invmod_h(ctx[j] % ctx[i], ctx[i], &garner[(size_t)i * L + j]))
-          throw FheError(FHE_B200_INVALID_MODULUS, "NonCoprimeModuli");
-    d.garner = sk->to_dev(garner);
-    std::vector<u64> qw;
-    const BigUint& Q = from.product;
-    for (size_t k = 0; k < Q.w.size(); k += 2)
-      qw.push_back((u64)Q.w[k] | (k + 1 < Q.w.size() ? (u64)Q.w[k + 1] << 32 : 0));
-    d.W = (u32)qw.size();
-    d.q_words = sk->to_dev(qw);
-  }
-  params_retain(p);
-  cleanup.k = nullptr;
   *out = sk.release();
   API_END
 }
 
 int fhe_b200_secret_key_free(fhe_b200_secret_key* sk) {
-  if (!sk) return FHE_B200_OK;
-  {
-    ScopedDevice g(sk->par->device);
-    // SecretKey's Zeroize (secret_key.rs:28-40): erase the words of s before the memory is released.  Work that reads
-    // s may still be queued on streams that do not order against the legacy stream the memset runs on (the chunk
-    // runner's side streams, a caller's non-blocking stream): wait for the device first, as cudaFree would, so that
-    // releasing the key right after an enqueue-only call is as safe as releasing any other handle.
-    cudaDeviceSynchronize();
-    if (sk->s) cudaMemset(sk->s, 0, ((size_t)sk->par->Lmax * sk->par->N) * sizeof(u64));
-    cudaDeviceSynchronize();
-    for (void* d : sk->d_allocs) cudaFree(d);
-    cudaGetLastError();
-  }
-  params_release(sk->par);
   delete sk;
   return FHE_B200_OK;
 }
@@ -1499,12 +1436,12 @@ static void decrypt_range(const fhe_b200_secret_key* sk, const fhe_b200_batch* c
   const u32 L = lv.L, logn = par->logn;
   const size_t rows = (size_t)n * L;
   u64* ph = ph_ntt ? ph_ntt : ws.secret_words(rows << logn);
-  launch_phase(ct->d + (((size_t)c0 * ct->parts * L) << logn), sk->s, ph, n, ct->parts, lv.ctx_ids, par->d_limbs, logn,
-               st);
+  launch_phase(ct->d + (((size_t)c0 * ct->parts * L) << logn), sk->s.d, ph, n, ct->parts, lv.ctx_ids, par->d_limbs,
+               logn, st);
   u64* pb = ph_ntt ? ws.secret_words(rows << logn) : ph;
   launch_ntt(ph, pb, (u32)rows, lv.ctx_ids, par->d_limbs, logn, true, 1, false, st);
   // only output row 0 (q_0): the reference keeps v[..degree], and every output limb of the scaler is independent
-  launch_scale(sk->levels[ct->level].scaler.dev, par->d_limbs, pb, w, nullptr, n, 1, 0, 1, 0, logn, st);
+  launch_scale(lv.plain.dev, par->d_limbs, pb, w, nullptr, n, 1, 0, 1, 0, logn, st);
   const LimbDev& q0 = par->h_limbs[0];
   launch_decrypt_epilogue(w, (size_t)n << logn, PlainMod{q0.p, q0.bhi, q0.blo}, par->t_mod, st);
 }
@@ -1521,16 +1458,14 @@ int fhe_b200_decrypt(const fhe_b200_secret_key* sk, const fhe_b200_batch* ct, fh
   DeviceGuard g(par);
   const LevelData& lv = par->level(ct->level);
   const u32 L = lv.L, logn = par->logn;
-  u64 qmin = ~0ull;
-  for (u32 j = 0; j < L; j++) qmin = std::min(qmin, par->moduli[j]);
-  const bool reduce = par->t_mod.t > 4 * qmin - 1;   // the lifted words are below t
   ChunkRunner chunks(par, ct->count, (cudaStream_t)stream);
   chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
     Workspace ws(par, st);
     u64* w = ws.secret_words((size_t)n << logn);
     decrypt_range(sk, ct, c0, n, w, nullptr, ws, st);
     // Poly::try_convert_from(w, ctx).into_ntt(): every limb of plaintext k transforms row k of w
-    launch_ntt(w, out->d + ((size_t)c0 * L << logn), n * L, lv.ctx_ids, par->d_limbs, logn, false, L, reduce, st);
+    launch_ntt(w, out->d + ((size_t)c0 * L << logn), n * L, lv.ctx_ids, par->d_limbs, logn, false, L, lv.lift_reduce,
+               st);
   });
   FHE_CUDA(cudaGetLastError());
   out->repr = FHE_B200_NTT;
@@ -1546,7 +1481,6 @@ int fhe_b200_measure_noise(const fhe_b200_secret_key* sk, const fhe_b200_batch* 
   REQUIRE(par->t_mod.t < par->moduli[0], FHE_B200_UNSUPPORTED, "to_poly needs t below the first ciphertext modulus");
   DeviceGuard g(par);
   const LevelData& lv = par->level(ct->level);
-  const fhe_b200_secret_key::Level& kl = sk->levels[ct->level];
   const u32 L = lv.L, logn = par->logn;
   cudaStream_t user = (cudaStream_t)stream;
   Workspace out_ws(par, user);   // the per-ciphertext maxima, filled by the chunks' atomics
@@ -1565,7 +1499,7 @@ int fhe_b200_measure_noise(const fhe_b200_secret_key* sk, const fhe_b200_batch* 
       to_poly_from_coefficients(par, lv, w, n, m, st);
       launch_add_scaled(ph, m, n, 1, n, lv.d_delta, lv.d_delta_s, true, lv.ctx_ids, par->d_limbs, logn, st);
       launch_ntt(ph, ph, n * L, lv.ctx_ids, par->d_limbs, logn, true, 1, false, st);
-      launch_noise(ph, noise + c0, n, L, kl.garner, kl.q_words, kl.W, par->d_limbs, logn, st);
+      launch_noise(ph, noise + c0, n, L, lv.garner, lv.q_words, lv.W, par->d_limbs, logn, st);
     });
   }
   FHE_CUDA(cudaMemcpyAsync(noise_bits, noise, ct->count * sizeof(u32), cudaMemcpyDefault, user));
@@ -1676,7 +1610,7 @@ int fhe_b200_encrypt_sk(const fhe_b200_secret_key* sk, const fhe_b200_batch* pts
     launch_cbd(e, n, c0, 1, 1, variance, K, lv.ctx_ids, par->d_limbs, logn, st);
     launch_ntt(e, e, n * L, lv.ctx_ids, par->d_limbs, logn, false, 1, false, st);
     u64* dst = out->d + (((size_t)c0 * 2 * L) << logn);
-    launch_encrypt_sk(sk->s, e, dst, n, c0, K, lv.ctx_ids, par->d_limbs, logn, st);
+    launch_encrypt_sk(sk->s.d, e, dst, n, c0, K, lv.ctx_ids, par->d_limbs, logn, st);
     if (pts) add_to_poly(par, lv, pts, c0, n, dst, ws, st);
   });
   FHE_CUDA(cudaGetLastError());
@@ -1769,22 +1703,8 @@ static void generate_keys(const fhe_b200_secret_key* sk, u32 n_keys, u32 ct_leve
     G.g[j] = v;
     G.g_s[j] = ModulusH(q).shoup(v);
   }
-  struct Made {   // the handles made so far, freed again unless the call succeeds
-    std::vector<fhe_b200_ksk*> k;
-    ~Made() { for (fhe_b200_ksk* h : k) fhe_b200_ksk_free(h); }
-  } made;
-  const size_t bytes = (size_t)n_dig * Lk * row * sizeof(u64);
-  for (u32 k = 0; k < n_keys; k++) {
-    DevPtr g0, g1;
-    FHE_CUDA(cudaMalloc(&g0.p, bytes));
-    FHE_CUDA(cudaMalloc(&g1.p, bytes));
-    fhe_b200_ksk* h = new fhe_b200_ksk();
-    h->par = params_retain(par); h->ct_level = ct_level; h->ksk_level = key_level; h->n_dig = n_dig; h->Lk = Lk;
-    h->log_base = log_base;
-    h->k0 = (u64*)g0.release();
-    h->k1 = (u64*)g1.release();
-    made.k.push_back(h);
-  }
+  std::vector<std::unique_ptr<fhe_b200_ksk>> made;   // freed again unless the call succeeds
+  for (u32 k = 0; k < n_keys; k++) made.push_back(make_ksk(par, ct_level, key_level, n_dig, Lk, log_base));
   ChunkRunner chunks(par, n_keys * n_dig, user, std::max(1u, chunk_size() / Lk));
   chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
     Workspace ws(par, st);
@@ -1795,15 +1715,14 @@ static void generate_keys(const fhe_b200_secret_key* sk, u32 n_keys, u32 ct_leve
     for (u32 it = c0; it < c0 + n;) {
       const u32 key = it / n_dig, d0 = it % n_dig, nd = std::min(n_dig - d0, c0 + n - it);
       x_of(key, x, st);
-      const fhe_b200_ksk* h = made.k[key];
-      launch_ksk_gen(sk->s, e + (size_t)(it - c0) * Lk * row, x, h->k0, h->k1, key, d0, nd, n_dig, G, K, kl.ctx_ids,
+      const fhe_b200_ksk* h = made[key].get();
+      launch_ksk_gen(sk->s.d, e + (size_t)(it - c0) * Lk * row, x, h->k0, h->k1, key, d0, nd, n_dig, G, K, kl.ctx_ids,
                      par->d_limbs, logn, st);
       it += nd;
     }
   });
   FHE_CUDA(cudaGetLastError());
-  for (u32 k = 0; k < n_keys; k++) out[k] = made.k[k];
-  made.k.clear();
+  for (u32 k = 0; k < n_keys; k++) out[k] = made[k].release();
 }
 
 // x = a * s on the limbs of the level (a: [L][N] NTT words, s the secret key's rows)
@@ -1811,7 +1730,7 @@ static void times_s(const fhe_b200_secret_key* sk, const LevelData& lv, const u6
   const fhe_b200_params* par = sk->par;
   const size_t words = (size_t)lv.L << par->logn;
   FHE_CUDA(cudaMemcpyAsync(x, a, words * sizeof(u64), cudaMemcpyDeviceToDevice, st));
-  launch_mul_plain(x, sk->s, 1, 1, 1, lv.ctx_ids, par->d_limbs, par->logn, st, 0);
+  launch_mul_plain(x, sk->s.d, 1, 1, 1, lv.ctx_ids, par->d_limbs, par->logn, st, 0);
 }
 
 int fhe_b200_relin_key_generate(const fhe_b200_secret_key* sk, uint32_t ciphertext_level, uint32_t key_level,
@@ -1827,7 +1746,7 @@ int fhe_b200_relin_key_generate(const fhe_b200_secret_key* sk, uint32_t cipherte
   const LevelData& cl = par->level(ciphertext_level);
   // x = s * s (relinearization_key.rs:56-60)
   generate_keys(sk, 1, ciphertext_level, key_level, variance, seed_words(seed),
-                [&](u32, u64* x, cudaStream_t st) { times_s(sk, cl, sk->s, x, st); }, out, (cudaStream_t)stream);
+                [&](u32, u64* x, cudaStream_t st) { times_s(sk, cl, sk->s.d, x, st); }, out, (cudaStream_t)stream);
   API_END
 }
 
@@ -1850,7 +1769,7 @@ int fhe_b200_galois_keys_generate(const fhe_b200_secret_key* sk, const uint32_t*
   for (u32 k = 0; k < n_keys; k++) perms[k] = par->perm(exps[k]);
   // x = s substituted by the exponent (galois_key.rs:40-46), a gather of the NTT words
   generate_keys(sk, n_keys, ciphertext_level, key_level, variance, seed_words(seed),
-                [&](u32 k, u64* x, cudaStream_t st) { launch_gather(sk->s, x, cl.L, perms[k], par->logn, st); }, out,
+                [&](u32 k, u64* x, cudaStream_t st) { launch_gather(sk->s.d, x, cl.L, perms[k], par->logn, st); }, out,
                 (cudaStream_t)stream);
   API_END
 }
@@ -1965,7 +1884,7 @@ int fhe_b200_pk_share(const fhe_b200_secret_key* sk, const fhe_b200_batch* crp, 
     launch_cbd(e, n, c0, 8, 1, variance, K, lv.ctx_ids, par->d_limbs, logn, st);
     launch_ntt(e, e, n * L, lv.ctx_ids, par->d_limbs, logn, false, 1, false, st);
     const size_t off = ((size_t)c0 * L) << logn;
-    launch_mbfv_share(SHARE_PK, sk->s, nullptr, crp->d + off, nullptr, e, out->d + off, n, lv.ctx_ids, par->d_limbs,
+    launch_mbfv_share(SHARE_PK, sk->s.d, nullptr, crp->d + off, nullptr, e, out->d + off, n, lv.ctx_ids, par->d_limbs,
                       logn, st);
   });
   FHE_CUDA(cudaGetLastError());
@@ -2034,7 +1953,7 @@ int fhe_b200_sks_share(const fhe_b200_secret_key* sk_in, const fhe_b200_secret_k
     u64* e = ws.secret_words(((size_t)n * L) << logn);
     launch_cbd(e, n, c0, 14, 1, variance, K, lv.ctx_ids, par->d_limbs, logn, st);
     launch_ntt(e, e, n * L, lv.ctx_ids, par->d_limbs, logn, false, 1, false, st);
-    launch_mbfv_share(SHARE_SKS, sk_in->s, sk_out ? sk_out->s : nullptr, ct->d + ((2 * (size_t)c0 * L) << logn),
+    launch_mbfv_share(SHARE_SKS, sk_in->s.d, sk_out ? sk_out->s.d : nullptr, ct->d + ((2 * (size_t)c0 * L) << logn),
                       nullptr, e, out->d + (((size_t)c0 * L) << logn), n, lv.ctx_ids, par->d_limbs, logn, st);
   });
   FHE_CUDA(cudaGetLastError());
@@ -2092,7 +2011,7 @@ int fhe_b200_pks_share(const fhe_b200_secret_key* sk, const fhe_b200_batch* pk, 
     launch_cbd(uee, n, c0, 15, 3, variance, K, lv.ctx_ids, par->d_limbs, logn, st);
     launch_ntt(uee, uee, n * 3 * L, lv.ctx_ids, par->d_limbs, logn, false, 1, false, st);
     const size_t off = ((2 * (size_t)c0 * L) << logn);
-    launch_mbfv_share(SHARE_PKS, sk->s, nullptr, ct->d + off, c, uee, out->d + off, n, lv.ctx_ids, par->d_limbs, logn,
+    launch_mbfv_share(SHARE_PKS, sk->s.d, nullptr, ct->d + off, c, uee, out->d + off, n, lv.ctx_ids, par->d_limbs, logn,
                       st);
   });
   FHE_CUDA(cudaGetLastError());
@@ -2126,11 +2045,14 @@ int fhe_b200_pks_aggregate(const fhe_b200_batch* ct, const fhe_b200_batch* const
 // RelinKeyGenerator (relin_key_gen.rs:36-96): the party's secret key, the level-0 CRPs a_i (one per level-0 limb,
 // borrowed as in the reference) and u on the device, erased when the generator is freed.
 struct fhe_b200_rkg {
-  const fhe_b200_params* par;   // a reference of its own: freeing the generator never reads sk
+  ParamsRef par;   // a reference of its own: freeing the generator never reads sk
   const fhe_b200_secret_key* sk;
   const fhe_b200_batch* crp;
   u32 variance;
-  u64* u;   // [Lmax][N] NTT
+  SecretBuffer u;   // [Lmax][N] NTT
+  fhe_b200_rkg(const fhe_b200_secret_key* k, const fhe_b200_batch* c, u32 v)
+      : par(static_cast<const fhe_b200_params*>(k->par)), sk(k), crp(c), variance(v),
+        u(par->device, (size_t)par->Lmax << par->logn) {}
 };
 
 int fhe_b200_rkg_create(const fhe_b200_secret_key* sk, const fhe_b200_batch* crp, uint32_t variance,
@@ -2149,34 +2071,16 @@ int fhe_b200_rkg_create(const fhe_b200_secret_key* sk, const fhe_b200_batch* crp
   const EncSeed K = seed_words(seed);
   DeviceGuard g(par);
   const LevelData& lv = par->level(0);
-  const size_t words = (size_t)lv.L << par->logn;
-  DevPtr du;
-  FHE_CUDA(cudaMalloc(&du.p, words * sizeof(u64)));
+  std::unique_ptr<fhe_b200_rkg> r(new fhe_b200_rkg(sk, crp, variance));
   cudaStream_t st = (cudaStream_t)stream;
-  launch_cbd((u64*)du.p, 1, 0, 9, 1, variance, K, lv.ctx_ids, par->d_limbs, par->logn, st);   // u: role 9
-  launch_ntt((u64*)du.p, (u64*)du.p, lv.L, lv.ctx_ids, par->d_limbs, par->logn, false, 1, false, st);
+  launch_cbd(r->u.d, 1, 0, 9, 1, variance, K, lv.ctx_ids, par->d_limbs, par->logn, st);   // u: role 9
+  launch_ntt(r->u.d, r->u.d, lv.L, lv.ctx_ids, par->d_limbs, par->logn, false, 1, false, st);
   FHE_CUDA(cudaGetLastError());
-  std::unique_ptr<fhe_b200_rkg> r(new fhe_b200_rkg());
-  r->par = par; r->sk = sk; r->crp = crp; r->variance = variance;
-  r->u = (u64*)du.release();
-  params_retain(par);
   *out = r.release();
   API_END
 }
 
 int fhe_b200_rkg_free(fhe_b200_rkg* r) {
-  if (!r) return FHE_B200_OK;
-  const fhe_b200_params* par = r->par;
-  {
-    ScopedDevice g(par->device);
-    // u is erased as SecretKey's s is (fhe_b200_secret_key_free): wait for work that may still read it, then zero it
-    cudaDeviceSynchronize();
-    cudaMemset(r->u, 0, ((size_t)par->Lmax << par->logn) * sizeof(u64));
-    cudaDeviceSynchronize();
-    cudaFree(r->u);
-    cudaGetLastError();
-  }
-  params_release(par);
   delete r;
   return FHE_B200_OK;
 }
@@ -2200,8 +2104,8 @@ static void rkg_round(const fhe_b200_rkg* r, MbfvShare kind, const fhe_b200_batc
     launch_cbd(e, n, c0, role0, 2, r->variance, K, lv.ctx_ids, par->d_limbs, logn, st, L);
     launch_ntt(e, e, n * 2 * L, lv.ctx_ids, par->d_limbs, logn, false, 1, false, st);
     const size_t off = ((size_t)c0 * L) << logn;
-    launch_mbfv_share(kind, r->sk->s, nullptr, x->d + off, y ? y->d + off : nullptr, e, h0->d + off, n, lv.ctx_ids,
-                      par->d_limbs, logn, st, r->u, h1->d + off, c0);
+    launch_mbfv_share(kind, r->sk->s.d, nullptr, x->d + off, y ? y->d + off : nullptr, e, h0->d + off, n, lv.ctx_ids,
+                      par->d_limbs, logn, st, r->u.d, h1->d + off, c0);
   });
   FHE_CUDA(cudaGetLastError());
   h0->repr = h1->repr = FHE_B200_NTT;
@@ -2246,13 +2150,11 @@ int fhe_b200_rkg_aggregate(const fhe_b200_batch* const* h0s, const fhe_b200_batc
   DeviceGuard g(par);
   const LevelData& lv = par->level(0);
   const size_t words = (size_t)L << logn, row = (size_t)1 << logn;
-  DevPtr g0, g1;
-  FHE_CUDA(cudaMalloc(&g0.p, L * words * sizeof(u64)));
-  FHE_CUDA(cudaMalloc(&g1.p, L * words * sizeof(u64)));
+  std::unique_ptr<fhe_b200_ksk> k = make_ksk(par, 0, 0, L, L, 0);
   std::vector<const fhe_b200_batch*> all(h0s, h0s + n);
   all.insert(all.end(), h1s, h1s + n);
   const fhe_b200_batch* r1[] = {r1_h1};
-  u64 *k0 = (u64*)g0.p, *k1 = (u64*)g1.p;
+  u64 *k0 = k->k0, *k1 = k->k1;
   // digit i of the key: c0_i = sum h0'_i + sum h1'_i, c1_i = r1_h1_i, written straight into the key's device layout
   // [limb j][digit i][N] (relin_key_gen.rs:299-350): item i of the sum starts at digit i's row, rows L * N apart
   ChunkRunner chunks(par, L, (cudaStream_t)stream, std::max(1u, chunk_size() / L));
@@ -2266,31 +2168,8 @@ int fhe_b200_rkg_aggregate(const fhe_b200_batch* const* h0s, const fhe_b200_batc
                       L * row);
   });
   FHE_CUDA(cudaGetLastError());
-  std::unique_ptr<fhe_b200_ksk> k(new fhe_b200_ksk());
-  k->par = par; k->ct_level = 0; k->ksk_level = 0; k->n_dig = L; k->Lk = L; k->log_base = 0;
-  k->k0 = (u64*)g0.release();
-  k->k1 = (u64*)g1.release();
-  params_retain(par);
   *out = k.release();
   API_END
-}
-
-// cipher_plain_context.scaler of `level` (parameters.rs:638-643) on the encoder, built on first use
-static const ScalerDev& plain_scaler(const fhe_b200_encoder* ce, u32 level) {
-  fhe_b200_encoder* e = const_cast<fhe_b200_encoder*>(ce);
-  const fhe_b200_params* p = e->par;
-  std::lock_guard<std::mutex> lock(e->mu);
-  auto it = e->plain_scalers.find(level);
-  if (it != e->plain_scalers.end()) return it->second->dev;
-  const std::vector<u64> plain(p->moduli.begin(), p->moduli.begin() + plaintext_moduli_count(p));
-  const std::vector<u64> ctx(p->moduli.begin(), p->moduli.begin() + (p->Lmax - level));
-  const RnsContextH from(ctx), to(plain);
-  std::unique_ptr<ScalerData> s(new ScalerData());
-  s->h = make_scaler_tables(from, to, p->t, from.product);
-  upload_scaler_tables(*s, plain, [&](const auto& v) { return e->to_dev(v); }, [&](u64 q) { return p->prime_index(q); });
-  const ScalerDev& d = s->dev;
-  e->plain_scalers[level] = std::move(s);
-  return d;
 }
 
 int fhe_b200_decryption_aggregate(const fhe_b200_encoder* e, const fhe_b200_batch* ct,
@@ -2306,13 +2185,9 @@ int fhe_b200_decryption_aggregate(const fhe_b200_encoder* e, const fhe_b200_batc
   REQUIRE(par->t_small && par->t_mod.t < par->moduli[0], FHE_B200_UNSUPPORTED,
           "Plaintext::from_shares needs t below the first ciphertext modulus");
   const LevelData& lv = par->level(ct->level);
-  const ScalerDev& S = plain_scaler(e, ct->level);
   const u32 L = lv.L, logn = par->logn;
   const size_t words = (size_t)L << logn;
-  u64 qmin = ~0ull;
-  for (u32 j = 0; j < L; j++) qmin = std::min(qmin, par->moduli[j]);
-  const bool reduce = par->t_mod.t > 4 * qmin - 1;   // the lifted words are below t
-  const bool q0_context = plaintext_moduli_count(par) == 1;
+  const bool q0_context = par->plaintext_moduli_count() == 1;
   ChunkRunner chunks(par, ct->count, (cudaStream_t)stream);
   chunks.run([&](u32 c0, u32 m, cudaStream_t st) {
     Workspace ws(par, st);
@@ -2322,13 +2197,14 @@ int fhe_b200_decryption_aggregate(const fhe_b200_encoder* e, const fhe_b200_batc
     sum_shares(shares, n, 0, words, ct->d + 2 * (size_t)c0 * words, 2 * words, c, words, c0, m, lv, st);
     launch_ntt(c, c, m * L, lv.ctx_ids, par->d_limbs, logn, true, 1, false, st);
     u64* w = ws.secret_words((size_t)m << logn);
-    launch_scale(S, par->d_limbs, c, w, nullptr, m, 1, 0, 1, 0, logn, st);
+    launch_scale(lv.plain.dev, par->d_limbs, c, w, nullptr, m, 1, 0, 1, 0, logn, st);
     // w = ((v + t) mod Q_p) mod t over the plaintext context Q_p (:164-173).  With one plaintext modulus Q_p = q_0 and
     // this is try_decrypt's lift; with more, (v + t) mod Q_p = v + t and w = v mod t.
     const LimbDev& q0 = par->h_limbs[0];
     if (q0_context) launch_decrypt_epilogue(w, (size_t)m << logn, PlainMod{q0.p, q0.bhi, q0.blo}, par->t_mod, st);
     else launch_from_shares_epilogue(w, (size_t)m << logn, q0.p, par->t_mod, st);
-    launch_ntt(w, pts_out->d + (size_t)c0 * words, m * L, lv.ctx_ids, par->d_limbs, logn, false, L, reduce, st);
+    launch_ntt(w, pts_out->d + (size_t)c0 * words, m * L, lv.ctx_ids, par->d_limbs, logn, false, L, lv.lift_reduce,
+               st);
   });
   FHE_CUDA(cudaGetLastError());
   pts_out->repr = FHE_B200_NTT;
@@ -2463,12 +2339,7 @@ int fhe_b200_multiplicator_create(const fhe_b200_params* p, uint32_t level, cons
   REQUIRE(n_basis <= (u32)kMaxPos, FHE_B200_UNSUPPORTED, "too many limbs");
   const LevelData& lv = p->level(level);   // context_at_level: InvalidLevel when out of range
   DeviceGuard g(p);
-  std::unique_ptr<fhe_b200_multiplicator> m(new fhe_b200_multiplicator());
-  struct Cleanup {   // frees the device tables if construction throws
-    fhe_b200_multiplicator* m;
-    ~Cleanup() { if (m) { for (void* d : m->d_allocs) cudaFree(d); cudaGetLastError(); } }
-  } cleanup{m.get()};
-  m->par = p;
+  std::unique_ptr<fhe_b200_multiplicator> m(new fhe_b200_multiplicator(p));
   m->level = level;
   m->L = lv.L;
   m->K = n_basis;
@@ -2487,7 +2358,7 @@ int fhe_b200_multiplicator_create(const fhe_b200_params* p, uint32_t level, cons
   m->mul_ids.limbs_per_poly = n_basis;
   for (u32 i = 0; i < n_basis; i++) {
     const u64 q = extended_basis[i];
-    int idx = m->prime_index(q);
+    int idx = prime_index(m->plan_primes, q);
     if (idx >= 0 && psi && psi[i] != p->psi[(size_t)idx] && (size_t)idx < p->primes.size())
       throw FheError(FHE_B200_INVALID_ARGUMENT, "psi differs from the parameter set's root for " + std::to_string(q));
     if (idx < 0) {
@@ -2495,11 +2366,11 @@ int fhe_b200_multiplicator_create(const fhe_b200_params* p, uint32_t level, cons
       NttTablesH t = make_ntt_tables(q, p->N, r);
       idx = (int)m->plan_primes.size();
       m->plan_primes.push_back(q);
-      m->h_limbs.push_back(make_limb_dev(q, t, [&](const std::vector<ulonglong2>& v) { return m->to_dev(v); }));
+      m->h_limbs.push_back(make_limb_dev(q, t, m->uploads));
     }
     m->mul_ids.ids[i] = (unsigned short)idx;
   }
-  m->d_limbs = m->to_dev(m->h_limbs);
+  m->d_limbs = m->uploads.put(m->h_limbs);
   std::vector<u64> base(p->moduli.begin(), p->moduli.begin() + lv.L);
   RnsContextH from(base), to(m->mul_moduli);
   auto factor = [](const uint8_t* b, uint32_t n) { return BigUint::from_le_bytes(b, n); };
@@ -2519,23 +2390,14 @@ int fhe_b200_multiplicator_create(const fhe_b200_params* p, uint32_t level, cons
   m->nc_l = common(m->ext_l, base, m->mul_moduli);
   m->nc_r = common(m->ext_r, base, m->mul_moduli);
   m->nc_d = common(m->down, m->mul_moduli, base);
-  m->upload_scaler(m->ext_l, m->mul_moduli);
-  m->upload_scaler(m->ext_r, m->mul_moduli);
-  m->upload_scaler(m->down, base);
-  params_retain(p);
-  cleanup.m = nullptr;
+  upload_scaler_tables(m->ext_l, m->mul_moduli, m->plan_primes, m->uploads);
+  upload_scaler_tables(m->ext_r, m->mul_moduli, m->plan_primes, m->uploads);
+  upload_scaler_tables(m->down, base, m->plan_primes, m->uploads);
   *out = m.release();
   API_END
 }
 
 int fhe_b200_multiplicator_free(fhe_b200_multiplicator* m) {
-  if (!m) return FHE_B200_OK;
-  if (m->par->device >= 0) {
-    ScopedDevice g(m->par->device);
-    for (void* d : m->d_allocs) cudaFree(d);
-    cudaGetLastError();
-  }
-  params_release(m->par);
   delete m;
   return FHE_B200_OK;
 }
@@ -2777,11 +2639,7 @@ int fhe_b200_scale(const fhe_b200_batch* in, int which, fhe_b200_batch* out, voi
                                cudaMemcpyDeviceToDevice, st));
     u64* x = ws.words((size_t)polys * lv.E * row);
     launch_scale(lv.ext.dev, par->d_limbs, pb, x, nullptr, polys, lv.E, lv.L, lv.E, 0, par->logn, st);
-    RowIds ext_ids;
-    std::memset(&ext_ids, 0, sizeof(ext_ids));
-    ext_ids.limbs_per_poly = lv.E;
-    for (u32 j = 0; j < lv.E; j++) ext_ids.ids[j] = lv.mul_ids.ids[lv.L + j];
-    launch_ntt(x, x, polys * lv.E, ext_ids, par->d_limbs, par->logn, false, 1, false, st);
+    launch_ntt(x, x, polys * lv.E, lv.ext_ids, par->d_limbs, par->logn, false, 1, false, st);
     FHE_CUDA(cudaMemcpy2DAsync(out->d + lv.L * row, lv.K * row * 8, x, lv.E * row * 8, lv.E * row * 8, polys,
                                cudaMemcpyDeviceToDevice, st));
   } else {
@@ -2907,7 +2765,7 @@ int fhe_b200_debug_ntt_tables(const fhe_b200_params* p, uint64_t q, uint64_t* om
                               uint64_t* zetas_inv, uint64_t* zetas_inv_shoup, uint64_t* size_inv) {
   API_BEGIN
   REQUIRE(p, FHE_B200_INVALID_ARGUMENT, "null argument");
-  int i = p->prime_index(q);
+  int i = prime_index(p->primes, q);
   REQUIRE(i >= 0, FHE_B200_INVALID_MODULUS, "prime not in parameter set");
   const NttTablesH& t = p->tables[i];
   auto cp = [](uint64_t* dst, const std::vector<u64>& v) {
