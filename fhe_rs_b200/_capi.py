@@ -104,6 +104,9 @@ SYMBOLS = {
     "fhe_b200_batch_packed_bytes": (_i, [_vp, C.POINTER(C.c_size_t)]),
     "fhe_b200_batch_pack": (_i, [_vp, _u32, _u32, _vp, _vp]),
     "fhe_b200_batch_unpack": (_i, [_vp, _u32, _u32, _vp, _vp]),
+    "fhe_b200_transcode": (_i, [_vp, _vp, _u32, C.c_size_t, C.c_size_t, _u32, _vp, _u32, C.c_size_t, C.c_size_t,
+                                _u32, _u32, _vp]),
+    "fhe_b200_fold": (_i, [_vp, _u32, _u32, _vp, _vp]),
     "fhe_b200_sync": (_i, [_vp]),
     "fhe_b200_launch_count": (_u64, []),
     "fhe_b200_debug_scaler_tables": (_i, [_vp, _u32, _i, _pu32, _pu32, _pu32] + [_vp] * 8),

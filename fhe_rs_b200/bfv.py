@@ -23,7 +23,8 @@ from .wire import WireError
 
 __all__ = ["BfvParameters", "BfvParametersBuilder", "Ciphertext", "KeySwitchingKey", "RelinearizationKey", "RGSWCiphertext",
            "GaloisKey", "EvaluationKey", "Multiplicator", "ScalingFactor", "dot_product_scalar", "FheError", "WireError", "NTT", "POWER_BASIS",
-           "Encoding", "Plaintext", "PlaintextVec", "SecretKey", "PublicKey", "EvaluationKeyBuilder"]
+           "Encoding", "Plaintext", "PlaintextVec", "SecretKey", "PublicKey", "EvaluationKeyBuilder",
+           "transcode_bidirectional", "transcode_to_bytes", "transcode_from_bytes"]
 
 
 def _release(free_name: str, handle) -> None:
@@ -487,6 +488,20 @@ class Ciphertext:
         out = self._like()
         check(_capi.lib().fhe_b200_substitute(self._h, exponent, out._h, self.stream))
         return out
+
+    def fold(self, in_bits: int, out_bits: int, level: int) -> "PlaintextVec":
+        """The reply fold of the SealPIR server (examples/sealpir.rs:176-200) of every ciphertext: the stored words of
+        each part transcoded from in_bits to out_bits, concatenated over the parts and encoded as
+        PlaintextVec::try_encode(values, Encoding::poly_at_level(level)) (fhe_b200_fold).  Plaintext i of ciphertext
+        j is entry i * count + j of the result, the operand dot_product_scalar(selectors, pts, n_terms=count) takes."""
+        n = self.par.degree()
+        per_ct = 1
+        if 1 <= in_bits <= 64 and 1 <= out_bits <= 64:     # (otherwise fhe_b200_fold refuses the widths)
+            e = -(-self.limbs * n * in_bits // out_bits)
+            per_ct = -(-len(self) * e // n)
+        out = Ciphertext(self.par, per_ct * self.count, 1, level, NTT, self.stream)
+        check(_capi.lib().fhe_b200_fold(self._h, in_bits, out_bits, out._h, self.stream))
+        return PlaintextVec(out, Encoding.poly_at_level(level))
 
     def scale(self, which: int) -> "Ciphertext":
         """Poly::scale with the level's extender (0) / down scaler (1) (rq/mod.rs:669, rq/scaler.rs:55)."""
@@ -984,9 +999,10 @@ class GaloisKey:
         return wire.encode_galois_key(self.ksk.to_bytes(), self.exponent)
 
     @staticmethod
-    def from_bytes(par: BfvParameters, data: bytes) -> "GaloisKey":  # galois_key.rs:155-173
+    def from_bytes(par: BfvParameters, data: bytes, seeded_c1: Optional[np.ndarray] = None) -> "GaloisKey":
+        """galois_key.rs:155-173; `seeded_c1` as for KeySwitchingKey.from_bytes"""
         msg, exponent = wire.decode_galois_key(data)
-        ksk = KeySwitchingKey.from_bytes(par, msg)
+        ksk = KeySwitchingKey.from_bytes(par, msg, seeded_c1)
         exponent %= 2 * par.degree()            # SubstitutionExponent::new (rq/mod.rs:99-106)
         if exponent & 1 == 0:
             raise WireError("InvalidSubstitutionExponent", _capi.INVALID_EXPONENT, str(exponent))
@@ -1014,12 +1030,37 @@ def _galois_keys(sk: SecretKey, exponents: Sequence[int], ciphertext_level: int,
 
 
 class EvaluationKey:
-    """The rotation subset of fhe::bfv::EvaluationKey (keys/evaluation_key.rs:110-170):
-    a map Galois exponent -> GaloisKey."""
+    """fhe::bfv::EvaluationKey (keys/evaluation_key.rs:21-310): a map Galois exponent -> GaloisKey, and the levels
+    of the ciphertexts it takes and of its keys (both 0 unless an EvaluationKeyBuilder or a message sets them)."""
 
-    def __init__(self, par: BfvParameters):
+    def __init__(self, par: BfvParameters, ciphertext_level: int = 0, evaluation_key_level: int = 0):
         self.par = par
         self.gk: Dict[int, GaloisKey] = {}
+        self.ciphertext_level, self.evaluation_key_level = ciphertext_level, evaluation_key_level
+
+    def to_bytes(self) -> bytes:
+        """EvaluationKey::to_bytes (evaluation_key.rs:293-297, :494-505), the Galois keys in ascending exponent order"""
+        return wire.encode_evaluation_key([self.gk[e].to_bytes() for e in sorted(self.gk)], self.ciphertext_level,
+                                          self.evaluation_key_level)
+
+    @staticmethod
+    def from_bytes(par: BfvParameters, data: bytes,
+                   seeded_c1: Optional[Dict[int, np.ndarray]] = None) -> "EvaluationKey":
+        """EvaluationKey::from_bytes (evaluation_key.rs:299-310, :507-550): every key through GaloisKey.from_bytes, a
+        key at other levels than the message's or a ciphertext level beyond the parameters' -> InvalidLevel, and a
+        repeated exponent keeps the later key.  `seeded_c1`: exponent -> the host-expanded c1 of a compact key."""
+        msgs, ct_level, ek_level = wire.decode_evaluation_key(data)
+        ek = EvaluationKey(par, ct_level, ek_level)
+        for m in msgs:
+            exponent = wire.decode_galois_key(m)[1] % (2 * par.degree())
+            gk = GaloisKey.from_bytes(par, m, (seeded_c1 or {}).get(exponent))
+            for got, want in ((gk.ksk.ciphertext_level, ct_level), (gk.ksk.ksk_level, ek_level)):
+                if got != want:
+                    raise WireError("InvalidLevel", _capi.INVALID_LEVEL, "level %d, expected %d" % (got, want))
+            ek.add_galois_key(gk)
+        if ct_level > par.max_level():
+            raise WireError("InvalidLevel", _capi.INVALID_LEVEL, "level %d, max %d" % (ct_level, par.max_level()))
+        return ek
 
     def add_galois_key(self, gk: GaloisKey):
         self.gk[gk.exponent % (2 * self.par.degree())] = gk
@@ -1158,7 +1199,7 @@ class EvaluationKeyBuilder:
     def build(self, seed: Optional[bytes] = None) -> EvaluationKey:
         """EvaluationKeyBuilder::build (evaluation_key.rs:429-491): every Galois key in one device call, the exponents
         ascending, so a seed fixes the key of each exponent"""
-        ek = EvaluationKey(self.sk.par)
+        ek = EvaluationKey(self.sk.par, self.ciphertext_level, self.evaluation_key_level)
         exps = self.exponents()
         if exps:
             for gk in _galois_keys(self.sk, exps, self.ciphertext_level, self.evaluation_key_level, seed):
@@ -1189,6 +1230,89 @@ def dot_product_scalar(cts: "Ciphertext", pts, n_terms: Optional[int] = None) ->
     out = Ciphertext(cts.par, max(groups, 1), len(cts), cts.level, NTT, cts.stream)
     check(_capi.lib().fhe_b200_dot_product_scalar(cts._h, pts._h, n, out._h, cts.stream))
     return out
+
+
+def _rows(a, elem: int, what: str, output: bool = False):
+    """(pointer, rows, length, row stride in elements, keep-alive, is_2d) of a 1-D or 2-D array of `elem`-byte integers:
+    a numpy array (or, as input, a sequence or bytes) in pageable memory, or a torch tensor (pinned host or CUDA).  The
+    library reads and writes rows of contiguous elements at a row stride of at least the row length.  An input laid out
+    otherwise (a strided view, broadcast or overlapping rows) is copied first; an output laid out otherwise is refused,
+    because the values would land in a copy the caller never sees."""
+    def bad(why):
+        return FheError(_capi.INVALID_ARGUMENT, "%s: expected a 1-D or 2-D array of %d-byte integers%s" % (why, elem, what))
+
+    def in_place(ndim, shape, strides):   # strides in elements
+        if ndim == 1:
+            return shape[0] <= 1 or strides[0] == 1
+        return shape[0] * shape[1] == 0 or ((shape[1] <= 1 or strides[1] == 1) and (shape[0] <= 1 or strides[0] >= shape[1]))
+
+    if hasattr(a, "data_ptr") and hasattr(a, "is_cuda"):   # torch.Tensor
+        if a.element_size() != elem or a.is_floating_point() or a.is_complex() or a.dim() not in (1, 2):
+            raise bad("wrong element type or rank")
+        if not in_place(a.dim(), tuple(a.shape), tuple(a.stride())):
+            if output:
+                raise bad("the output's rows are not contiguous at a stride of at least their length")
+            a = a.contiguous()
+        rows, n = (1, a.shape[0]) if a.dim() == 1 else tuple(a.shape)
+        stride = a.stride(0) if a.dim() == 2 and rows > 1 else n
+        return a.data_ptr(), rows, n, stride, a, a.dim() == 2
+    if output and not isinstance(a, np.ndarray):
+        raise bad("the output must be a numpy array or a torch tensor")
+    if isinstance(a, (bytes, bytearray, memoryview)):
+        a = np.frombuffer(a, np.uint8)
+    a = np.asarray(a)
+    if a.size == 0 and a.dtype.kind not in "iu" and not output:
+        a = a.astype(np.uint8 if elem == 1 else np.uint64)
+    if a.dtype.kind not in "iu" or a.dtype.itemsize != elem or a.ndim not in (1, 2):
+        raise bad("wrong element type or rank")
+    strides = tuple(x // elem if x % elem == 0 else -1 for x in a.strides)
+    if not in_place(a.ndim, a.shape, strides):
+        if output:
+            raise bad("the output's rows are not contiguous at a stride of at least their length")
+        a = np.ascontiguousarray(a)
+        strides = tuple(x // elem for x in a.strides)
+    if output and not a.flags.writeable:
+        raise bad("the output is read-only")
+    rows, n = (1, a.shape[0]) if a.ndim == 1 else a.shape
+    stride = strides[0] if a.ndim == 2 and rows > 1 else n
+    return a.ctypes.data, rows, n, stride, a, a.ndim == 2
+
+
+def _transcode(par: BfvParameters, a, in_elem: int, in_bits: int, out_elem: int, out_bits: int,
+               out_len: Optional[int], out, stream: int):
+    ptr, rows, n, stride, keep, two_d = _rows(a, in_elem, " (input)")
+    if out_len is None:
+        out_len = -(-n * in_bits // out_bits) if 1 <= in_bits <= 64 and 1 <= out_bits <= 64 else 0
+    if out is None:
+        out = np.empty((rows, out_len) if two_d else out_len, np.uint64 if out_elem == 8 else np.uint8)
+    optr, orows, olen, ostride, okeep, _ = _rows(out, out_elem, " (output)", output=True)
+    if orows != rows or olen != out_len:
+        raise FheError(_capi.INVALID_ARGUMENT, "output must hold %d rows of %d values" % (rows, out_len))
+    check(_capi.lib().fhe_b200_transcode(par._h, ptr if n else None, in_elem, n, stride, in_bits,
+                                         optr if out_len else None, out_elem, out_len, ostride, out_bits, rows, stream))
+    check(_capi.lib().fhe_b200_sync(stream))
+    del keep, okeep
+    return out
+
+
+def transcode_bidirectional(par: BfvParameters, a, input_nbits: int, output_nbits: int, out_len: Optional[int] = None,
+                            out=None, stream: int = 0):
+    """fhe_util::transcode_bidirectional (fhe-util/src/lib.rs:148-187) of every row of `a` (u64 words, 1-D or 2-D
+    with contiguous rows) on the device of `par` (fhe_b200_transcode).  Each row gives its first `out_len` values
+    (default: all ceil(len * input_nbits / output_nbits) of them), zero-padded past the stream.  `out`: an array or
+    tensor (host, pinned or CUDA) of that shape receiving them; otherwise a new uint64 numpy array is returned."""
+    return _transcode(par, a, 8, input_nbits, 8, output_nbits, out_len, out, stream)
+
+
+def transcode_to_bytes(par: BfvParameters, a, nbits: int, out_len: Optional[int] = None, out=None, stream: int = 0):
+    """fhe_util::transcode_to_bytes (lib.rs:68-108) of every row of `a`: uint8 output, as transcode_bidirectional"""
+    return _transcode(par, a, 8, nbits, 1, 8, out_len, out, stream)
+
+
+def transcode_from_bytes(par: BfvParameters, b, nbits: int, out_len: Optional[int] = None, out=None, stream: int = 0):
+    """fhe_util::transcode_from_bytes (lib.rs:110-146) of every row of `b` (bytes, uint8): uint64 output, as
+    transcode_bidirectional"""
+    return _transcode(par, b, 1, 8, 8, nbits, out_len, out, stream)
 
 
 class ScalingFactor:

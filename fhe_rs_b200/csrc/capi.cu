@@ -2729,6 +2729,113 @@ int fhe_b200_batch_unpack(fhe_b200_batch* b, uint32_t first, uint32_t n, const u
   API_END
 }
 
+// ---- bit transcoding and the SealPIR reply fold
+static bool device_resident(const void* ptr, int device) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, ptr) != cudaSuccess) {
+    cudaGetLastError();
+    return false;
+  }
+  return a.type == cudaMemoryTypeManaged || (a.type == cudaMemoryTypeDevice && a.device == device);
+}
+
+// rows [r0, r0 + n) of a strided host or device array, as one contiguous copy when the rows are adjacent
+static void copy_rows(char* dst, size_t dst_pitch, const char* src, size_t src_pitch, size_t width, size_t n,
+                      cudaStream_t st) {
+  if (!width || !n) return;
+  if (dst_pitch == width && src_pitch == width)
+    FHE_CUDA(cudaMemcpyAsync(dst, src, width * n, cudaMemcpyDefault, st));
+  else
+    FHE_CUDA(cudaMemcpy2DAsync(dst, dst_pitch, src, src_pitch, width, n, cudaMemcpyDefault, st));
+}
+
+int fhe_b200_transcode(const fhe_b200_params* p, const void* in, uint32_t in_elem, size_t in_len, size_t in_stride,
+                       uint32_t in_bits, void* out, uint32_t out_elem, size_t out_len, size_t out_stride,
+                       uint32_t out_bits, uint32_t n_rows, void* stream) {
+  API_BEGIN
+  REQUIRE(p, FHE_B200_INVALID_ARGUMENT, "null argument");
+  REQUIRE(in_bits >= 1 && in_bits <= 64 && out_bits >= 1 && out_bits <= 64, FHE_B200_INVALID_ARGUMENT,
+          "bit widths must be in 1..64");
+  REQUIRE((in_elem == 8 || (in_elem == 1 && in_bits == 8)) && (out_elem == 8 || (out_elem == 1 && out_bits == 8)),
+          FHE_B200_INVALID_ARGUMENT, "elements are u64 words (8) or bytes (1, with 8 bits)");
+  REQUIRE(n_rows > 0, FHE_B200_INVALID_ARGUMENT, "no rows");
+  REQUIRE(in_stride >= in_len && out_stride >= out_len, FHE_B200_INVALID_ARGUMENT, "stride shorter than the row");
+  REQUIRE((in || !in_len) && (out || !out_len), FHE_B200_INVALID_ARGUMENT, "null rows");
+  const uintptr_t ib = (uintptr_t)in, ob = (uintptr_t)out;
+  const uintptr_t ie = ib + ((size_t)(n_rows - 1) * in_stride + in_len) * in_elem;
+  const uintptr_t oe = ob + ((size_t)(n_rows - 1) * out_stride + out_len) * out_elem;
+  REQUIRE(!in_len || !out_len || ie <= ob || oe <= ib, FHE_B200_INVALID_ARGUMENT, "in and out overlap");
+  DeviceGuard g(p);
+  const bool in_dev = !in_len || device_resident(in, p->device), out_dev = !out_len || device_resident(out, p->device);
+  // a chunk stages at most what one chunk of level-0 ciphertexts holds
+  const size_t budget = ((size_t)chunk_size() * 2 * p->Lmax) << p->logn;
+  const size_t row_words = std::max<size_t>({1, (in_len * in_elem + 7) / 8, (out_len * out_elem + 7) / 8});
+  const u32 rows_per_chunk = (u32)std::max<size_t>(1, std::min<size_t>(budget / row_words, n_rows));
+  ChunkRunner chunks(p, n_rows, (cudaStream_t)stream, rows_per_chunk);
+  chunks.run([&](u32 r0, u32 n, cudaStream_t st) {
+    Workspace ws(p, st);
+    TranscodeRows T;
+    T.in_len = in_len; T.in_elem = in_elem; T.in_bits = in_bits;
+    T.out_len = out_len; T.out_elem = out_elem; T.out_bits = out_bits;
+    const char* src = (const char*)in + (size_t)r0 * in_stride * in_elem;
+    char* dst = (char*)out + (size_t)r0 * out_stride * out_elem;
+    if (in_dev) {
+      T.in = src;
+      T.in_stride = in_stride;
+    } else {
+      char* staged = (char*)ws.words(((size_t)n * in_len * in_elem + 7) / 8);
+      copy_rows(staged, in_len * in_elem, src, in_stride * in_elem, in_len * in_elem, n, st);
+      T.in = staged;
+      T.in_stride = in_len;
+    }
+    if (out_dev) {
+      T.out = dst;
+      T.out_stride = out_stride;
+    } else {
+      T.out = ws.words(((size_t)n * out_len * out_elem + 7) / 8);
+      T.out_stride = out_len;
+    }
+    launch_transcode(T, n, st);
+    if (!out_dev) copy_rows(dst, out_stride * out_elem, (const char*)T.out, out_len * out_elem, out_len * out_elem, n, st);
+  });
+  FHE_CUDA(cudaGetLastError());
+  API_END
+}
+
+int fhe_b200_fold(const fhe_b200_batch* ct, uint32_t in_bits, uint32_t out_bits, fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  REQUIRE(ct && out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  REQUIRE(ct->par == out->par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch");
+  REQUIRE(!ct->mul_basis && !out->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
+  REQUIRE(out->parts == 1, FHE_B200_BAD_POLY_COUNT, "a plaintext batch has one polynomial per entry");
+  REQUIRE(in_bits >= 1 && in_bits <= 64 && out_bits >= 1 && out_bits <= 64, FHE_B200_INVALID_ARGUMENT,
+          "bit widths must be in 1..64");
+  REQUIRE(out != ct, FHE_B200_INVALID_ARGUMENT, "out aliases ct");
+  const fhe_b200_params* par = ct->par;
+  const size_t N = par->N, row_words = (size_t)ct->limbs * N;
+  const size_t E = (row_words * in_bits + out_bits - 1) / out_bits;
+  const size_t P = (ct->parts * E + N - 1) / N;
+  REQUIRE(out->count == P * ct->count, FHE_B200_INVALID_ARGUMENT,
+          "out must hold ceil(parts * ceil(L * N * in_bits / out_bits) / N) plaintexts per ciphertext");
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(out->level);
+  const u32 L = lv.L, logn = par->logn, count = ct->count;
+  // Poly u64 words are arbitrary: the forward butterflies reduce them on load, as fhe_b200_encode does
+  ChunkRunner chunks(par, count, (cudaStream_t)stream, std::max<u32>(1, chunk_size() / (u32)P));
+  chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace ws(par, st);
+    u64* coeffs = ws.words((P * n) << logn);
+    launch_fold_stage(ct->d + c0 * ct->words_per_ct(), n, ct->parts, row_words, in_bits, out_bits, (u32)P, coeffs, logn,
+                      st);
+    for (size_t i = 0; i < P; i++)
+      launch_ntt(coeffs + ((i * n) << logn), out->d + ((i * count + c0) * L << logn), n * L, lv.ctx_ids, par->d_limbs,
+                 logn, false, L, true, st);
+  });
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
+  API_END
+}
+
 int fhe_b200_sync(void* stream) {
   API_BEGIN
   FHE_CUDA(cudaStreamSynchronize((cudaStream_t)stream));

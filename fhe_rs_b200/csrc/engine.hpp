@@ -269,4 +269,22 @@ struct PackDev {
 void launch_pack(const PackDev& P, const u64* words, unsigned char* bytes, size_t n_rows, u32 logn, cudaStream_t st);
 void launch_unpack(const PackDev& P, const unsigned char* bytes, u64* words, size_t n_rows, u32 logn, cudaStream_t st);
 
+// fhe_util::transcode_bidirectional / _to_bytes / _from_bytes (fhe-util/src/lib.rs:68-187) over independent rows, one
+// output value per thread.  Row r reads in_len elements (u64 words when in_elem == 8, bytes when 1) at
+// in + r * in_stride elements and writes out_len values (u64 or bytes) at out + r * out_stride: value k is bits
+// [k*out_bits, (k+1)*out_bits) of the row's LSB-first stream of in_bits-bit fields, zero past the stream's end.
+struct TranscodeRows {
+  const void* in;
+  void* out;
+  size_t in_len, in_stride, out_len, out_stride;
+  u32 in_elem, in_bits, out_elem, out_bits;
+};
+void launch_transcode(const TranscodeRows& T, size_t n_rows, cudaStream_t st);
+// The reply fold of the SealPIR server (examples/sealpir.rs:176-200) up to its plaintext coefficients: every part of
+// the n_ct ciphertexts at `ct` ([n_ct][parts][row_words]) is transcoded from in_bits to out_bits, giving E values per
+// part; the parts' values are concatenated and cut into P rows of N.  Row i of ciphertext j goes to
+// coeffs + (i * n_ct + j) * N, zero past the parts * E values.
+void launch_fold_stage(const u64* ct, u32 n_ct, u32 parts, size_t row_words, u32 in_bits, u32 out_bits, u32 P,
+                       u64* coeffs, u32 logn, cudaStream_t st);
+
 }  // namespace fhe_b200

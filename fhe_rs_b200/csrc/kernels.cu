@@ -1020,6 +1020,48 @@ __global__ void unpack_kernel(PackDev P, const unsigned char* bytes, u64* words,
   }
 }
 
+// ------------------------------------------------------------------ row transcoding
+// Value k of a row of `len` in_bits-bit fields read as one LSB-first bit stream: bits [k*out_bits, (k+1)*out_bits),
+// cut at the stream's end (the leftover bits of the reference's last value), zero past it.  Fields are masked to
+// in_bits, as the reference's release build does.  It reads elements floor(k*out_bits / in_bits) through
+// floor((min((k+1)*out_bits, len*in_bits) - 1) / in_bits), at most ceil(out_bits / in_bits) + 1 of them, so no value
+// depends on another.
+template <class T>
+__device__ __forceinline__ u64 bit_window(const T* row, size_t len, u32 in_bits, u32 out_bits, size_t k) {
+  const u64 total = (u64)len * in_bits, b0 = (u64)k * out_bits;
+  if (b0 >= total) return 0;
+  const u64 b1 = b0 + out_bits < total ? b0 + out_bits : total;
+  const u64 in_mask = in_bits == 64 ? ~0ull : ((1ull << in_bits) - 1);
+  u64 v = 0;
+  for (u64 e = b0 / in_bits, s = e * in_bits; s < b1; e++, s += in_bits) {
+    const u64 w = (u64)row[e] & in_mask;
+    v |= s >= b0 ? w << (s - b0) : w >> (b0 - s);   // both shifts are below 64
+  }
+  return out_bits == 64 ? v : v & ((1ull << out_bits) - 1);
+}
+
+template <class TI, class TO>
+__global__ void transcode_kernel(TranscodeRows T, size_t n_values) {
+  const TI* in = (const TI*)T.in;
+  TO* out = (TO*)T.out;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_values; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t r = i / T.out_len, k = i - r * T.out_len;
+    out[r * T.out_stride + k] = (TO)bit_window(in + r * T.in_stride, T.in_len, T.in_bits, T.out_bits, k);
+  }
+}
+
+// one thread per coefficient of the staged plaintext rows [P][n_ct][N]
+__global__ void fold_stage_kernel(const u64* ct, u32 n_ct, u32 parts, size_t row_words, u32 in_bits, u32 out_bits,
+                                  u64 E, u64* coeffs, size_t n_words, u32 logn) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_words) return;
+  const size_t c = i & ((1ull << logn) - 1), row = i >> logn;
+  const size_t p = row / n_ct, j = row - p * n_ct;
+  const u64 v = ((u64)p << logn) + c, part = v / E;
+  coeffs[i] = part < parts ? bit_window(ct + (j * parts + part) * row_words, row_words, in_bits, out_bits, v - part * E)
+                           : 0;
+}
+
 // ------------------------------------------------------------------ plaintext encoding
 // one thread per (plaintext, coefficient): reads are coalesced for Poly, writes always are
 __global__ void encode_load_kernel(const u64* staged, u64* coeffs, size_t n_words, size_t n_values, const u32* inv_map,
@@ -1921,6 +1963,27 @@ void launch_unpack(const PackDev& P, const unsigned char* bytes, u64* words, siz
   const size_t groups = n_rows << (logn - 3);
   if (!groups) return;
   unpack_kernel<<<(unsigned)((groups + 127) / 128), 128, 0, st>>>(P, bytes, words, groups, logn);
+  g_launches++;
+}
+
+void launch_transcode(const TranscodeRows& T, size_t n_rows, cudaStream_t st) {
+  const size_t n = n_rows * T.out_len;
+  if (!n) return;
+  const unsigned blocks = (unsigned)std::min<size_t>((n + 255) / 256, 1u << 20);
+  if (T.in_elem == 8 && T.out_elem == 8) transcode_kernel<u64, u64><<<blocks, 256, 0, st>>>(T, n);
+  else if (T.in_elem == 8) transcode_kernel<u64, unsigned char><<<blocks, 256, 0, st>>>(T, n);
+  else if (T.out_elem == 8) transcode_kernel<unsigned char, u64><<<blocks, 256, 0, st>>>(T, n);
+  else transcode_kernel<unsigned char, unsigned char><<<blocks, 256, 0, st>>>(T, n);
+  g_launches++;
+}
+
+void launch_fold_stage(const u64* ct, u32 n_ct, u32 parts, size_t row_words, u32 in_bits, u32 out_bits, u32 P,
+                       u64* coeffs, u32 logn, cudaStream_t st) {
+  const size_t n = ((size_t)P * n_ct) << logn;
+  if (!n) return;
+  const u64 E = ((u64)row_words * in_bits + out_bits - 1) / out_bits;
+  fold_stage_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ct, n_ct, parts, row_words, in_bits, out_bits, E,
+                                                                 coeffs, n, logn);
   g_launches++;
 }
 

@@ -6,6 +6,7 @@ The reference serialises polynomials, ciphertexts and key-switching keys with pr
     fhers.bfv.Ciphertext         fhe/src/proto/bfv.proto:5-9         (bfv/ciphertext.rs:230-257)
     fhers.bfv.KeySwitchingKey    bfv.proto:16-23                     (keys/key_switching_key.rs:365-385)
     fhers.bfv.RelinearizationKey bfv.proto:25-27, GaloisKey :29-32, RGSWCiphertext :11-14
+    fhers.bfv.EvaluationKey      bfv.proto:34-38                     (keys/evaluation_key.rs:293-310, :494-550)
     fhers.bfv.SecretKey          bfv.proto:54-56                     (keys/secret_key.rs:142-175)
 
 The heavy part of every one of them -- `Rq.coefficients`, the bit-packed power-basis words -- is produced and consumed
@@ -297,6 +298,31 @@ def decode_galois_key(data: Bytes) -> Tuple[memoryview, int]:   # galois_key.rs:
     if f[1] is None:
         raise WireError("MissingField", detail="GaloisKeySwitchingKey")
     return f[1], f[-1].get(2, 0) & 0xFFFFFFFF   # type: ignore[union-attr]
+
+
+def encode_evaluation_key(galois_keys: Sequence[Bytes], ciphertext_level: int, evaluation_key_level: int) -> bytes:
+    """EvaluationKeyProto::from(&ek).encode_to_vec() (evaluation_key.rs:494-505): the GaloisKey messages in the order
+    given (the reference writes HashMap order, so a reader may depend on none), then the two levels"""
+    out: List[Bytes] = []
+    for gk in galois_keys:
+        _put_len(out, 2, gk)
+    _put_uint(out, 3, ciphertext_level)
+    _put_uint(out, 4, evaluation_key_level)
+    return _join(out)
+
+
+def decode_evaluation_key(data: Bytes) -> Tuple[List[memoryview], int, int]:
+    """(GaloisKey messages in wire order, ciphertext_level, evaluation_key_level) of an EvaluationKey message"""
+    gks: List[memoryview] = []
+    levels = {3: 0, 4: 0}
+    for field, wt, v in _fields(data):
+        if field == 2:
+            _expect(wt, _LEN)
+            gks.append(v)
+        elif field in levels:
+            _expect(wt, _VARINT)
+            levels[field] = v & 0xFFFFFFFF
+    return gks, levels[3], levels[4]
 
 
 def encode_rgsw(ksk0: Bytes, ksk1: Bytes) -> bytes:         # rgsw_ciphertext.rs:30-37

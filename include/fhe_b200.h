@@ -493,6 +493,33 @@ int fhe_b200_batch_pack(const fhe_b200_batch* b, uint32_t first, uint32_t n, uin
  * `p.into_ntt()` does).  The whole batch must be filled with one call per disjoint range before it is used. */
 int fhe_b200_batch_unpack(fhe_b200_batch* b, uint32_t first, uint32_t n, const uint8_t* host_in, void* stream);
 
+/* ---- bit transcoding and the SealPIR reply fold ---------------------------------------------
+ * fhe_util::transcode_bidirectional, transcode_to_bytes and transcode_from_bytes (fhe-util/src/lib.rs:68-187) over
+ * n_rows independent rows in one call, on the device of `p`.  Row r of `in` is in_len elements starting r * in_stride
+ * elements from `in`; an element is a u64 word (in_elem = 8), masked to in_bits as the reference's release build does,
+ * or a byte (in_elem = 1, in_bits = 8).  Value k of output row r is bits [k*out_bits, (k+1)*out_bits) of the row's
+ * LSB-first bit stream for k < ceil(in_len * in_bits / out_bits), the last one holding the leftover bits, exactly as
+ * the reference's loop; row r receives its first out_len values, zeros after them (the truncation of
+ * examples/sealpir.rs:249-252, the zero padding of examples/util.rs:97-145), at out + r * out_stride elements, as u64
+ * words (out_elem = 8) or bytes (out_elem = 1, out_bits = 8: transcode_to_bytes).  in_len = 0 is valid (an empty
+ * stream, lib.rs:364-371).  `in` and `out` may be pageable host, pinned host or device memory; the call is only
+ * enqueued, read `out` after fhe_b200_sync(stream).  Errors: bits outside 1..64, an element size other than 1 or 8, a
+ * byte element with bits != 8, n_rows == 0, a stride shorter than its length, NULL with a non-zero length, or
+ * overlapping `in` and `out` ranges -> INVALID_ARGUMENT; host-only parameters -> NO_DEVICE. */
+int fhe_b200_transcode(const fhe_b200_params* p, const void* in, uint32_t in_elem, size_t in_len, size_t in_stride,
+                       uint32_t in_bits, void* out, uint32_t out_elem, size_t out_len, size_t out_stride,
+                       uint32_t out_bits, uint32_t n_rows, void* stream);
+/* The reply fold of the SealPIR server (examples/sealpir.rs:176-200) for every ciphertext j of `ct` in one call: the
+ * stored words of each part ([limb][N], whatever the representation, as Poly::coefficients returns them) are
+ * transcoded from in_bits to out_bits, E = ceil(L * N * in_bits / out_bits) values per part; the values of the parts,
+ * concatenated, are encoded as PlaintextVec::try_encode(values, Encoding::poly_at_level(out.level)) with the words of
+ * fhe_b200_encode (POLY, u64): P = ceil(parts * E / N) plaintexts per ciphertext.  Plaintext i of ciphertext j is entry
+ * i * ct.count + j of `out`, a 1-part batch of P * ct.count entries that becomes NTT: fhe_b200_dot_product_scalar of
+ * the dim2 selectors (shared) with `out` and n_terms = ct.count gives all P response ciphertexts in one call.
+ * Errors: operands of different parameter sets or over the multiplication basis -> CONTEXT_MISMATCH; `out` not 1-part
+ * -> BAD_POLY_COUNT; a wrong `out` count, bits outside 1..64 or `out` == `ct` -> INVALID_ARGUMENT. */
+int fhe_b200_fold(const fhe_b200_batch* ct, uint32_t in_bits, uint32_t out_bits, fhe_b200_batch* out, void* stream);
+
 int fhe_b200_sync(void* stream);
 /* kernels launched by this library in the calling process so far (bench.py "gpu_launches") */
 uint64_t fhe_b200_launch_count(void);

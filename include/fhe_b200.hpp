@@ -198,6 +198,9 @@ class Ciphertext {
     check(fhe_b200_batch_copy(c.h_, h_, stream_));
     return c;
   }
+  // the SealPIR reply fold (examples/sealpir.rs:176-200, fhe_b200_fold): plaintext i of ciphertext j is entry
+  // i * count() + j of the result, encoded with Encoding::poly_at_level(level)
+  PlaintextVec fold(uint32_t in_bits, uint32_t out_bits, uint32_t level) const;
   // a new batch of the n ciphertexts first, first + stride, ..., first + (n-1)*stride
   Ciphertext take(uint32_t first, uint32_t n, uint32_t stride = 1) const {
     Ciphertext c(par_, n, len(), level(), representation(), stream_);
@@ -337,6 +340,7 @@ class PlaintextVec {
 
  protected:
   friend class SecretKey;
+  friend class Ciphertext;              // Ciphertext::fold
   friend class mbfv::PlaintextAccess;   // Plaintext::from_shares builds plaintexts without an encoding
   PlaintextVec(Ciphertext b, const Encoding& e) : batch_(std::move(b)), encoding_(e) {}
   explicit PlaintextVec(Ciphertext b) : batch_(std::move(b)), encoding_(Encoding::poly()), has_encoding_(false) {}
@@ -365,6 +369,48 @@ class Plaintext : public PlaintextVec {
  private:
   explicit Plaintext(PlaintextVec&& v) : PlaintextVec(std::move(v)) {}
 };
+
+inline PlaintextVec Ciphertext::fold(uint32_t in_bits, uint32_t out_bits, uint32_t level) const {
+  const uint64_t n = par_->degree();
+  uint64_t per_ct = 1;
+  if (in_bits >= 1 && in_bits <= 64 && out_bits >= 1 && out_bits <= 64) {   // (otherwise fhe_b200_fold refuses them)
+    const uint64_t e = (limbs() * n * in_bits + out_bits - 1) / out_bits;
+    per_ct = (len() * e + n - 1) / n;
+  }
+  Ciphertext out(par_, (uint32_t)(per_ct * count()), 1, level, Representation::Ntt, stream_);
+  check(fhe_b200_fold(h_, in_bits, out_bits, out.h_, stream_));
+  return PlaintextVec(std::move(out), Encoding::poly_at_level(level));
+}
+
+// fhe_util::transcode_bidirectional / transcode_to_bytes / transcode_from_bytes (fhe-util/src/lib.rs:68-187) on the
+// device of `par` (fhe_b200_transcode), one row
+inline std::vector<uint64_t> transcode_bidirectional(const std::shared_ptr<BfvParameters>& par, const std::vector<uint64_t>& a,
+                                                     uint32_t input_nbits, uint32_t output_nbits) {
+  const size_t n = output_nbits ? (a.size() * input_nbits + output_nbits - 1) / output_nbits : 0;
+  std::vector<uint64_t> out(n);
+  check(fhe_b200_transcode(par->handle(), a.empty() ? nullptr : a.data(), 8, a.size(), a.size(), input_nbits,
+                           out.empty() ? nullptr : out.data(), 8, n, n, output_nbits, 1, nullptr));
+  check(fhe_b200_sync(nullptr));
+  return out;
+}
+inline std::vector<uint8_t> transcode_to_bytes(const std::shared_ptr<BfvParameters>& par, const std::vector<uint64_t>& a,
+                                               uint32_t nbits) {
+  const size_t n = (a.size() * nbits + 7) / 8;
+  std::vector<uint8_t> out(n);
+  check(fhe_b200_transcode(par->handle(), a.empty() ? nullptr : a.data(), 8, a.size(), a.size(), nbits,
+                           out.empty() ? nullptr : out.data(), 1, n, n, 8, 1, nullptr));
+  check(fhe_b200_sync(nullptr));
+  return out;
+}
+inline std::vector<uint64_t> transcode_from_bytes(const std::shared_ptr<BfvParameters>& par, const std::vector<uint8_t>& b,
+                                                  uint32_t nbits) {
+  const size_t n = nbits ? (b.size() * 8 + nbits - 1) / nbits : 0;
+  std::vector<uint64_t> out(n);
+  check(fhe_b200_transcode(par->handle(), b.empty() ? nullptr : b.data(), 1, b.size(), b.size(), 8,
+                           out.empty() ? nullptr : out.data(), 8, n, n, nbits, 1, nullptr));
+  check(fhe_b200_sync(nullptr));
+  return out;
+}
 
 inline Ciphertext& Ciphertext::mul_plain(const PlaintextVec& pts) {
   check(fhe_b200_mul_plain_batch(h_, pts.batch().handle(), stream_));
@@ -604,9 +650,16 @@ class RGSWCiphertext {
   std::shared_ptr<KeySwitchingKey> ksk0, ksk1;
 };
 
+// fhe::bfv::EvaluationKey (keys/evaluation_key.rs:21-310): Galois keys by exponent, and the levels of the ciphertexts
+// it takes and of its keys (both 0 unless an EvaluationKeyBuilder or a message sets them)
 class EvaluationKey {
  public:
-  explicit EvaluationKey(std::shared_ptr<BfvParameters> par) : par_(std::move(par)) {}
+  explicit EvaluationKey(std::shared_ptr<BfvParameters> par, uint32_t ciphertext_level = 0,
+                         uint32_t evaluation_key_level = 0)
+      : par_(std::move(par)), ciphertext_level_(ciphertext_level), evaluation_key_level_(evaluation_key_level) {}
+  uint32_t ciphertext_level() const { return ciphertext_level_; }
+  uint32_t evaluation_key_level() const { return evaluation_key_level_; }
+  const std::map<uint32_t, std::shared_ptr<GaloisKey>>& galois_keys() const { return gk_; }   // ascending exponents
   void add_galois_key(std::shared_ptr<GaloisKey> gk) { gk_[gk->exponent % (2 * (uint32_t)par_->degree())] = std::move(gk); }
   Ciphertext rotates_rows(const Ciphertext& ct) const { return at(2 * (uint32_t)par_->degree() - 1).relinearize(ct); }
   Ciphertext rotates_columns_by(const Ciphertext& ct, uint32_t i) const { return at(column_exponent(i)).relinearize(ct); }
@@ -673,6 +726,7 @@ class EvaluationKey {
     return *it->second;
   }
   std::shared_ptr<BfvParameters> par_;
+  uint32_t ciphertext_level_, evaluation_key_level_;
   std::map<uint32_t, std::shared_ptr<GaloisKey>> gk_;
 };
 
@@ -729,7 +783,7 @@ class EvaluationKeyBuilder {
   // EvaluationKeyBuilder::build (evaluation_key.rs:429-491): every Galois key in one device call, the exponents
   // ascending, so a seed fixes the key of each exponent
   EvaluationKey build(const uint8_t* seed = nullptr) const {
-    EvaluationKey ek(sk_.par());
+    EvaluationKey ek(sk_.par(), ciphertext_level_, key_level_);
     const std::vector<uint64_t> e = exponents();
     if (e.empty()) return ek;
     for (GaloisKey& gk : GaloisKey::generate(sk_, e, ciphertext_level_, key_level_, seed))

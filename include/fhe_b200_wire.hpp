@@ -5,7 +5,8 @@
 //   fhers.bfv.Ciphertext          fhe/src/proto/bfv.proto:5-9,       fhe/src/bfv/ciphertext.rs:230-317
 //   fhers.bfv.KeySwitchingKey     bfv.proto:16-23,                   fhe/src/bfv/keys/key_switching_key.rs:365-482
 //   fhers.bfv.RelinearizationKey  bfv.proto:25-27 (keys/relinearization_key.rs:113-135), GaloisKey :29-32
-//                                 (keys/galois_key.rs:146-173)
+//                                 (keys/galois_key.rs:146-173), EvaluationKey :34-38 (keys/evaluation_key.rs:293-310,
+//                                 :494-550)
 //   fhers.bfv.SecretKey           bfv.proto:54-56,                   fhe/src/bfv/keys/secret_key.rs:142-175
 //   fhers.bfv.PublicKey           bfv.proto:50-52,                   fhe/src/bfv/keys/public_key.rs:95-149
 // `Rq.coefficients` -- the bit-packed power-basis words, all but a few bytes of every message -- is produced and consumed
@@ -250,6 +251,30 @@ inline std::string encode_galois_key(const std::string& ksk, uint32_t exponent) 
   put_uint(out, 2, exponent);
   return out;
 }
+// EvaluationKeyProto::from(&ek).encode_to_vec() (evaluation_key.rs:494-505): the GaloisKey messages in the order given
+// (the reference writes HashMap order, so a reader may depend on none), then the two levels
+inline std::string encode_evaluation_key(const std::vector<std::string>& gks, uint32_t ciphertext_level,
+                                         uint32_t evaluation_key_level) {
+  std::string out;
+  for (auto& g : gks) put_len(out, 2, g);
+  put_uint(out, 3, ciphertext_level);
+  put_uint(out, 4, evaluation_key_level);
+  return out;
+}
+struct EvaluationKeyMsg {
+  std::vector<Span> gk;   // wire order
+  uint32_t ciphertext_level = 0, evaluation_key_level = 0;
+};
+inline EvaluationKeyMsg decode_evaluation_key(const void* data, size_t n) {
+  EvaluationKeyMsg m;
+  Reader r(data, n);
+  while (r.next()) {
+    if (r.field == 2) { r.expect(2); m.gk.push_back(r.span); }
+    else if (r.field == 3) { r.expect(0); m.ciphertext_level = (uint32_t)r.value; }
+    else if (r.field == 4) { r.expect(0); m.evaluation_key_level = (uint32_t)r.value; }
+  }
+  return m;
+}
 inline std::string encode_rgsw(const std::string& ksk0, const std::string& ksk1) {   // rgsw_ciphertext.rs:30-37
   std::string out;
   put_len(out, 1, ksk0);
@@ -444,11 +469,13 @@ inline RelinearizationKey relinearization_key_from_bytes(std::shared_ptr<BfvPara
   return RelinearizationKey(key_switching_key_from_bytes(std::move(par), s.p, s.n));
 }
 // GaloisKey::from_bytes (galois_key.rs:155-173)
-inline GaloisKey galois_key_from_bytes(std::shared_ptr<BfvParameters> par, const std::string& data) {
+// (seeded_c1 as for key_switching_key_from_bytes)
+inline GaloisKey galois_key_from_bytes(std::shared_ptr<BfvParameters> par, const std::string& data,
+                                       const uint64_t* seeded_c1 = nullptr) {
   uint32_t exponent = 0;
   wire::Span s = wire::sub_message(data.data(), data.size(), 1, "GaloisKeySwitchingKey", &exponent);
   const uint32_t two_n = 2 * (uint32_t)par->degree();
-  auto ksk = key_switching_key_from_bytes(std::move(par), s.p, s.n);
+  auto ksk = key_switching_key_from_bytes(std::move(par), s.p, s.n, seeded_c1);
   exponent %= two_n;                        // SubstitutionExponent::new (rq/mod.rs:99-106)
   if (!(exponent & 1)) throw WireError("InvalidSubstitutionExponent", FHE_B200_INVALID_EXPONENT);
   return GaloisKey(exponent, std::move(ksk));
@@ -480,6 +507,33 @@ inline std::string to_bytes(const KeySwitchingKey& k) {
 inline std::string to_bytes(const RelinearizationKey& rk) { return wire::encode_relinearization_key(to_bytes(*rk.ksk)); }
 inline std::string to_bytes(const GaloisKey& gk) { return wire::encode_galois_key(to_bytes(*gk.ksk), gk.exponent); }
 inline std::string to_bytes(const RGSWCiphertext& r) { return wire::encode_rgsw(to_bytes(*r.ksk0), to_bytes(*r.ksk1)); }
+// EvaluationKey::to_bytes (evaluation_key.rs:293-297, :494-505), the Galois keys in ascending exponent order
+inline std::string to_bytes(const EvaluationKey& ek) {
+  std::vector<std::string> gks;
+  for (auto& kv : ek.galois_keys()) gks.push_back(to_bytes(*kv.second));
+  return wire::encode_evaluation_key(gks, ek.ciphertext_level(), ek.evaluation_key_level());
+}
+// EvaluationKey::from_bytes (evaluation_key.rs:299-310, :507-550): every key through galois_key_from_bytes; a key at
+// other levels than the message's, or a message ciphertext level beyond the parameters', -> InvalidLevel; a repeated
+// exponent keeps the later key (HashMap::insert).  seeded_c1: exponent (mod 2N) -> the host-expanded c1 of a compact key.
+inline EvaluationKey evaluation_key_from_bytes(std::shared_ptr<BfvParameters> par, const std::string& data,
+                                               const std::map<uint32_t, const uint64_t*>& seeded_c1 = {}) {
+  const wire::EvaluationKeyMsg m = wire::decode_evaluation_key(data.data(), data.size());
+  EvaluationKey ek(par, m.ciphertext_level, m.evaluation_key_level);
+  const uint32_t two_n = 2 * (uint32_t)par->degree();
+  for (const wire::Span& g : m.gk) {
+    uint32_t exponent = 0;
+    wire::sub_message(g.p, g.n, 1, "GaloisKeySwitchingKey", &exponent);
+    auto it = seeded_c1.find(exponent % two_n);
+    auto gk = std::make_shared<GaloisKey>(
+        galois_key_from_bytes(par, std::string((const char*)g.p, g.n), it == seeded_c1.end() ? nullptr : it->second));
+    if (gk->ksk->ciphertext_level() != m.ciphertext_level || gk->ksk->ksk_level() != m.evaluation_key_level)
+      throw WireError("InvalidLevel", FHE_B200_INVALID_LEVEL);
+    ek.add_galois_key(std::move(gk));
+  }
+  if (m.ciphertext_level > par->max_level()) throw WireError("InvalidLevel", FHE_B200_INVALID_LEVEL);
+  return ek;
+}
 
 // SecretKey::to_bytes / from_bytes (secret_key.rs:142-175)
 inline std::string to_bytes(const SecretKey& sk) { return wire::encode_secret_key(sk.coeffs().data(), sk.coeffs().size()); }
