@@ -65,6 +65,8 @@ SYMBOLS = {
     "fhe_b200_add_plain_batch": (_i, [_vp, _vp, _i, _vp]),
     "fhe_b200_secret_key_create": (_i, [_vp, _vp, _pp]),
     "fhe_b200_secret_key_free": (_i, [_vp]),
+    "fhe_b200_secret_keys_random": (_i, [_vp, _u32, _u32, _vp, _pp, _vp]),
+    "fhe_b200_secret_key_coeffs": (_i, [_vp, _vp, _vp]),
     "fhe_b200_decrypt": (_i, [_vp, _vp, _vp, _vp]),
     "fhe_b200_decode": (_i, [_vp, _i, _i, _vp, _vp, C.c_size_t, _vp]),
     "fhe_b200_measure_noise": (_i, [_vp, _vp, _vp, _vp]),

@@ -126,6 +126,17 @@ class BfvParameters:
     def degree(self) -> int:  # parameters.rs:130
         return self._degree
 
+    def to_bytes(self) -> bytes:
+        """BfvParameters::to_bytes (parameters.rs:741-759): the Parameters message (bfv.proto:40-48)"""
+        return wire.encode_parameters(self._degree, self._moduli, self._plaintext, self.variance)
+
+    @staticmethod
+    def from_bytes(data: bytes, device: int = 0) -> "BfvParameters":
+        """BfvParameters::try_deserialize (parameters.rs:762-789): built with the message's explicit moduli and variance,
+        so every builder error keeps its code (a variance of 0, the proto3 default, is InvalidVariance)."""
+        degree, moduli, plaintext, variance = wire.decode_parameters(data)
+        return BfvParameters(degree, plaintext, moduli=moduli, device=device, variance=variance)
+
     def moduli(self):  # parameters.rs:136
         return list(self._moduli)
 
@@ -627,11 +638,11 @@ class PlaintextVec:
 
 
 class SecretKey:
-    """fhe::bfv::SecretKey (keys/secret_key.rs:25-53) on the device, from its N signed coefficients.  Encryption,
-    decryption and noise measurement run on the device; the device copy of s is erased when the key is released.
-    Encryption and key generation (RelinearizationKey.new, GaloisKey.new, EvaluationKeyBuilder, try_encrypt_rgsw) draw
-    their randomness from the seeded ChaCha20 stream of include/fhe_b200.h.  The coefficients themselves
-    (SecretKey::random) come from the client."""
+    """fhe::bfv::SecretKey (keys/secret_key.rs:25-53) on the device, from its N signed coefficients or drawn on the
+    device (SecretKey.random / random_vec).  Encryption, decryption and noise measurement run on the device; the device
+    copy of s is erased when the key is released.  Encryption and key generation (RelinearizationKey.new, GaloisKey.new,
+    EvaluationKeyBuilder, try_encrypt_rgsw) draw their randomness from the seeded ChaCha20 stream of
+    include/fhe_b200.h."""
 
     def __init__(self, par: BfvParameters, coeffs):
         c = np.array(coeffs, dtype=np.int64)   # our own copy, kept for to_bytes (the reference keeps SecretKey.coeffs)
@@ -650,8 +661,40 @@ class SecretKey:
         if c is not None:
             c[:] = 0
 
+    @staticmethod
+    def random(par: BfvParameters, seed: Optional[bytes] = None) -> "SecretKey":
+        """SecretKey::random (secret_key.rs:42-45): s = sample_vec_cbd(N, par.variance) drawn on the device from the
+        seeded stream (role 18, key 0).  seed: 32 bytes; None draws os.urandom(32) (a seed must never be reused)."""
+        return SecretKey.random_vec(par, 1, seed)[0]
+
+    @staticmethod
+    def random_vec(par: BfvParameters, n: int, seed: Optional[bytes] = None) -> "List[SecretKey]":
+        """n independent SecretKey::random keys in one device call (key k is stream word 13 = k), e.g. one per party of
+        multiparty BFV.  The coefficients stay on the device; to_bytes downloads them."""
+        hs = (C.c_void_p * max(1, int(n)))()
+        check(_capi.lib().fhe_b200_secret_keys_random(par._h, int(n), par.variance, _seed(seed),
+                                                      C.cast(hs, C.POINTER(C.c_void_p)), 0))
+        out = []
+        for h in hs[:n]:
+            sk = SecretKey.__new__(SecretKey)
+            sk._coeffs, sk._h, sk.par = None, C.c_void_p(h), par
+            out.append(sk)
+        return out
+
     def to_bytes(self) -> bytes:   # secret_key.rs:142-148
-        return wire.encode_secret_key(self._coeffs.tolist())
+        if self._coeffs is not None:
+            return wire.encode_secret_key(self._coeffs.tolist())
+        c = self._download_coeffs()
+        try:
+            return wire.encode_secret_key(c.tolist())
+        finally:
+            c[:] = 0
+
+    def _download_coeffs(self) -> np.ndarray:
+        """the key's N signed coefficients from the device (fhe_b200_secret_key_coeffs); the caller erases them"""
+        c = np.zeros(self.par.degree(), np.int64)
+        check(_capi.lib().fhe_b200_secret_key_coeffs(self._h, _ptr(c), 0))
+        return c
 
     @staticmethod
     def from_bytes(par: BfvParameters, data: bytes) -> "SecretKey":   # secret_key.rs:151-175

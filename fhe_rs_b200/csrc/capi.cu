@@ -1666,6 +1666,69 @@ int fhe_b200_encrypt_pk(const fhe_b200_batch* pk, const fhe_b200_batch* pts, uin
   API_END
 }
 
+// ---- SecretKey::random (secret_key.rs:42-45) for n_keys keys in one call.  Key k is sample_vec_cbd(N, variance) of
+// the role-18 row (k, limb 0), written as its canonical residue into every limb (Poly::try_convert_from(&[i64])) and
+// transformed: the words fhe_b200_secret_key_create makes from the same coefficients, which never reach the host.  The
+// keys go through the chunk runner, per chunk at most chunk_size() rows of scratch (chunk_size() / Lmax keys): one
+// launch draws the chunk's keys, one transform takes them to the NTT domain, then each key's rows are copied into its
+// own SecretBuffer.  On failure the keys made so far are freed and out is left untouched.
+int fhe_b200_secret_keys_random(const fhe_b200_params* p, uint32_t n_keys, uint32_t variance, const uint8_t* seed,
+                                fhe_b200_secret_key** out, void* stream) {
+  API_BEGIN
+  REQUIRE(p && seed && out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  REQUIRE(n_keys, FHE_B200_INVALID_ARGUMENT, "n_keys is 0");
+  check_variance(variance);
+  REQUIRE(p->t_small, FHE_B200_UNSUPPORTED, "the plaintext modulus does not fit a u64 Modulus");
+  DeviceGuard g(p);
+  const EncSeed K = seed_words(seed);
+  const LevelData& l0 = p->level(0);
+  const u32 Lmax = p->Lmax, logn = p->logn;
+  const size_t words = (size_t)Lmax << logn;
+  std::vector<std::unique_ptr<fhe_b200_secret_key>> made;   // freed again unless the call succeeds
+  for (u32 k = 0; k < n_keys; k++) made.emplace_back(new fhe_b200_secret_key(p));
+  cudaStream_t user = (cudaStream_t)stream;
+  {
+    ChunkRunner chunks(p, n_keys, user, std::max(1u, chunk_size() / Lmax));
+    chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+      Workspace ws(p, st);
+      u64* s = ws.secret_words(n * words);
+      launch_cbd(s, n, c0, 18, 1, variance, K, l0.ctx_ids, p->d_limbs, logn, st);
+      launch_ntt(s, s, n * Lmax, l0.ctx_ids, p->d_limbs, logn, false, 1, false, st);   // into_ntt
+      for (u32 k = 0; k < n; k++)
+        FHE_CUDA(cudaMemcpyAsync(made[c0 + k]->s.d, s + k * words, words * sizeof(u64), cudaMemcpyDeviceToDevice, st));
+    });
+  }
+  FHE_CUDA(cudaGetLastError());
+  FHE_CUDA(cudaStreamSynchronize(user));   // the keys are ready on every stream, as after fhe_b200_secret_key_create
+  for (u32 k = 0; k < n_keys; k++) out[k] = made[k].release();
+  API_END
+}
+
+// SecretKey.coeffs (secret_key.rs:25-30, read by to_bytes :142-148): limb 0 of s back to the power basis, each word
+// centred modulo q_0 on the host (v - q_0 when v > q_0 / 2, by a mask)
+int fhe_b200_secret_key_coeffs(const fhe_b200_secret_key* sk, int64_t* out, void* stream) {
+  API_BEGIN
+  REQUIRE(sk && out, FHE_B200_INVALID_ARGUMENT, "null argument");
+  const fhe_b200_params* par = sk->par;
+  DeviceGuard g(par);
+  const u32 N = par->N;
+  cudaStream_t st = (cudaStream_t)stream;
+  {
+    Workspace ws(par, st);
+    u64* w = ws.secret_words(N);
+    launch_ntt(sk->s.d, w, 1, par->level(0).ctx_ids, par->d_limbs, par->logn, true, 1, false, st);
+    FHE_CUDA(cudaMemcpyAsync(out, w, (size_t)N * sizeof(u64), cudaMemcpyDefault, st));
+  }
+  FHE_CUDA(cudaGetLastError());
+  FHE_CUDA(cudaStreamSynchronize(st));
+  const u64 q0 = par->moduli[0];
+  for (u32 i = 0; i < N; i++) {
+    const u64 v = (u64)out[i];
+    out[i] = (int64_t)(v - (q0 & (0 - (u64)(v > (q0 >> 1)))));
+  }
+  API_END
+}
+
 // ---- key generation (key_switching_key.rs:71-238, relinearization_key.rs:43-65, galois_key.rs:26-60,
 // rgsw_ciphertext.rs:94-120).  Every value is a canonical residue and the NTT is linear, so the key is built in the NTT
 // domain: c0_i = NTT(e_i) - c1_i s + G[i] x, with x the key's polynomial at the ciphertext level.  The switch-up of x

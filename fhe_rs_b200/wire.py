@@ -8,10 +8,11 @@ The reference serialises polynomials, ciphertexts and key-switching keys with pr
     fhers.bfv.RelinearizationKey bfv.proto:25-27, GaloisKey :29-32, RGSWCiphertext :11-14
     fhers.bfv.EvaluationKey      bfv.proto:34-38                     (keys/evaluation_key.rs:293-310, :494-550)
     fhers.bfv.SecretKey          bfv.proto:54-56                     (keys/secret_key.rs:142-175)
+    fhers.bfv.Parameters         bfv.proto:40-48                     (bfv/parameters.rs:741-789)
 
 The heavy part of every one of them -- `Rq.coefficients`, the bit-packed power-basis words -- is produced and consumed
 on the device (fhe_b200_batch_pack / fhe_b200_batch_unpack).  This module is the few bytes around it: a hand-written
-proto3 wire codec for exactly these messages, emitting what prost emits (fields in field-number order, zero scalars
+proto3 wire codec for exactly these messages, emitting what prost emits (fields in field-number order, a oneof at its lowest field number, zero scalars
 and empty singular `bytes` omitted, every element of a repeated `bytes` present, a present sub-message always
 written) and accepting what prost accepts (any field order, unknown fields skipped, last scalar wins).  It depends on
 nothing but the standard library; the tests compare it byte for byte with the google.protobuf runtime.
@@ -388,6 +389,60 @@ def decode_secret_key(data: Bytes, degree: int) -> List[int]:   # secret_key.rs:
     if len(coeffs) != degree:
         raise WireError("InvalidSecretKeyCoefficientCount", detail="%d coefficients, expected %d" % (len(coeffs), degree))
     return coeffs
+
+
+# ------------------------------------------------------------------------------------------ Parameters
+def plaintext_is_small(t: int) -> bool:
+    """t is a zq::Modulus (2 <= t < 2^62): where PlaintextModulus::as_u64 is Some and the message carries `plaintext`"""
+    return 2 <= t < 1 << 62
+
+
+def encode_parameters(degree: int, moduli: Sequence[int], plaintext: int, variance: int) -> bytes:
+    """BfvParameters::to_bytes (parameters.rs:741-759), bfv.proto:40-48: degree = 1, moduli = 2 (packed), the oneof
+    plaintext = 3 (uint64) / plaintext_big = 5 (little-endian bytes), variance = 4.  prost writes a oneof at the
+    position of its lowest field number, so plaintext_big goes before variance, as plaintext does."""
+    out: List[Bytes] = []
+    _put_uint(out, 1, degree)
+    if len(moduli):
+        _put_len(out, 2, b"".join(_varint(int(q)) for q in moduli))
+    t = int(plaintext)
+    if plaintext_is_small(t):
+        out.append(_key(3, _VARINT) + _varint(t))         # a set oneof member is written even when it is zero
+    else:
+        _put_len(out, 5, t.to_bytes(max(1, (t.bit_length() + 7) // 8), "little"))   # BigUint::to_bytes_le
+    _put_uint(out, 4, variance)
+    return _join(out)
+
+
+def decode_parameters(data: Bytes) -> Tuple[int, List[int], int, int]:
+    """(degree, moduli, plaintext modulus, variance) of a Parameters message (parameters.rs:762-781): packed and
+    unpacked moduli are both accepted, the last oneof member wins; malformed bytes are Decode, a message without
+    either member is MissingField (ParametersPlaintextModulus)."""
+    degree = variance = 0
+    moduli: List[int] = []
+    plaintext: Optional[int] = None
+    for field, wt, v in _fields(data):
+        if field in (1, 4):
+            _expect(wt, _VARINT)
+            if field == 1:
+                degree = v & 0xFFFFFFFF
+            else:
+                variance = v & 0xFFFFFFFF
+        elif field == 2:
+            if wt == _VARINT:
+                moduli.append(v)
+            else:
+                _expect(wt, _LEN)
+                moduli.extend(_packed_varints(v))
+        elif field == 3:
+            _expect(wt, _VARINT)
+            plaintext = v
+        elif field == 5:
+            _expect(wt, _LEN)
+            plaintext = int.from_bytes(bytes(v), "little")
+    if plaintext is None:
+        raise WireError("MissingField", detail="ParametersPlaintextModulus")
+    return degree, moduli, plaintext, variance
 
 
 def _packed_varints(buf: memoryview) -> Iterator[int]:

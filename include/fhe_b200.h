@@ -254,9 +254,9 @@ int fhe_b200_measure_noise(const fhe_b200_secret_key* sk, const fhe_b200_batch* 
  *     word 12      b, the block index within the row
  *     word 13      the index of the ciphertext within the call (0 .. out.count - 1)
  *     word 14      role << 8 | limb: role 0 = a, 1 = e (secret-key encryption), 2 = u, 3 = e1, 4 = e2 (public-key
- *                  encryption), 5 = c1, 6 = e (key generation, below), 7, 8, 14 - 17 (multiparty BFV, below); the
- *                  small polynomials use limb 0
- *     word 15      0 (encryption, multiparty BFV), the digit of the key (key generation)
+ *                  encryption), 5 = c1, 6 = e (key generation, below), 7 - 17 (multiparty BFV, below), 18 = s
+ *                  (fhe_b200_secret_keys_random, below, word 13 = the key's index); the small polynomials use limb 0
+ *     word 15      0 (encryption, multiparty BFV, secret keys), the digit of the key (key generation)
  * Each block is addressed only by its position, so the words do not depend on chunking or streams.  One 64-byte block
  * gives four 128-bit values: value m is u64 words 2m (low) and 2m + 1 (high) of the block, and coefficient 4b + m of
  * the row takes value m of block b.
@@ -284,6 +284,25 @@ int fhe_b200_encrypt_sk(const fhe_b200_secret_key* sk, const fhe_b200_batch* pts
  * one 2-part ciphertext -> INVALID_ARGUMENT; power-basis pk -> INVALID_REPRESENTATION. */
 int fhe_b200_encrypt_pk(const fhe_b200_batch* pk, const fhe_b200_batch* pts, uint32_t variance, const uint8_t* seed,
                         fhe_b200_batch* out, void* stream);
+/* SecretKey::random (secret_key.rs:42-45) for n_keys independent keys in one call (one per party of multiparty BFV):
+ * key k is s = sample_vec_cbd(N, variance) (fhe-util/src/lib.rs:22-67) drawn from the stream above as role 18, limb 0,
+ * word 13 = k, word 15 = 0, by the same 128-bit value -> centred binomial rule as e (the reference's distribution for
+ * every variance in 1..32).  The coefficients never pass through host memory: one kernel writes the canonical residue
+ * of every coefficient on every modulus (Poly::try_convert_from(&[i64])) and the NTT transforms them, so key k holds
+ * exactly the device words fhe_b200_secret_key_create makes from the same coefficients.  Scratch goes back to the pool
+ * zeroed, each key is erased when freed, and no kernel branches on the data.  out receives n_keys handles; the call
+ * returns once they are ready on every stream.  seed: 32 bytes of fresh entropy (a Rust host passes OsRng bytes);
+ * variance: BfvParameters::variance.  Errors: as fhe_b200_secret_key_create (t beyond a u64 Modulus -> UNSUPPORTED;
+ * host-only parameters -> NO_DEVICE); variance outside 1..32 (InvalidVariance), a NULL parameter set, seed or out,
+ * n_keys == 0 -> INVALID_ARGUMENT.  A failed call returns no handle and frees every key it made. */
+int fhe_b200_secret_keys_random(const fhe_b200_params* p, uint32_t n_keys, uint32_t variance, const uint8_t* seed,
+                                fhe_b200_secret_key** out, void* stream);
+/* SecretKey.coeffs (secret_key.rs:25-30), what SecretKey::to_bytes (:142-148) writes: out (N words of host memory)
+ * receives the inverse NTT of the key's limb 0, each word centred modulo q_0 (v - q_0 when v > q_0 / 2).  These are
+ * the key's coefficients whenever they lie within (-q_0 / 2, q_0 / 2], as every fhe_b200_secret_keys_random key's
+ * do.  The only way a device-born key's coefficients reach the host; the call returns once out is written.  Errors: a
+ * NULL key or out -> INVALID_ARGUMENT. */
+int fhe_b200_secret_key_coeffs(const fhe_b200_secret_key* sk, int64_t* out, void* stream);
 
 /* ---- key generation ------------------------------------------------------------------------------
  * KeySwitchingKey::new (key_switching_key.rs:71-238) on the device, for every digit i of every key of the call:

@@ -9,8 +9,8 @@
 //   bfv::GaloisKey / EvaluationKey              bfv/keys/galois_key.rs:18, evaluation_key.rs:110-170
 //   bfv::Multiplicator                          bfv/ops/mul.rs:22
 //   bfv::Encoding / Plaintext / PlaintextVec    bfv/encoding.rs, bfv/plaintext.rs:20, plaintext_vec.rs:20
-//   bfv::SecretKey / PublicKey                  bfv/keys/secret_key.rs:25, public_key.rs:17 (encryption, decryption,
-//                                               measure_noise; key generation stays client-side)
+//   bfv::SecretKey / PublicKey                  bfv/keys/secret_key.rs:25, public_key.rs:17 (SecretKey::random,
+//                                               encryption, decryption, measure_noise)
 // Fallible reference calls return Result<_, fhe::Error>; here they throw fhe_b200::Error carrying
 // the fhe_b200_status code (same variants, see fhe_b200.h).
 #pragma once
@@ -62,6 +62,8 @@ class BfvParameters {
   size_t max_level() const { return fhe_b200_params_n_moduli(h_) - 1; }
   // BfvParameters::variance (parameters.rs:98-99): the centred binomial parameter of encryption's errors
   uint32_t variance() const { return variance_; }
+  // the plaintext modulus as little-endian bytes without trailing zeros (BigUint::to_bytes_le, at least one byte)
+  const std::vector<uint8_t>& plaintext_le() const { return plaintext_le_; }
   std::vector<uint64_t> mul_basis(uint32_t level) const {
     uint32_t n = 0;
     check(fhe_b200_params_mul_basis(h_, level, nullptr, &n));
@@ -80,12 +82,13 @@ class BfvParameters {
 
  private:
   friend class BfvParametersBuilder;
-  BfvParameters(fhe_b200_params* h, bool has_psi_t, uint64_t psi_t, uint32_t variance)
-      : h_(h), has_plaintext_psi_(has_psi_t), plaintext_psi_(psi_t), variance_(variance) {}
+  BfvParameters(fhe_b200_params* h, bool has_psi_t, uint64_t psi_t, uint32_t variance, std::vector<uint8_t> t_le)
+      : h_(h), has_plaintext_psi_(has_psi_t), plaintext_psi_(psi_t), variance_(variance), plaintext_le_(std::move(t_le)) {}
   fhe_b200_params* h_;
   bool has_plaintext_psi_;
   uint64_t plaintext_psi_;
   uint32_t variance_;
+  std::vector<uint8_t> plaintext_le_;
   mutable std::once_flag enc_once_;
   mutable fhe_b200_encoder* enc_ = nullptr;
 
@@ -96,7 +99,13 @@ class BfvParameters {
 class BfvParametersBuilder {
  public:
   BfvParametersBuilder& set_degree(size_t d) { degree_ = (uint32_t)d; return *this; }
-  BfvParametersBuilder& set_plaintext_modulus(uint64_t t) { plaintext_ = t; return *this; }
+  BfvParametersBuilder& set_plaintext_modulus(uint64_t t) {
+    plaintext_.assign(8, 0);
+    for (int i = 0; i < 8; i++) plaintext_[i] = (uint8_t)(t >> (8 * i));
+    return *this;
+  }
+  // set_plaintext_modulus_biguint (parameters.rs:349-356): t as little-endian bytes of any length
+  BfvParametersBuilder& set_plaintext_modulus_le(const std::vector<uint8_t>& t_le) { plaintext_ = t_le; return *this; }
   BfvParametersBuilder& set_moduli(const std::vector<uint64_t>& m) { moduli_ = m; return *this; }
   BfvParametersBuilder& set_moduli_sizes(const std::vector<uint32_t>& s) { sizes_ = s; return *this; }
   BfvParametersBuilder& set_ntt_roots(const std::vector<uint64_t>& psi) { psi_ = psi; return *this; }
@@ -107,23 +116,25 @@ class BfvParametersBuilder {
   BfvParametersBuilder& set_plaintext_ntt_root(uint64_t psi_t) { psi_t_ = psi_t; has_psi_t_ = true; return *this; }
   // BfvParametersBuilder::build_arc (bfv/parameters.rs:555)
   std::shared_ptr<BfvParameters> build_arc() const {
-    uint8_t pt[8];
-    for (int i = 0; i < 8; i++) pt[i] = (uint8_t)(plaintext_ >> (8 * i));
+    std::vector<uint8_t> t_le = plaintext_;
+    while (t_le.size() > 1 && !t_le.back()) t_le.pop_back();
+    const uint8_t* pt = t_le.data();
     fhe_b200_params* h = nullptr;
     if (variance_ < 1 || variance_ > 32) throw Error(FHE_B200_INVALID_ARGUMENT, "InvalidVariance");
     if (!moduli_.empty() && !sizes_.empty())
       throw Error(FHE_B200_INVALID_ARGUMENT, "ConflictingCiphertextModulusSpecifications");
     if (!moduli_.empty())
-      check(fhe_b200_params_create(device_, degree_, moduli_.data(), (uint32_t)moduli_.size(), pt, 8,
+      check(fhe_b200_params_create(device_, degree_, moduli_.data(), (uint32_t)moduli_.size(), pt, (uint32_t)t_le.size(),
                                    psi_.empty() ? nullptr : psi_.data(), &h));
     else
-      check(fhe_b200_params_create_from_sizes(device_, degree_, sizes_.data(), (uint32_t)sizes_.size(), pt, 8, &h));
-    return std::shared_ptr<BfvParameters>(new BfvParameters(h, has_psi_t_, psi_t_, variance_));
+      check(fhe_b200_params_create_from_sizes(device_, degree_, sizes_.data(), (uint32_t)sizes_.size(), pt,
+                                              (uint32_t)t_le.size(), &h));
+    return std::shared_ptr<BfvParameters>(new BfvParameters(h, has_psi_t_, psi_t_, variance_, std::move(t_le)));
   }
 
  private:
   uint32_t degree_ = 0;
-  uint64_t plaintext_ = 0;
+  std::vector<uint8_t> plaintext_ = std::vector<uint8_t>(8, 0);
   uint64_t psi_t_ = 0;
   bool has_psi_t_ = false;
   uint32_t variance_ = 10;
@@ -432,6 +443,22 @@ class SecretKey {
   }
   SecretKey(const SecretKey&) = delete;
   SecretKey& operator=(const SecretKey&) = delete;
+  // SecretKey::random (secret_key.rs:42-45): s = sample_vec_cbd(N, par.variance()) drawn on the device from the
+  // stream of fhe_b200.h (role 18, key 0).  seed: 32 bytes (nullptr: fresh getrandom bytes).
+  static std::unique_ptr<SecretKey> random(const std::shared_ptr<BfvParameters>& par, const uint8_t* seed = nullptr) {
+    return std::move(random_vec(par, 1, seed)[0]);
+  }
+  // n independent SecretKey::random keys in one device call (key k is stream word 13 = k), e.g. one per party of
+  // multiparty BFV.  Their coefficients stay on the device: coeffs() is empty and to_bytes downloads them.
+  static inline std::vector<std::unique_ptr<SecretKey>> random_vec(const std::shared_ptr<BfvParameters>& par, uint32_t n,
+                                                                   const uint8_t* seed = nullptr);
+  // the N signed coefficients (fhe_b200_secret_key_coeffs for a device-born key); the caller erases them
+  std::vector<int64_t> download_coeffs() const {
+    if (!coeffs_.empty()) return coeffs_;
+    std::vector<int64_t> c(par_->degree());
+    check(fhe_b200_secret_key_coeffs(h_, c.data(), nullptr));
+    return c;
+  }
   ~SecretKey() {
     fhe_b200_secret_key_free(h_);
     volatile int64_t* c = coeffs_.data();
@@ -462,11 +489,12 @@ class SecretKey {
   // SecretKey::try_encrypt into RGSWCiphertext (rgsw_ciphertext.rs:94-120) of every plaintext of pts, at their level,
   // in one device call; seed as for try_encrypt
   inline std::vector<RGSWCiphertext> try_encrypt_rgsw(const PlaintextVec& pts, const uint8_t* seed = nullptr) const;
-  const std::vector<int64_t>& coeffs() const { return coeffs_; }
+  const std::vector<int64_t>& coeffs() const { return coeffs_; }   // empty for a device-born key
   const std::shared_ptr<BfvParameters>& par() const { return par_; }
   const fhe_b200_secret_key* handle() const { return h_; }
 
  private:
+  SecretKey(std::shared_ptr<BfvParameters> par, fhe_b200_secret_key* h) : par_(std::move(par)), h_(h) {}
   Ciphertext encrypt_into(const Ciphertext* pts, uint32_t count, uint32_t level, const uint8_t* seed, void* stream) const;
   std::shared_ptr<BfvParameters> par_;
   std::vector<int64_t> coeffs_;
@@ -485,6 +513,16 @@ struct EncryptionSeed {
     }
   }
 };
+
+inline std::vector<std::unique_ptr<SecretKey>> SecretKey::random_vec(const std::shared_ptr<BfvParameters>& par,
+                                                                    uint32_t n, const uint8_t* seed) {
+  const EncryptionSeed s(seed);
+  std::vector<fhe_b200_secret_key*> hs(std::max<uint32_t>(1, n), nullptr);
+  check(fhe_b200_secret_keys_random(par->handle(), n, par->variance(), s.bytes, hs.data(), nullptr));
+  std::vector<std::unique_ptr<SecretKey>> out;
+  for (uint32_t k = 0; k < n; k++) out.emplace_back(new SecretKey(par, hs[k]));
+  return out;
+}
 
 inline Ciphertext SecretKey::encrypt_into(const Ciphertext* pts, uint32_t count, uint32_t level, const uint8_t* seed,
                                           void* stream) const {

@@ -9,11 +9,12 @@
 //                                 :494-550)
 //   fhers.bfv.SecretKey           bfv.proto:54-56,                   fhe/src/bfv/keys/secret_key.rs:142-175
 //   fhers.bfv.PublicKey           bfv.proto:50-52,                   fhe/src/bfv/keys/public_key.rs:95-149
+//   fhers.bfv.Parameters          bfv.proto:40-48,                   fhe/src/bfv/parameters.rs:741-789
 // `Rq.coefficients` -- the bit-packed power-basis words, all but a few bytes of every message -- is produced and consumed
 // on the device (fhe_b200_batch_pack / fhe_b200_batch_unpack); this header is the proto3 framing around it, emitting
-// what prost emits (fields in field-number order, zero scalars and empty singular `bytes` omitted) and accepting what
-// prost accepts (any order, unknown fields skipped, last scalar wins), plus the checks of the reference's decoders
-// under the reference's variant names (WireError::variant).  The Python mirror's fhe_rs_b200/wire.py is the same
+// what prost emits (fields in field-number order, a oneof at its lowest field number, zero scalars and empty singular
+// `bytes` omitted) and accepting what prost accepts (any order, unknown fields skipped, last scalar wins), plus the
+// checks of the reference's decoders under the reference's variant names (WireError::variant).  The Python mirror's fhe_rs_b200/wire.py is the same
 // codec; both are tested byte for byte against the google.protobuf runtime.
 //
 // Seeded messages carry a 32-byte ChaCha8 seed instead of their last polynomial (row c1 for keys).  Expanding it is
@@ -322,6 +323,84 @@ inline std::vector<int64_t> decode_secret_key(const void* data, size_t n, size_t
   return c;
 }
 
+// ---- Parameters (bfv.proto:40-48) ---------------------------------------------------------------------------------
+// degree = 1 (uint32), moduli = 2 (repeated uint64, packed), the oneof plaintext_modulus { plaintext = 3 (uint64),
+// plaintext_big = 5 (bytes, little-endian) }, variance = 4 (uint32)
+struct ParametersMsg {
+  uint32_t degree = 0, variance = 0;
+  std::vector<uint64_t> moduli;
+  bool has_plaintext = false;           // a member of the oneof was present
+  std::vector<uint8_t> plaintext_le;    // the plaintext modulus, little-endian (either member)
+};
+// true when t (little-endian) is a zq::Modulus, 2 <= t < 2^62: where PlaintextModulus::as_u64 is Some
+inline bool plaintext_is_small(const std::vector<uint8_t>& t_le, uint64_t* t = nullptr) {
+  size_t n = t_le.size();
+  while (n && !t_le[n - 1]) n--;
+  if (n > 8) return false;
+  uint64_t v = 0;
+  for (size_t i = 0; i < n; i++) v |= (uint64_t)t_le[i] << (8 * i);
+  if (t) *t = v;
+  return v >= 2 && v < (1ull << 62);
+}
+// BfvParameters::to_bytes (parameters.rs:741-759).  prost writes a oneof at the position of its lowest field number,
+// so plaintext_big (5) goes before variance (4), as plaintext (3) does.
+inline std::string encode_parameters(uint32_t degree, const std::vector<uint64_t>& moduli,
+                                     const std::vector<uint8_t>& plaintext_le, uint32_t variance) {
+  std::string out, packed;
+  put_uint(out, 1, degree);
+  for (uint64_t q : moduli) put_varint(packed, q);
+  if (!moduli.empty()) put_len(out, 2, packed);
+  uint64_t t = 0;
+  if (plaintext_is_small(plaintext_le, &t)) {
+    put_varint(out, 3 << 3);   // a set oneof member is written even when it is zero
+    put_varint(out, t);
+  } else {
+    size_t n = plaintext_le.size();
+    while (n > 1 && !plaintext_le[n - 1]) n--;   // BigUint::to_bytes_le: no trailing zeros, one byte for zero
+    const uint8_t zero = 0;
+    put_len(out, 5, n ? plaintext_le.data() : &zero, n ? n : 1);
+  }
+  put_uint(out, 4, variance);
+  return out;
+}
+// the fields of a Parameters message (parameters.rs:762-781): packed and unpacked moduli are both accepted, the last
+// oneof member wins, malformed bytes are Decode and a missing oneof is MissingField (ParametersPlaintextModulus)
+inline ParametersMsg decode_parameters(const void* data, size_t n) {
+  ParametersMsg m;
+  Reader r(data, n);
+  while (r.next()) {
+    if (r.field == 1) { r.expect(0); m.degree = (uint32_t)r.value; }
+    else if (r.field == 4) { r.expect(0); m.variance = (uint32_t)r.value; }
+    else if (r.field == 3) {
+      r.expect(0);
+      m.has_plaintext = true;
+      m.plaintext_le.clear();
+      for (int i = 0; i < 8; i++) m.plaintext_le.push_back((uint8_t)(r.value >> (8 * i)));
+    } else if (r.field == 5) {
+      r.expect(2);
+      m.has_plaintext = true;
+      m.plaintext_le.assign(r.span.p, r.span.p + r.span.n);
+    } else if (r.field == 2) {
+      if (r.wire_type == 0) { m.moduli.push_back(r.value); continue; }
+      r.expect(2);
+      const uint8_t *p = r.span.p, *end = r.span.p + r.span.n;
+      while (p < end) {
+        uint64_t v = 0;
+        for (int shift = 0;; shift += 7) {
+          if (p >= end) throw WireError("Decode", FHE_B200_INVALID_ARGUMENT, "truncated varint");
+          const uint8_t b = *p++;
+          if (shift == 63 && b > 1) throw WireError("Decode", FHE_B200_INVALID_ARGUMENT, "varint overflows 64 bits");
+          v |= (uint64_t)(b & 0x7f) << shift;
+          if (!(b & 0x80)) break;
+        }
+        m.moduli.push_back(v);
+      }
+    }
+  }
+  if (!m.has_plaintext) throw WireError("MissingField", FHE_B200_INVALID_ARGUMENT, "ParametersPlaintextModulus");
+  return m;
+}
+
 inline std::string encode_public_key(const std::string& ciphertext) {   // public_key.rs:95-107, bfv.proto:50-52
   std::string out;
   put_len(out, 1, ciphertext);
@@ -536,7 +615,14 @@ inline EvaluationKey evaluation_key_from_bytes(std::shared_ptr<BfvParameters> pa
 }
 
 // SecretKey::to_bytes / from_bytes (secret_key.rs:142-175)
-inline std::string to_bytes(const SecretKey& sk) { return wire::encode_secret_key(sk.coeffs().data(), sk.coeffs().size()); }
+// A device-born key's coefficients come from fhe_b200_secret_key_coeffs and are erased once encoded.
+inline std::string to_bytes(const SecretKey& sk) {
+  std::vector<int64_t> c = sk.download_coeffs();
+  std::string msg = wire::encode_secret_key(c.data(), c.size());
+  volatile int64_t* w = c.data();
+  for (size_t i = 0; i < c.size(); i++) w[i] = 0;
+  return msg;
+}
 inline std::unique_ptr<SecretKey> secret_key_from_bytes(std::shared_ptr<BfvParameters> par, const std::string& data) {
   std::vector<int64_t> c = wire::decode_secret_key(data.data(), data.size(), par->degree());
   std::unique_ptr<SecretKey> sk(new SecretKey(std::move(par), c));
@@ -559,6 +645,22 @@ inline PublicKey public_key_from_bytes(std::shared_ptr<BfvParameters> par, const
     throw WireError("SeedExpansion", FHE_B200_UNSUPPORTED, "pass the host-expanded c1 (ciphertext.rs:287-300)");
   Ciphertext c = ciphertext_from_bytes(par, {std::string((const char*)s.p, s.n)}, seeded_c1);
   return PublicKey(std::move(par), std::move(c));
+}
+
+// BfvParameters::to_bytes / try_deserialize (parameters.rs:741-789).  The decoder builds through BfvParametersBuilder
+// with explicit moduli and the decoded variance, so every builder error keeps its code (variance 0 is InvalidVariance).
+inline std::string parameters_to_bytes(const BfvParameters& par) {
+  return wire::encode_parameters((uint32_t)par.degree(), par.moduli(), par.plaintext_le(), par.variance());
+}
+inline std::shared_ptr<BfvParameters> parameters_from_bytes(const std::string& data, int device = 0) {
+  const wire::ParametersMsg m = wire::decode_parameters(data.data(), data.size());
+  return BfvParametersBuilder()
+      .set_degree(m.degree)
+      .set_moduli(m.moduli)
+      .set_plaintext_modulus_le(m.plaintext_le)
+      .set_variance(m.variance)
+      .set_device(device)
+      .build_arc();
 }
 
 }  // namespace bfv
