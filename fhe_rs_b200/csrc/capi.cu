@@ -1478,7 +1478,8 @@ int fhe_b200_measure_noise(const fhe_b200_secret_key* sk, const fhe_b200_batch* 
   check_secret_input(sk, ct);
   REQUIRE(noise_bits, FHE_B200_INVALID_ARGUMENT, "null argument");
   const fhe_b200_params* par = sk->par;
-  REQUIRE(par->t_mod.t < par->moduli[0], FHE_B200_UNSUPPORTED, "to_poly needs t below the first ciphertext modulus");
+  REQUIRE(par->t_small && par->t_mod.t < par->moduli[0], FHE_B200_UNSUPPORTED,
+          "to_poly needs t below the first ciphertext modulus");
   DeviceGuard g(par);
   const LevelData& lv = par->level(ct->level);
   const u32 L = lv.L, logn = par->logn;
@@ -2913,7 +2914,8 @@ int fhe_b200_debug_scaler_tables(const fhe_b200_params* p, uint32_t level, int w
   API_BEGIN
   REQUIRE(p, FHE_B200_INVALID_ARGUMENT, "null argument");
   const LevelData& lv = p->level(level);
-  const ScalerTablesH& h = which ? lv.down.h : lv.ext.h;
+  REQUIRE(which >= 0 && which <= 2, FHE_B200_INVALID_ARGUMENT, "which must be 0, 1 or 2");
+  const ScalerTablesH& h = which == 0 ? lv.ext.h : which == 1 ? lv.down.h : lv.plain.h;
   if (n_from) *n_from = h.n_from;
   if (n_to) *n_to = h.n_to;
   if (shift) *shift = h.shift;

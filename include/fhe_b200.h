@@ -544,8 +544,10 @@ int fhe_b200_sync(void* stream);
 uint64_t fhe_b200_launch_count(void);
 
 /* ---- inspection of the host precompute (CPU-only tests of the parameter builder) -------
- * RnsScaler tables (rns/scaler.rs:52-73) of the level's extender (which=0) / down scaler
- * (which=1).  Any output pointer may be NULL.  omega is [n_to][n_from]. */
+ * RnsScaler tables (rns/scaler.rs:52-73) of the level's extender (which=0), down scaler
+ * (which=1) or decryption scaler t / Q_l into the plaintext context (which=2, parameters.rs:638-643;
+ * its n_to is the plaintext context's modulus count).  Any output pointer may be NULL.
+ * omega is [n_to][n_from]. */
 int fhe_b200_debug_scaler_tables(const fhe_b200_params* p, uint32_t level, int which, uint32_t* n_from,
                                  uint32_t* n_to, uint32_t* shift, uint64_t* gamma, uint64_t* omega,
                                  uint64_t* theta_gamma /* lo,hi,sign */, uint64_t* theta_omega_lo,
