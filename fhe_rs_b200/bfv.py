@@ -24,7 +24,9 @@ from .wire import WireError
 __all__ = ["BfvParameters", "BfvParametersBuilder", "Ciphertext", "KeySwitchingKey", "RelinearizationKey", "RGSWCiphertext",
            "GaloisKey", "EvaluationKey", "Multiplicator", "ScalingFactor", "dot_product_scalar", "FheError", "WireError", "NTT", "POWER_BASIS",
            "Encoding", "Plaintext", "PlaintextVec", "SecretKey", "PublicKey", "EvaluationKeyBuilder",
-           "transcode_bidirectional", "transcode_to_bytes", "transcode_from_bytes"]
+           "transcode_bidirectional", "transcode_to_bytes", "transcode_from_bytes", "key_switch_keyed",
+           "relinearizes_keyed", "multiply_keyed", "galois_keyed", "rotates_columns_by_keyed", "rotates_rows_keyed",
+           "expands_keyed", "expands_batch_keyed", "external_products_keyed"]
 
 
 def _release(free_name: str, handle) -> None:
@@ -1452,3 +1454,111 @@ class Multiplicator:
         check(_capi.lib().fhe_b200_multiplicator_multiply(
             self._h, lhs._h, rhs._h, self.rk.ksk._h if self.rk is not None else None, ms, out._h, lhs.stream))
         return out
+
+
+# ---- per-ciphertext keys: one batch, one key per ciphertext (a server answering many clients).  `index[j]` names the
+# key of ciphertext j (for expands_keyed: of query j); output j is what the single-key method gives on ciphertext j
+# with that key.  One device call each (the fhe_b200_*_keyed entry points of include/fhe_b200.h).
+
+def _keyed_args(ksks: Sequence["KeySwitchingKey"], index, count: int):
+    idx = np.ascontiguousarray(np.asarray(index, dtype=np.int64).reshape(-1))
+    if idx.size != count:
+        raise FheError(_capi.INVALID_ARGUMENT, "expected one key index per ciphertext (%d), got %d" % (count, idx.size))
+    if idx.size and (idx.min() < 0 or idx.max() > 0xFFFFFFFF):
+        raise FheError(_capi.INVALID_ARGUMENT, "key index out of range")
+    hs = (C.c_void_p * max(1, len(ksks)))(*[k._h.value for k in ksks])
+    ix = (C.c_uint32 * max(1, idx.size))(*[int(v) for v in idx])
+    return C.cast(hs, C.POINTER(C.c_void_p)), len(ksks), ix
+
+
+def key_switch_keyed(p: Ciphertext, part: int, ksks: Sequence["KeySwitchingKey"], index) -> Ciphertext:
+    """KeySwitchingKey.key_switch of ciphertext j of `p` with ksks[index[j]]"""
+    args = _keyed_args(ksks, index, p.count)
+    out = Ciphertext(p.par, p.count, 2, ksks[0].ksk_level if ksks else p.level, NTT, p.stream)
+    check(_capi.lib().fhe_b200_key_switch_keyed(p._h, part, *args, out._h, p.stream))
+    return out
+
+
+def relinearizes_keyed(ct: Ciphertext, rks: Sequence["RelinearizationKey"], index) -> Ciphertext:
+    """RelinearizationKey.relinearizes of ciphertext j with rks[index[j]]"""
+    args = _keyed_args([rk.ksk for rk in rks], index, ct.count)
+    out = ct._like(parts=2)
+    check(_capi.lib().fhe_b200_relinearize_keyed(ct._h, *args, out._h, ct.stream))
+    return out
+
+
+def multiply_keyed(lhs: Ciphertext, rhs: Ciphertext, rks: Sequence["RelinearizationKey"], index,
+                   mod_switch: bool = False) -> Ciphertext:
+    """Multiplicator.default(rks[index[j]]).multiply of the pair j (with enable_mod_switching when mod_switch)"""
+    ms = 1 if mod_switch else 0
+    args = _keyed_args([rk.ksk for rk in rks], index, lhs.count)
+    out = lhs._like(parts=2, level=lhs.level + ms)
+    check(_capi.lib().fhe_b200_mul_relin_keyed(lhs._h, rhs._h, *args, ms, out._h, lhs.stream))
+    return out
+
+
+def galois_keyed(ct: Ciphertext, gks: Sequence["GaloisKey"], index) -> Ciphertext:
+    """GaloisKey.relinearize of ciphertext j with gks[index[j]]; every key must be for the same exponent"""
+    if gks and any(g.exponent != gks[0].exponent for g in gks):
+        raise FheError(_capi.INVALID_ARGUMENT, "the Galois keys of one call must share their exponent")
+    args = _keyed_args([g.ksk for g in gks], index, ct.count)
+    out = ct._like()
+    check(_capi.lib().fhe_b200_galois_keyed(ct._h, gks[0].exponent if gks else 1, *args, out._h, ct.stream))
+    return out
+
+
+def _galois_of(eks: Sequence["EvaluationKey"], exponent: int, what: str) -> "List[GaloisKey]":
+    for ek in eks:
+        if exponent % (2 * ek.par.degree()) not in ek.gk:
+            raise FheError(_capi.INVALID_ARGUMENT, "EvaluationKeyError: %s not supported by this key" % what)
+    return [ek.gk[exponent % (2 * ek.par.degree())] for ek in eks]
+
+
+def rotates_columns_by_keyed(ct: Ciphertext, eks: Sequence["EvaluationKey"], index, i: int) -> Ciphertext:
+    """EvaluationKey.rotates_columns_by(ct_j, i) with eks[index[j]] (evaluation_key.rs:145-170)"""
+    return galois_keyed(ct, _galois_of(eks, pow(3, i, 2 * ct.par.degree()), "column rotation"), index)
+
+
+def rotates_rows_keyed(ct: Ciphertext, eks: Sequence["EvaluationKey"], index) -> Ciphertext:
+    """EvaluationKey.rotates_rows(ct_j) with eks[index[j]] (evaluation_key.rs:110-126)"""
+    return galois_keyed(ct, _galois_of(eks, 2 * ct.par.degree() - 1, "row rotation"), index)
+
+
+def expands_keyed(ct: Ciphertext, eks: Sequence["EvaluationKey"], index, size: int) -> "List[Ciphertext]":
+    """EvaluationKey.expands of query q of `ct` with eks[index[q]]: a list of `size` batches, batch i holding output i
+    of every query (as EvaluationKey.expands)"""
+    whole = expands_batch_keyed(ct, eks, index, size)
+    q = ct.count
+    return [whole.take(i * q, q) for i in range(size)]
+
+
+def expands_batch_keyed(ct: Ciphertext, eks: Sequence["EvaluationKey"], index, size: int) -> Ciphertext:
+    """expands_keyed as one batch of size * Q: entry i*Q + q is output i of query q (as EvaluationKey.expands_batch)"""
+    n = ct.par.degree()
+    if size == 0 or size > n:
+        raise FheError(_capi.INVALID_ARGUMENT, "EvaluationKeyError: invalid expansion size")
+    level = max(0, (size - 1).bit_length())
+    hs = []
+    for ek in eks:
+        for l in range(level):
+            gk = ek.gk.get((n >> l) + 1)
+            hs.append(gk.ksk._h.value if gk is not None else None)
+    keys, _, ix = _keyed_args([], index, ct.count)
+    arr = (C.c_void_p * max(1, len(hs)))(*hs)
+    out = Ciphertext(ct.par, size * ct.count, 2, ct.level, NTT, ct.stream)
+    check(_capi.lib().fhe_b200_expand_keyed(ct._h, size, C.cast(arr, C.POINTER(C.c_void_p)), level, len(eks), ix,
+                                            out._h, ct.stream))
+    return out
+
+
+def external_products_keyed(cts: Ciphertext, rgsws: Sequence["RGSWCiphertext"], index) -> Ciphertext:
+    """&cts[j] * &rgsws[index[j]] (rgsw_ciphertext.rs:122-155): two keyed key switches and an add, as
+    RGSWCiphertext.external_product composes them"""
+    if any(r.ksk0.ciphertext_level != cts.level for r in rgsws):
+        raise FheError(_capi.INVALID_LEVEL, "Ciphertext and RGSWCiphertext must have the same level")
+    if len(cts) != 2:
+        raise FheError(_capi.BAD_POLY_COUNT, "Ciphertext must have two parts")
+    pb = cts.clone().into_power_basis()
+    out = key_switch_keyed(pb, 0, [r.ksk0 for r in rgsws], index)
+    out += key_switch_keyed(pb, 1, [r.ksk1 for r in rgsws], index)
+    return out

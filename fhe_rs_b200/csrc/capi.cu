@@ -601,10 +601,54 @@ void switch_down_polys(const fhe_b200_params* par, u32 level, u64* d, u32 polys,
   launch_ntt(tmp, d, polys * nl.L, nl.ctx_ids, par->d_limbs, par->logn, false, 1, false, st);
 }
 
+// The keys of a key switch: ciphertext c of the call uses keys[index[c]], or keys[0] when index is null (the
+// single-key entry points).  Every key has the levels, digit count and base of keys[0] (check_keys).
+struct KeySet {
+  const fhe_b200_ksk* const* keys;
+  u32 n;
+  const u32* index;   // host memory, one entry per ciphertext; nullable
+  // the same keys for the ciphertexts from c0 on
+  KeySet from(u32 c0) const { return {keys, n, index ? index + c0 : nullptr}; }
+};
+
+// The inner-product launches of `cts` ciphertexts: consecutive ranges of at most kKeyPairs distinct keys (a handle
+// listed twice is one key) and, once a range holds two keys, at most kKeySlots ciphertexts.  One key: one range.
+std::vector<KeyRange> key_ranges(const KeySet& K, u32 cts) {
+  std::vector<KeyRange> out;
+  KeyRange* r = nullptr;
+  for (u32 c = 0; c < cts; c++) {
+    const fhe_b200_ksk* k = K.keys[K.index ? K.index[c] : 0];
+    u32 s = 0;
+    if (r) {
+      while (s < r->keys.n && r->keys.k0[s] != k->k0) s++;
+      const u32 n_after = r->keys.n + (s == r->keys.n);
+      if (n_after > kKeyPairs || (n_after > 1 && r->cts >= kKeySlots)) r = nullptr;
+    }
+    if (!r) {
+      out.emplace_back();
+      r = &out.back();
+      std::memset(r, 0, sizeof(KeyRange));
+      r->ct0 = c;
+      s = 0;
+    }
+    if (s == r->keys.n) {
+      r->keys.k0[s] = k->k0;
+      r->keys.k1[s] = k->k1;
+      r->keys.n++;
+    }
+    if (r->cts < kKeySlots) r->keys.slot[r->cts] = (unsigned char)s;
+    r->cts++;
+  }
+  return out;
+}
+
 // KeySwitchingKey::key_switch core on a contiguous power-basis buffer c2 [cts][L][N]
-// (key_switching_key.rs:241-270): out0/out1 (+ optional bases), rows (ct, j) at (ct*out_ct_rows + j).
-void key_switch_core(const fhe_b200_params* par, const fhe_b200_ksk* k, const u64* c2, u32 cts, const u64* base0,
+// (key_switching_key.rs:241-270): out0/out1 (+ optional bases), rows (ct, j) at (ct*out_ct_rows + j).  The digit
+// transforms do not depend on the key; the inner product runs once per key range (key_ranges).
+void key_switch_core(const fhe_b200_params* par, const KeySet& K, const u64* c2, u32 cts, const u64* base0,
                      const u64* base1, u64* out0, u64* out1, u32 out_ct_rows, Workspace& ws, cudaStream_t st) {
+  const fhe_b200_ksk* k = K.keys[0];
+  const std::vector<KeyRange> ranges = key_ranges(K, cts);
   const LevelData& kl = par->level(k->ksk_level);
   const u32 L = k->n_dig, Lk = k->Lk;
   u64* inter = ws.words(((size_t)cts * L * Lk) << par->logn);
@@ -634,13 +678,13 @@ void key_switch_core(const fhe_b200_params* par, const fhe_b200_ksk* k, const u6
   // never go through HBM.  FHE_B200_KSMAC=tma keeps the unfused TMA chain (rows pass, then ksmac_tma_kernel),
   // =classic the per-thread inner product.
   if (adjacent && switches().ksmac == Switches::KSMAC_FUSED &&
-      launch_key_switch_tma(c2, inter, k->k0, k->k1, base0, base1, out0, out1, cts, L, Lk, out_ct_rows, kl.ctx_ids,
+      launch_key_switch_tma(c2, inter, ranges, base0, base1, out0, out1, cts, L, Lk, out_ct_rows, kl.ctx_ids,
                             par->d_limbs, par->logn, reduce, st))
     return;
   launch_ntt(c2, inter, cts * L * Lk, kl.ctx_ids, par->d_limbs, par->logn, false, Lk, reduce, st, true, adjacent, L);
   }
-  launch_ksmac(inter, k->k0, k->k1, base0, base1, out0, out1, cts, L, Lk, out_ct_rows, kl.ctx_ids, par->d_limbs,
-               par->logn, st, adjacent);
+  launch_ksmac(inter, ranges, base0, base1, out0, out1, L, Lk, out_ct_rows, kl.ctx_ids, par->d_limbs, par->logn, st,
+               adjacent);
 }
 
 // key switch + the reference's post-processing (relinearization_key.rs:88-95, galois_key.rs:69-76):
@@ -648,19 +692,20 @@ void key_switch_core(const fhe_b200_params* par, const fhe_b200_ksk* k, const u6
 // taken to power basis, switched down to the ciphertext context and transformed back before it is added.
 // c2: [cts][L][N] power basis at the ciphertext level; out: [cts][2][L][N]; base (nullable) is added:
 // base_mode 0: none, 1: out += result (in place), 2: out = result + (base part 0 only; base is [cts][2][L][N])
-void key_switch_apply(const fhe_b200_params* par, const fhe_b200_ksk* k, const u64* c2, u32 cts, u64* out,
+void key_switch_apply(const fhe_b200_params* par, const KeySet& K, const u64* c2, u32 cts, u64* out,
                       int base_mode, u64* base, Workspace& ws, cudaStream_t st) {
+  const fhe_b200_ksk* k = K.keys[0];
   const LevelData& cl = par->level(k->ct_level);
   const u32 L = cl.L, Lk = k->Lk, logn = par->logn;
   const size_t row = (size_t)1 << logn;
   if (Lk == L) {
     const u64* b0 = base_mode == 1 ? out : base_mode == 2 ? base : nullptr;
     const u64* b1 = base_mode == 1 ? out + L * row : nullptr;
-    key_switch_core(par, k, c2, cts, b0, b1, out, out + L * row, 2 * L, ws, st);
+    key_switch_core(par, K, c2, cts, b0, b1, out, out + L * row, 2 * L, ws, st);
     return;
   }
   u64* cur = ws.words((size_t)cts * 2 * Lk * row);
-  key_switch_core(par, k, c2, cts, nullptr, nullptr, cur, cur + Lk * row, 2 * Lk, ws, st);
+  key_switch_core(par, K, c2, cts, nullptr, nullptr, cur, cur + Lk * row, 2 * Lk, ws, st);
   const LevelData& kl = par->level(k->ksk_level);
   launch_ntt(cur, cur, cts * 2 * Lk, kl.ctx_ids, par->d_limbs, logn, true, 1, false, st);
   for (u32 lv = k->ksk_level; lv < k->ct_level; lv++) {  // Poly::switch_down_to, rq/mod.rs:498-507
@@ -684,7 +729,7 @@ void key_switch_apply(const fhe_b200_params* par, const fhe_b200_ksk* k, const u
 
 // GaloisKey::relinearize (galois_key.rs:63-86) of n 2-part NTT ciphertexts [n][2][L][N] at `src` into `dst` (same
 // layout), on one stream: the chunk body of fhe_b200_galois and of every level of fhe_b200_expand.
-void galois_range(const fhe_b200_params* par, const LevelData& lv, const int* perm, const fhe_b200_ksk* gk,
+void galois_range(const fhe_b200_params* par, const LevelData& lv, const int* perm, const KeySet& gk,
                   const u64* src, u64* dst, u32 n, cudaStream_t st) {
   const size_t row = (size_t)1 << par->logn, L = lv.L;
   Workspace ws(par, st);
@@ -2313,15 +2358,40 @@ static void check_ksk(const fhe_b200_ksk* k, const fhe_b200_params* par, u32 lev
   REQUIRE(k->ct_level == level, FHE_B200_INVALID_LEVEL, "InvalidLevel: key is for another ciphertext level");
 }
 
-int fhe_b200_relinearize(const fhe_b200_batch* ct3, const fhe_b200_ksk* rk, fhe_b200_batch* out2, void* stream) {
-  API_BEGIN
-  REQUIRE(ct3 && rk && out2, FHE_B200_INVALID_ARGUMENT, "null argument");
+// a keyed call's key list and index: present, non-empty, no NULL key
+static KeySet key_list(const fhe_b200_ksk* const* keys, u32 n_keys, const u32* index) {
+  REQUIRE(keys && n_keys && index, FHE_B200_INVALID_ARGUMENT, "null key list or index, or no keys");
+  for (u32 i = 0; i < n_keys; i++) REQUIRE(keys[i], FHE_B200_INVALID_ARGUMENT, "null key");
+  return {keys, n_keys, index};
+}
+
+// what a key switch over several keys needs beyond each key's own checks: one key level, digit count and base for
+// every key, and every index of the `count` ciphertexts naming a key
+static void check_key_set(const KeySet& K, u32 count) {
+  const fhe_b200_ksk* k0 = K.keys[0];
+  for (u32 i = 1; i < K.n; i++)
+    REQUIRE(K.keys[i]->ksk_level == k0->ksk_level && K.keys[i]->n_dig == k0->n_dig &&
+                K.keys[i]->log_base == k0->log_base,
+            FHE_B200_INVALID_ARGUMENT, "keys of one call differ in key level, digit count or base");
+  if (K.index)
+    for (u32 c = 0; c < count; c++)
+      REQUIRE(K.index[c] < K.n, FHE_B200_INVALID_ARGUMENT, "key index " + std::to_string(K.index[c]) + " of ciphertext " +
+                                                               std::to_string(c) + " beyond the key list");
+}
+
+static void check_ksks(const KeySet& K, const fhe_b200_params* par, u32 level, u32 count) {
+  for (u32 i = 0; i < K.n; i++) check_ksk(K.keys[i], par, level);
+  check_key_set(K, count);
+}
+
+static void relinearize_run(const fhe_b200_batch* ct3, const KeySet& rk, fhe_b200_batch* out2, void* stream) {
+  REQUIRE(ct3 && rk.keys[0] && out2, FHE_B200_INVALID_ARGUMENT, "null argument");
   check_same(ct3, out2);
   REQUIRE(!ct3->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
   REQUIRE(ct3->parts == 3 && out2->parts == 2, FHE_B200_BAD_POLY_COUNT, "InvalidPolynomialCount: expected 3 -> 2");
   REQUIRE(ct3->count == out2->count, FHE_B200_INVALID_ARGUMENT, "batch sizes differ");
   need_repr(ct3, FHE_B200_NTT);
-  check_ksk(rk, ct3->par, ct3->level);
+  check_ksks(rk, ct3->par, ct3->level, ct3->count);
   DeviceGuard g(ct3->par);
   cudaStream_t st_user = (cudaStream_t)stream;
   const fhe_b200_params* par = ct3->par;
@@ -2337,17 +2407,28 @@ int fhe_b200_relinearize(const fhe_b200_batch* ct3, const fhe_b200_ksk* rk, fhe_
     FHE_CUDA(cudaMemcpy2DAsync(c2, L * row * 8, src + 2 * L * row, 3 * L * row * 8, L * row * 8, n, cudaMemcpyDeviceToDevice, st));
     // relinearization_key.rs:85: c2 -> power basis
     launch_ntt(c2, c2, n * (u32)L, lv.ctx_ids, par->d_limbs, par->logn, true, 1, false, st);
-    key_switch_apply(par, rk, c2, n, dst, 1, nullptr, ws, st);
+    key_switch_apply(par, rk.from(c0), c2, n, dst, 1, nullptr, ws, st);
   });
   FHE_CUDA(cudaGetLastError());
   out2->repr = FHE_B200_NTT;
+}
+
+int fhe_b200_relinearize(const fhe_b200_batch* ct3, const fhe_b200_ksk* rk, fhe_b200_batch* out2, void* stream) {
+  API_BEGIN
+  relinearize_run(ct3, {&rk, 1, nullptr}, out2, stream);
   API_END
 }
 
-int fhe_b200_mul_relin(const fhe_b200_batch* a, const fhe_b200_batch* b, const fhe_b200_ksk* rk, int mod_switch,
-                       fhe_b200_batch* out2, void* stream) {
+int fhe_b200_relinearize_keyed(const fhe_b200_batch* ct3, const fhe_b200_ksk* const* rks, uint32_t n_keys,
+                               const uint32_t* key_index, fhe_b200_batch* out2, void* stream) {
   API_BEGIN
-  REQUIRE(a && b && rk && out2, FHE_B200_INVALID_ARGUMENT, "null argument");
+  relinearize_run(ct3, key_list(rks, n_keys, key_index), out2, stream);
+  API_END
+}
+
+static void mul_relin_run(const fhe_b200_batch* a, const fhe_b200_batch* b, const KeySet& rk, int mod_switch,
+                          fhe_b200_batch* out2, void* stream) {
+  REQUIRE(a && b && rk.keys[0] && out2, FHE_B200_INVALID_ARGUMENT, "null argument");
   check_same(a, b);
   REQUIRE(a->par == out2->par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch");
   REQUIRE(!a->mul_basis && !out2->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
@@ -2356,7 +2437,7 @@ int fhe_b200_mul_relin(const fhe_b200_batch* a, const fhe_b200_batch* b, const f
   REQUIRE(a->count == b->count && a->count == out2->count, FHE_B200_INVALID_ARGUMENT, "batch sizes differ");
   need_repr(a, FHE_B200_NTT);
   need_repr(b, FHE_B200_NTT);
-  check_ksk(rk, a->par, a->level);
+  check_ksks(rk, a->par, a->level, a->count);
   const fhe_b200_params* par = a->par;
   const LevelData& lv = par->level(a->level);
   if (mod_switch) {
@@ -2376,7 +2457,7 @@ int fhe_b200_mul_relin(const fhe_b200_batch* a, const fhe_b200_batch* b, const f
     // c0, c1 back to NTT.  c2 stays in power basis: mul.rs:206 + :212 forward- then inverse-transform it,
     // and backward(forward(x)) == x for reduced x (ntt/mod.rs:73-74), so skipping both is bit-exact.
     launch_ntt(o, o, n * 2 * (u32)L, lv.ctx_ids, par->d_limbs, par->logn, false, 1, false, st);
-    key_switch_apply(par, rk, c2, n, o, 1, nullptr, ws, st);
+    key_switch_apply(par, rk.from(c0), c2, n, o, 1, nullptr, ws, st);
     if (mod_switch) {  // Ciphertext::switch_down, ciphertext.rs:148-161
       launch_ntt(o, o, n * 2 * (u32)L, lv.ctx_ids, par->d_limbs, par->logn, true, 1, false, st);
       u64* dst = out2->d + (size_t)c0 * 2 * (L - 1) * row;
@@ -2387,6 +2468,20 @@ int fhe_b200_mul_relin(const fhe_b200_batch* a, const fhe_b200_batch* b, const f
   });
   FHE_CUDA(cudaGetLastError());
   out2->repr = FHE_B200_NTT;
+}
+
+int fhe_b200_mul_relin(const fhe_b200_batch* a, const fhe_b200_batch* b, const fhe_b200_ksk* rk, int mod_switch,
+                       fhe_b200_batch* out2, void* stream) {
+  API_BEGIN
+  mul_relin_run(a, b, {&rk, 1, nullptr}, mod_switch, out2, stream);
+  API_END
+}
+
+int fhe_b200_mul_relin_keyed(const fhe_b200_batch* a, const fhe_b200_batch* b, const fhe_b200_ksk* const* rks,
+                             uint32_t n_keys, const uint32_t* key_index, int mod_switch, fhe_b200_batch* out2,
+                             void* stream) {
+  API_BEGIN
+  mul_relin_run(a, b, key_list(rks, n_keys, key_index), mod_switch, out2, stream);
   API_END
 }
 
@@ -2507,7 +2602,7 @@ int fhe_b200_multiplicator_multiply(const fhe_b200_multiplicator* m, const fhe_b
       FHE_CUDA(cudaMemcpy2DAsync(c2, L * row * 8, W + 2 * L * row, 3 * L * row * 8, L * row * 8, n,
                                  cudaMemcpyDeviceToDevice, st));
       launch_ntt(o, o, n * 2 * (u32)L, lv.ctx_ids, par->d_limbs, par->logn, false, 1, false, st);
-      key_switch_apply(par, rk, c2, n, o, 1, nullptr, ws, st);   // mul.rs:210-228
+      key_switch_apply(par, {&rk, 1, nullptr}, c2, n, o, 1, nullptr, ws, st);   // mul.rs:210-228
     } else {
       launch_ntt(o, o, n * 3 * (u32)L, lv.ctx_ids, par->d_limbs, par->logn, false, 1, false, st);
     }
@@ -2543,16 +2638,15 @@ int fhe_b200_substitute(const fhe_b200_batch* in, uint32_t exponent, fhe_b200_ba
   API_END
 }
 
-int fhe_b200_galois(const fhe_b200_batch* ct, uint32_t exponent, const fhe_b200_ksk* gk, fhe_b200_batch* out,
-                    void* stream) {
-  API_BEGIN
-  REQUIRE(ct && gk && out && ct != out, FHE_B200_INVALID_ARGUMENT, "null or aliased argument");
+static void galois_run(const fhe_b200_batch* ct, uint32_t exponent, const KeySet& gk, fhe_b200_batch* out,
+                       void* stream) {
+  REQUIRE(ct && gk.keys[0] && out && ct != out, FHE_B200_INVALID_ARGUMENT, "null or aliased argument");
   check_same(ct, out);
   REQUIRE(!ct->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
   REQUIRE(ct->parts == 2 && out->parts == 2, FHE_B200_BAD_POLY_COUNT, "InvalidPolynomialCount: expected 2");
   REQUIRE(ct->count == out->count, FHE_B200_INVALID_ARGUMENT, "batch sizes differ");
   need_repr(ct, FHE_B200_NTT);
-  check_ksk(gk, ct->par, ct->level);
+  check_ksks(gk, ct->par, ct->level, ct->count);
   const fhe_b200_params* par = ct->par;
   exponent %= 2 * par->N;
   REQUIRE(exponent & 1, FHE_B200_INVALID_EXPONENT, "InvalidSubstitutionExponent");
@@ -2562,16 +2656,30 @@ int fhe_b200_galois(const fhe_b200_batch* ct, uint32_t exponent, const fhe_b200_
   const int* perm = par->perm(exponent);
   ChunkRunner chunks(par, ct->count, (cudaStream_t)stream);
   chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
-    galois_range(par, lv, perm, gk, ct->d + c0 * W, out->d + c0 * W, n, st);
+    galois_range(par, lv, perm, gk.from(c0), ct->d + c0 * W, out->d + c0 * W, n, st);
   });
   FHE_CUDA(cudaGetLastError());
   out->repr = FHE_B200_NTT;
+}
+
+int fhe_b200_galois(const fhe_b200_batch* ct, uint32_t exponent, const fhe_b200_ksk* gk, fhe_b200_batch* out,
+                    void* stream) {
+  API_BEGIN
+  galois_run(ct, exponent, {&gk, 1, nullptr}, out, stream);
   API_END
 }
 
-int fhe_b200_expand(const fhe_b200_batch* ct, uint32_t size, const fhe_b200_ksk* const* gks, uint32_t n_gks,
-                    fhe_b200_batch* out, void* stream) {
+int fhe_b200_galois_keyed(const fhe_b200_batch* ct, uint32_t exponent, const fhe_b200_ksk* const* gks, uint32_t n_keys,
+                          const uint32_t* key_index, fhe_b200_batch* out, void* stream) {
   API_BEGIN
+  galois_run(ct, exponent, key_list(gks, n_keys, key_index), out, stream);
+  API_END
+}
+
+// gks[s * n_gks + l]: the key of expansion level l of key set s; set_index[q] (nullable: set 0 for every query) the
+// key set of query q
+static void expand_run(const fhe_b200_batch* ct, uint32_t size, const fhe_b200_ksk* const* gks, uint32_t n_gks,
+                       uint32_t n_sets, const uint32_t* set_index, fhe_b200_batch* out, void* stream) {
   REQUIRE(ct && out, FHE_B200_INVALID_ARGUMENT, "null argument");
   const fhe_b200_params* par = ct->par;
   REQUIRE(size > 0 && size <= par->N, FHE_B200_INVALID_ARGUMENT,
@@ -2589,10 +2697,25 @@ int fhe_b200_expand(const fhe_b200_batch* ct, uint32_t size, const fhe_b200_ksk*
   while ((1u << level) < size) level++;
   REQUIRE(n_gks >= level && (level == 0 || gks), FHE_B200_INVALID_ARGUMENT,
           "EvaluationKeyError: Missing GaloisKey: expansion level " + std::to_string(level) + " needs that many keys");
+  if (set_index)
+    for (u32 q = 0; q < Q; q++)
+      REQUIRE(set_index[q] < n_sets, FHE_B200_INVALID_ARGUMENT, "key set index " + std::to_string(set_index[q]) +
+                                                                    " of query " + std::to_string(q) + " beyond the sets");
+  // the keys of level l, one per key set, and the key set of each of its step * Q inputs (entry i*Q + q: query q)
+  std::vector<std::vector<const fhe_b200_ksk*>> keys(level, std::vector<const fhe_b200_ksk*>(n_sets));
+  std::vector<std::vector<u32>> index(set_index ? level : 0);
   for (u32 l = 0; l < level; l++) {
-    REQUIRE(gks[l], FHE_B200_INVALID_ARGUMENT,
-            "EvaluationKeyError: Missing GaloisKey { element: " + std::to_string((par->N >> l) + 1) + " }");
-    check_ksk(gks[l], par, ct->level);
+    for (u32 k = 0; k < n_sets; k++) {
+      keys[l][k] = gks[(size_t)k * n_gks + l];
+      REQUIRE(keys[l][k], FHE_B200_INVALID_ARGUMENT,
+              "EvaluationKeyError: Missing GaloisKey { element: " + std::to_string((par->N >> l) + 1) + " }");
+      check_ksk(keys[l][k], par, ct->level);
+    }
+    check_key_set({keys[l].data(), n_sets, nullptr}, Q);
+    if (set_index) {
+      index[l].resize((size_t)Q << l);
+      for (u32 c = 0; c < index[l].size(); c++) index[l][c] = set_index[c % Q];
+    }
   }
   DeviceGuard g(par);
   cudaStream_t user = (cudaStream_t)stream;
@@ -2616,32 +2739,50 @@ int fhe_b200_expand(const fhe_b200_batch* ct, uint32_t size, const fhe_b200_ksk*
     const u32 step = 1u << l, pairs = step * Q, n_hi = (std::min(2 * step, size) - step) * Q;
     u64* hi = out->d + (size_t)pairs * W;
     ChunkRunner chunks(par, pairs, user);
+    const KeySet K{keys[l].data(), n_sets, set_index ? index[l].data() : nullptr};
     chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
       const u32 e = c0 + n, mid = std::min(std::max(c0, n_hi), e);
-      if (mid > c0) galois_range(par, lv, perms[l], gks[l], out->d + c0 * W, hi + c0 * W, mid - c0, st);
-      if (e > mid) galois_range(par, lv, perms[l], gks[l], out->d + mid * W, spill + (mid - n_hi) * W, e - mid, st);
+      if (mid > c0) galois_range(par, lv, perms[l], K.from(c0), out->d + c0 * W, hi + c0 * W, mid - c0, st);
+      if (e > mid) galois_range(par, lv, perms[l], K.from(mid), out->d + mid * W, spill + (mid - n_hi) * W, e - mid, st);
     });
     launch_expand_butterfly(out->d, hi, spill, pairs, n_hi, monos[l], lv.ctx_ids, par->d_limbs, par->logn, user);
   }
   FHE_CUDA(cudaGetLastError());
   out->repr = FHE_B200_NTT;
+}
+
+int fhe_b200_expand(const fhe_b200_batch* ct, uint32_t size, const fhe_b200_ksk* const* gks, uint32_t n_gks,
+                    fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  expand_run(ct, size, gks, n_gks, 1, nullptr, out, stream);
   API_END
 }
 
-int fhe_b200_key_switch(const fhe_b200_batch* pb, uint32_t part, const fhe_b200_ksk* k, fhe_b200_batch* out2,
-                        void* stream) {
+int fhe_b200_expand_keyed(const fhe_b200_batch* ct, uint32_t size, const fhe_b200_ksk* const* gks, uint32_t n_gks,
+                          uint32_t n_sets, const uint32_t* set_index, fhe_b200_batch* out, void* stream) {
   API_BEGIN
-  REQUIRE(pb && k && out2, FHE_B200_INVALID_ARGUMENT, "null argument");
-  REQUIRE(pb->par == out2->par && pb->par == k->par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch");
+  REQUIRE(n_sets && set_index, FHE_B200_INVALID_ARGUMENT, "null key set index, or no key sets");
+  expand_run(ct, size, gks, n_gks, n_sets, set_index, out, stream);
+  API_END
+}
+
+static void key_switch_run(const fhe_b200_batch* pb, uint32_t part, const KeySet& K, fhe_b200_batch* out2,
+                           void* stream) {
+  REQUIRE(pb && K.keys[0] && out2, FHE_B200_INVALID_ARGUMENT, "null argument");
+  for (u32 i = 0; i < K.n; i++)
+    REQUIRE(pb->par == out2->par && pb->par == K.keys[i]->par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch");
   REQUIRE(!pb->mul_basis && !out2->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
   REQUIRE(part < pb->parts && out2->parts == 2, FHE_B200_BAD_POLY_COUNT, "bad part index / output parts");
-  REQUIRE(pb->level == k->ct_level && out2->level == k->ksk_level, FHE_B200_INVALID_LEVEL, "InvalidLevel");
+  for (u32 i = 0; i < K.n; i++)
+    REQUIRE(pb->level == K.keys[i]->ct_level && out2->level == K.keys[i]->ksk_level, FHE_B200_INVALID_LEVEL,
+            "InvalidLevel");
   REQUIRE(pb->count == out2->count, FHE_B200_INVALID_ARGUMENT, "batch sizes differ");
   need_repr(pb, FHE_B200_POWER_BASIS);
+  check_key_set(K, pb->count);
   const fhe_b200_params* par = pb->par;
   DeviceGuard g(par);
   cudaStream_t st_user = (cudaStream_t)stream;
-  const size_t row = (size_t)1 << par->logn, L = pb->limbs, Lk = k->Lk;
+  const size_t row = (size_t)1 << par->logn, L = pb->limbs, Lk = K.keys[0]->Lk;
   ChunkRunner chunks(par, pb->count, st_user);
   chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
     Workspace ws(par, st);
@@ -2649,10 +2790,23 @@ int fhe_b200_key_switch(const fhe_b200_batch* pb, uint32_t part, const fhe_b200_
     FHE_CUDA(cudaMemcpy2DAsync(c2, L * row * 8, pb->d + ((size_t)c0 * pb->parts + part) * L * row,
                                pb->parts * L * row * 8, L * row * 8, n, cudaMemcpyDeviceToDevice, st));
     u64* dst = out2->d + (size_t)c0 * 2 * Lk * row;
-    key_switch_core(par, k, c2, n, nullptr, nullptr, dst, dst + Lk * row, 2 * (u32)Lk, ws, st);
+    key_switch_core(par, K.from(c0), c2, n, nullptr, nullptr, dst, dst + Lk * row, 2 * (u32)Lk, ws, st);
   });
   FHE_CUDA(cudaGetLastError());
   out2->repr = FHE_B200_NTT;
+}
+
+int fhe_b200_key_switch(const fhe_b200_batch* pb, uint32_t part, const fhe_b200_ksk* k, fhe_b200_batch* out2,
+                        void* stream) {
+  API_BEGIN
+  key_switch_run(pb, part, {&k, 1, nullptr}, out2, stream);
+  API_END
+}
+
+int fhe_b200_key_switch_keyed(const fhe_b200_batch* pb, uint32_t part, const fhe_b200_ksk* const* keys,
+                              uint32_t n_keys, const uint32_t* key_index, fhe_b200_batch* out2, void* stream) {
+  API_BEGIN
+  key_switch_run(pb, part, key_list(keys, n_keys, key_index), out2, stream);
   API_END
 }
 

@@ -3,6 +3,7 @@
 #include <atomic>
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <vector>
 
 #include "ntt.cuh"
 
@@ -137,21 +138,42 @@ struct ScalerDev {
 void launch_scale(const ScalerDev& S, const LimbDev* limbs, const u64* in, u64* out0, u64* out1, u32 polys,
                   u32 out_rows_per_poly, u32 start, u32 n_out, int split3, u32 logn, cudaStream_t st);
 
-// key-switch inner product (key_switching_key.rs:256-268) on already transformed digits:
+// The keys of one inner-product launch, carried in its kernel parameters: pair s is (k0[s], k1[s]), each
+// [Lk][n_dig][N], and ciphertext c of the launch uses pair slot[c].  With n == 1 every ciphertext uses pair 0 and
+// `slot` is not read, so a one-key launch may hold any number of ciphertexts; otherwise at most kKeySlots.
+constexpr u32 kKeyPairs = 64;
+constexpr u32 kKeySlots = 512;
+struct KeyTable {
+  const u64* k0[kKeyPairs];
+  const u64* k1[kKeyPairs];
+  u32 n;
+  unsigned char slot[kKeySlots];
+};
+// ciphertexts [ct0, ct0 + cts) of a key switch and their keys: one inner-product launch each
+struct KeyRange {
+  u32 ct0, cts;
+  KeyTable keys;
+};
+#ifdef __CUDACC__
+__device__ __forceinline__ u32 key_slot(const KeyTable& K, u32 ct) { return K.n > 1 ? K.slot[ct] : 0; }
+#endif
+
+// key-switch inner product (key_switching_key.rs:256-268) on already transformed digits, one launch per range:
 // inter: [ct][n_dig][Lk][N] NTT values (lazy, any 64-bit word), or [ct][Lk][n_dig][N] when `adjacent`;
-// k0,k1: [Lk][n_dig][N] (limb-major: the device copy of a key is transposed once at upload);
+// keys: [Lk][n_dig][N] (limb-major: the device copy of a key is transposed once at upload);
 // out0/out1 row (ct, j) at out + (ct*out_ct_rows + j)*N ; base0/base1 (nullable) same indexing.
-void launch_ksmac(const u64* inter, const u64* k0, const u64* k1, const u64* base0, const u64* base1, u64* out0,
-                  u64* out1, u32 cts, u32 n_dig, u32 Lk, u32 out_ct_rows, const RowIds& ids, const LimbDev* limbs,
-                  u32 logn, cudaStream_t st, bool adjacent = false);
+void launch_ksmac(const u64* inter, const std::vector<KeyRange>& ranges, const u64* base0, const u64* base1, u64* out0,
+                  u64* out1, u32 n_dig, u32 Lk, u32 out_ct_rows, const RowIds& ids, const LimbDev* limbs, u32 logn,
+                  cudaStream_t st, bool adjacent = false);
 
 // whether launch_ntt will take the TMA kernels for this shape (they can write the digit-adjacent layout)
 bool ntt_uses_tma(u32 n_rows, const RowIds& ids, u32 logn, u32 in_div, const u64* in, const u64* out);
 
 // the RNS-digit key switch on the TMA kernels: digit broadcast + forward cols pass of c2 [cts][n_dig][N] into
 // `inter` (scratch, cts*n_dig*Lk rows, digit-adjacent), then the forward rows pass fused with the inner product of
-// launch_ksmac (same outputs, same indexing).  Returns false, having launched nothing, outside the kernels' domain.
-bool launch_key_switch_tma(const u64* c2, u64* inter, const u64* k0, const u64* k1, const u64* base0,
+// launch_ksmac (same outputs, same indexing), one rows+MAC launch per range over the same `inter`.  Returns false,
+// having launched nothing, outside the kernels' domain.
+bool launch_key_switch_tma(const u64* c2, u64* inter, const std::vector<KeyRange>& ranges, const u64* base0,
                            const u64* base1, u64* out0, u64* out1, u32 cts, u32 n_dig, u32 Lk, u32 out_ct_rows,
                            const RowIds& ids, const LimbDev* limbs, u32 logn, bool reduce, cudaStream_t st);
 

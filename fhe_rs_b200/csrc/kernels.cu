@@ -727,7 +727,8 @@ __global__ void scale_small_kernel(ScaleArgs A) {
 
 // ------------------------------------------------------------------ key-switch MAC
 struct KsMacArgs {
-  const u64 *inter, *k0, *k1, *base0, *base1;
+  KeyTable keys;
+  const u64 *inter, *base0, *base1;
   u64 *out0, *out1;
   u32 cts, n_dig, Lk, out_ct_rows, logn;
   u32 adjacent;   // digit rows of one (ciphertext, limb) adjacent: inter is [ct][limb][digit][N], else [ct][digit][limb][N]
@@ -738,8 +739,8 @@ struct KsMacArgs {
 // One thread per (limb j, ciphertext, coefficient), limb-major: consecutive CTAs work on the same key limb for
 // every ciphertext of the chunk, so the 2 x n_dig key rows of that limb (7 MB at set C, stored limb-major
 // [limb][digit][N]) stay in L2 while the digit rows stream through -- each key word leaves HBM once per chunk instead
-// of once per ciphertext.
-__global__ void ksmac_kernel(KsMacArgs A) {
+// of once per ciphertext.  Each ciphertext reads the key pair its slot names.
+__global__ void ksmac_kernel(const __grid_constant__ KsMacArgs A) {
   const u32 N = 1u << A.logn;
   size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // over Lk*cts*N
   size_t total = ((size_t)A.cts * A.Lk) << A.logn;
@@ -755,8 +756,9 @@ __global__ void ksmac_kernel(KsMacArgs A) {
                                 : A.inter + ((((size_t)ct * A.n_dig) * A.Lk + j) << A.logn) + c;
   const size_t dstride = A.adjacent ? (size_t)1 << A.logn : (size_t)A.Lk << A.logn;
   const size_t kstride = (size_t)1 << A.logn;
-  const u64* k0_ptr = A.k0 + (((size_t)j * A.n_dig) << A.logn) + c;
-  const u64* k1_ptr = A.k1 + (((size_t)j * A.n_dig) << A.logn) + c;
+  const u32 slot = key_slot(A.keys, ct);
+  const u64* k0_ptr = A.keys.k0[slot] + (((size_t)j * A.n_dig) << A.logn) + c;
+  const u64* k1_ptr = A.keys.k1[slot] + (((size_t)j * A.n_dig) << A.logn) + c;
   // two digits per trip, the six words of the next trip requested before the multiplies of this one (the kernel
   // is bound by HBM latency, not by the multiplier: 2 x n_dig x 8 IMAD.WIDE per 48 bytes read).  Two
   // coefficients per thread with 16-byte accesses, and four ciphertexts per thread sharing each key word (a third
@@ -799,11 +801,12 @@ __global__ void ksmac_kernel(KsMacArgs A) {
 // load latency (about half of the device's copy rate): here one elected thread streams every operand with TMA box
 // copies and the compute threads only read shared memory.
 //   work item = (limb j, 128-coefficient tile tau, ciphertext ct), ct innermost: the two key tiles of (j, tau)
-//   ({128, n_dig} boxes, 2 x n_dig KiB) are fetched once and stay in shared memory for every ciphertext of the CTA's
-//   range; the digit tile of each ciphertext ({128, n_dig} box: its n_dig rows are adjacent) arrives through a ring of
+//   (2 n_dig row segments of 1 KiB) are fetched once and stay in shared memory for every ciphertext of the CTA's
+//   range that uses the same key pair; the digit tile of each ciphertext ({128, n_dig} box: its n_dig rows are adjacent) arrives through a ring of
 //   KS_STAGES buffers, refilled as soon as the CTA has consumed it.
 constexpr int kKsTC = 128;
 struct KsTmaArgs {
+  KeyTable keys;
   const u64 *base0, *base1;
   u64 *out0, *out1;
   u32 cts, n_dig, Lk, out_ct_rows, logn;
@@ -814,8 +817,7 @@ struct KsTmaArgs {
 
 template <int KS_STAGES>
 __global__ void __launch_bounds__(kKsTC) ksmac_tma_kernel(const __grid_constant__ CUtensorMap tm_t,
-                                                          const __grid_constant__ CUtensorMap tm_k0,
-                                                          const __grid_constant__ CUtensorMap tm_k1, const KsTmaArgs A) {
+                                                          const __grid_constant__ KsTmaArgs A) {
   using namespace tma;
   extern __shared__ __align__(128) u64 smem[];
   constexpr u32 TC = kKsTC, S = KS_STAGES;
@@ -854,20 +856,20 @@ __global__ void __launch_bounds__(kKsTC) ksmac_tma_kernel(const __grid_constant_
   if (cc == 0)
     while (loaded < n && loaded < S) load_next();
 
-  u32 cur_jt = 0xffffffffu, key_phase = 0;
+  u32 cur_jt = 0xffffffffu, cur_slot = 0, key_phase = 0;
   const LimbDev* Mp = A.limbs;
   for (u32 i = 0; i < n; i++) {
-    if (w.jt != cur_jt) {
-      // new (limb, tile): its two key tiles replace the previous ones (every thread has finished with those: the
-      // item loop ends with a CTA barrier)
+    const u32 slot = key_slot(A.keys, w.p);
+    if (w.jt != cur_jt || slot != cur_slot) {
+      // new (limb, tile) or new key: its two key tiles replace the previous ones (every thread has finished with
+      // those: the item loop ends with a CTA barrier)
       cur_jt = w.jt;
+      cur_slot = slot;
       const u32 j = cur_jt / tiles, tau = cur_jt - j * tiles;
       Mp = A.limbs + A.ids[j];
-      if (cc == 0) {
-        mbar_expect_tx(bar_key, 2 * box_bytes);
-        load_2d(smem_u32(s_k0), &tm_k0, tau * TC, j * nd, bar_key);
-        load_2d(smem_u32(s_k1), &tm_k1, tau * TC, j * nd, bar_key);
-      }
+      if (cc == 0)
+        load_key_tiles<TC>(smem_u32(s_k0), smem_u32(s_k1), A.keys.k0[slot], A.keys.k1[slot], j, tau, nd, A.logn,
+                           bar_key);
       mbar_wait(bar_key, key_phase);
       key_phase ^= 1;
     }
@@ -1882,26 +1884,38 @@ void launch_scale(const ScalerDev& S, const LimbDev* limbs, const u64* in, u64* 
   g_launches++;
 }
 
-void launch_ksmac(const u64* inter, const u64* k0, const u64* k1, const u64* base0, const u64* base1, u64* out0,
-                  u64* out1, u32 cts, u32 n_dig, u32 Lk, u32 out_ct_rows, const RowIds& ids, const LimbDev* limbs,
-                  u32 logn, cudaStream_t st, bool adjacent) {
-  size_t total = ((size_t)cts * Lk) << logn;
-  if (!total) return;
+void launch_ksmac(const u64* inter, const std::vector<KeyRange>& ranges, const u64* base0, const u64* base1, u64* out0,
+                  u64* out1, u32 n_dig, u32 Lk, u32 out_ct_rows, const RowIds& ids, const LimbDev* limbs, u32 logn,
+                  cudaStream_t st, bool adjacent) {
   const bool classic = switches().ksmac == Switches::KSMAC_CLASSIC;
   // ring depth: 2 buffers -> 4 resident CTAs per SM at set C: the kernel needs warps more than prefetch depth.
   // FHE_B200_KS_STAGES = 2 | 3 | 4.
   const int stages = (int)switches().ks_stages;
   const size_t smem_tma = ((size_t)(2 + stages) * n_dig * kKsTC + stages + 1) * sizeof(u64);
-  if (adjacent && !classic && tensor_map_encoder() && logn >= 7 && n_dig <= 256 && smem_tma <= 200 * 1024 &&
-      !((reinterpret_cast<uintptr_t>(inter) | reinterpret_cast<uintptr_t>(k0) | reinterpret_cast<uintptr_t>(k1)) & 127) &&
-      (u64)cts * Lk * n_dig < (1ull << 31)) {
-    CUtensorMap mt, m0, m1;
-    if (box_map(&mt, inter, (u64)cts * Lk * n_dig, logn, kKsTC, n_dig) &&
-        box_map(&m0, k0, (u64)Lk * n_dig, logn, kKsTC, n_dig) && box_map(&m1, k1, (u64)Lk * n_dig, logn, kKsTC, n_dig)) {
+  bool tma = adjacent && !classic && tensor_map_encoder() && logn >= 7 && n_dig <= 256 && smem_tma <= 200 * 1024 &&
+             !(reinterpret_cast<uintptr_t>(inter) & 127);
+  for (const KeyRange& r : ranges) {
+    tma = tma && (u64)r.cts * Lk * n_dig < (1ull << 31);
+    for (u32 s = 0; s < r.keys.n; s++)
+      tma = tma && !((reinterpret_cast<uintptr_t>(r.keys.k0[s]) | reinterpret_cast<uintptr_t>(r.keys.k1[s])) & 127);
+  }
+  // every tensor map first: a shape the TMA cannot describe takes the classic kernel for the whole call
+  std::vector<CUtensorMap> mt(ranges.size());
+  for (size_t r = 0; tma && r < ranges.size(); r++)
+    tma = box_map(&mt[r], inter + (((size_t)ranges[r].ct0 * Lk * n_dig) << logn), (u64)ranges[r].cts * Lk * n_dig,
+                  logn, kKsTC, n_dig);
+  for (size_t r = 0; r < ranges.size(); r++) {
+    const KeyRange& R = ranges[r];
+    const size_t total = ((size_t)R.cts * Lk) << logn;
+    if (!total) continue;
+    const size_t o = ((size_t)R.ct0 * out_ct_rows) << logn;
+    if (tma) {
       KsTmaArgs T;
-      T.base0 = base0; T.base1 = base1; T.out0 = out0; T.out1 = out1;
-      T.cts = cts; T.n_dig = n_dig; T.Lk = Lk; T.out_ct_rows = out_ct_rows; T.logn = logn;
-      T.items_total = Lk * ((1u << logn) / kKsTC) * cts;
+      T.keys = R.keys;
+      T.base0 = base0 ? base0 + o : nullptr; T.base1 = base1 ? base1 + o : nullptr;
+      T.out0 = out0 + o; T.out1 = out1 + o;
+      T.cts = R.cts; T.n_dig = n_dig; T.Lk = Lk; T.out_ct_rows = out_ct_rows; T.logn = logn;
+      T.items_total = Lk * ((1u << logn) / kKsTC) * R.cts;
       T.limbs = limbs;
       copy_ids(T.ids, ids);
       auto go = [&](auto kern) {
@@ -1909,23 +1923,26 @@ void launch_ksmac(const u64* inter, const u64* k0, const u64* k1, const u64* bas
         int per_sm = 0;
         FHE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)kern, kKsTC, smem_tma));
         const u32 grid = (u32)std::min<u64>(T.items_total, (u64)sm_count() * std::max(per_sm, 1));
-        kern<<<grid, kKsTC, smem_tma, st>>>(mt, m0, m1, T);
+        kern<<<grid, kKsTC, smem_tma, st>>>(mt[r], T);
       };
       if (stages == 2) go(ksmac_tma_kernel<2>);
       else if (stages == 3) go(ksmac_tma_kernel<3>);
       else go(ksmac_tma_kernel<4>);
       g_launches++;
-      return;
+      continue;
     }
+    KsMacArgs A;
+    A.keys = R.keys;
+    A.adjacent = adjacent ? 1 : 0;
+    A.inter = inter + ((((size_t)R.ct0 * Lk) * n_dig) << logn);
+    A.base0 = base0 ? base0 + o : nullptr; A.base1 = base1 ? base1 + o : nullptr;
+    A.out0 = out0 + o; A.out1 = out1 + o;
+    A.cts = R.cts; A.n_dig = n_dig; A.Lk = Lk; A.out_ct_rows = out_ct_rows; A.logn = logn;
+    A.limbs = limbs;
+    copy_ids(A.ids, ids);
+    ksmac_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(A);
+    g_launches++;
   }
-  KsMacArgs A;
-  A.adjacent = adjacent ? 1 : 0;
-  A.inter = inter; A.k0 = k0; A.k1 = k1; A.base0 = base0; A.base1 = base1; A.out0 = out0; A.out1 = out1;
-  A.cts = cts; A.n_dig = n_dig; A.Lk = Lk; A.out_ct_rows = out_ct_rows; A.logn = logn;
-  A.limbs = limbs;
-  copy_ids(A.ids, ids);
-  ksmac_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(A);
-  g_launches++;
 }
 
 void launch_decompose(const u64* in, u64* out, size_t polys, u32 n_dig, u32 log_base, u32 logn, cudaStream_t st) {

@@ -374,18 +374,27 @@ bool launch_tensor_intt_tma(const u64* a, const u64* b, const u64* xa, const u64
   return true;
 }
 
-template <int STAGES>
-void run_ks_rows_mac(const CUtensorMap& mi, const CUtensorMap& m0, const CUtensorMap& m1, const KsRowsArgs& A,
-                     cudaStream_t st) {
+template <int STAGES, class Kern, class Keys>
+void run_ks_rows_mac_with(Kern k, const CUtensorMap& mi, const CUtensorMap& m0, const CUtensorMap& m1,
+                          const KsRowsArgs& A, const Keys& keys, cudaStream_t st) {
   using Cfg = KsRowsCfg<STAGES>;
-  auto k = ks_rows_mac_tma_kernel<STAGES, 3>;
   const size_t smem = Cfg::smem(A.n_dig);
   ensure_dynamic_smem((const void*)k, smem);
   int per_sm = 0;
   FHE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)k, Cfg::NT + 32, smem));
   const u32 grid = (u32)std::min<u64>(A.items_total, (u64)sm_count() * std::max(per_sm, 1));
-  k<<<grid, Cfg::NT + 32, smem, st>>>(mi, m0, m1, A);
+  k<<<grid, Cfg::NT + 32, smem, st>>>(mi, m0, m1, A, keys);
   g_launches++;
+}
+
+template <int STAGES>
+void run_ks_rows_mac(const CUtensorMap& mi, const CUtensorMap& m0, const CUtensorMap& m1, const KsRowsArgs& A,
+                     const KeyTable& keys, cudaStream_t st) {
+  if (keys.n == 1) {   // one key: its tensor maps, and no key table in the launch parameters
+    run_ks_rows_mac_with<STAGES>(ks_rows_mac_tma_kernel<STAGES, 3, OneKey>, mi, m0, m1, A, OneKey{}, st);
+    return;
+  }
+  run_ks_rows_mac_with<STAGES>(ks_rows_mac_tma_kernel<STAGES, 3, KeyTable>, mi, mi, mi, A, keys, st);
 }
 
 }  // namespace
@@ -411,7 +420,7 @@ bool launch_tensor_inverse_ntt(const u64* a, const u64* b, const u64* xa, const 
   return launch_tensor_intt_tma(a, b, xa, xb, T, cts, L, K, mul_ids, limbs, logn, st);
 }
 
-bool launch_key_switch_tma(const u64* c2, u64* inter, const u64* k0, const u64* k1, const u64* base0,
+bool launch_key_switch_tma(const u64* c2, u64* inter, const std::vector<KeyRange>& ranges, const u64* base0,
                            const u64* base1, u64* out0, u64* out1, u32 cts, u32 n_dig, u32 Lk, u32 out_ct_rows,
                            const RowIds& ids, const LimbDev* limbs, u32 logn, bool reduce, cudaStream_t st) {
   // ring depth of the digit tiles: 2 (default) or 3 (FHE_B200_KS_STAGES >= 3); both keep 3 CTAs per SM at n_dig = 14
@@ -420,17 +429,24 @@ bool launch_key_switch_tma(const u64* c2, u64* inter, const u64* k0, const u64* 
   const u32 n_rows = cts * n_dig * Lk;
   if (logn < 13 || logn > 15 || !tensor_map_encoder() || ids.limbs_per_poly != Lk || n_dig == 0 || n_dig > 256)
     return false;
-  if ((reinterpret_cast<uintptr_t>(c2) | reinterpret_cast<uintptr_t>(inter) | reinterpret_cast<uintptr_t>(k0) |
-       reinterpret_cast<uintptr_t>(k1)) & 127)
-    return false;
+  if ((reinterpret_cast<uintptr_t>(c2) | reinterpret_cast<uintptr_t>(inter)) & 127) return false;
+  // the key tiles travel as 1 KiB row segments (cp.async.bulk: 16-byte aligned)
+  for (const KeyRange& r : ranges)
+    for (u32 s = 0; s < r.keys.n; s++)
+      if ((reinterpret_cast<uintptr_t>(r.keys.k0[s]) | reinterpret_cast<uintptr_t>(r.keys.k1[s])) & 127) return false;
   if ((stages == 3 ? KsRowsCfg<3>::smem(n_dig) : Cfg::smem(n_dig)) > 227 * 1024) return false;
-  // every tensor map first: a shape the TMA cannot describe launches nothing.  The keys [Lk][n_dig][N] are read as
-  // {128-coefficient, n_dig-row} boxes.
-  CUtensorMap m0, m1;
-  if (!box_map(&m0, k0, (u64)Lk * n_dig, logn, Cfg::TC, n_dig) || !box_map(&m1, k1, (u64)Lk * n_dig, logn, Cfg::TC, n_dig))
-    return false;
   try {
-    const CUtensorMap mi = rows_map(inter, n_rows, logn, 4 * Cfg::R);
+    // every tensor map first: a shape the TMA cannot describe launches nothing.  A one-key range reads its key
+    // [Lk][n_dig][N] as {128-coefficient, n_dig-row} boxes; a range of several keys copies 1 KiB row segments.
+    std::vector<CUtensorMap> mi(ranges.size()), m0(ranges.size()), m1(ranges.size());
+    for (size_t r = 0; r < ranges.size(); r++) {
+      mi[r] = rows_map(inter + (((size_t)ranges[r].ct0 * n_dig * Lk) << logn), (u64)ranges[r].cts * n_dig * Lk, logn,
+                       4 * Cfg::R);
+      const KeyTable& K = ranges[r].keys;
+      if (K.n == 1 && (!box_map(&m0[r], K.k0[0], (u64)Lk * n_dig, logn, Cfg::TC, n_dig) ||
+                       !box_map(&m1[r], K.k1[0], (u64)Lk * n_dig, logn, Cfg::TC, n_dig)))
+        return false;
+    }
     // digit broadcast + large-stride stages: inter [ct][j][d][N] (in_bcast: the source row of polynomial (ct, d) is
     // row ct*n_dig + d of c2 for every limb j)
     NttTmaArgs C;
@@ -445,16 +461,22 @@ bool launch_key_switch_tma(const u64* c2, u64* inter, const u64* k0, const u64* 
     C.logn = logn;
     for (int i = 0; i < kMaxPos; i++) C.ids[i] = ids.ids[i];
     run_tma_cols_for<false>(c2, (u64)cts * n_dig, inter, n_rows, C, st);
+    // the rows pass fused with the inner product, one launch per key range over the same transformed digits
     KsRowsArgs A;
     std::memset(&A, 0, sizeof(A));
     A.limbs = limbs;
-    A.base0 = base0; A.base1 = base1; A.out0 = out0; A.out1 = out1;
-    A.cts = cts; A.n_dig = n_dig; A.Lk = Lk; A.out_ct_rows = out_ct_rows; A.logn = logn;
+    A.n_dig = n_dig; A.Lk = Lk; A.out_ct_rows = out_ct_rows; A.logn = logn;
     A.tiles_per_row = (1u << logn) / Cfg::TC;
-    A.items_total = Lk * A.tiles_per_row * cts;
     for (int i = 0; i < kMaxPos; i++) A.ids[i] = ids.ids[i];
-    if (stages == 3) run_ks_rows_mac<3>(mi, m0, m1, A, st);
-    else run_ks_rows_mac<2>(mi, m0, m1, A, st);
+    for (size_t r = 0; r < ranges.size(); r++) {
+      const size_t o = ((size_t)ranges[r].ct0 * out_ct_rows) << logn;
+      A.base0 = base0 ? base0 + o : nullptr; A.base1 = base1 ? base1 + o : nullptr;
+      A.out0 = out0 + o; A.out1 = out1 + o;
+      A.cts = ranges[r].cts;
+      A.items_total = Lk * A.tiles_per_row * A.cts;
+      if (stages == 3) run_ks_rows_mac<3>(mi[r], m0[r], m1[r], A, ranges[r].keys, st);
+      else run_ks_rows_mac<2>(mi[r], m0[r], m1[r], A, ranges[r].keys, st);
+    }
   } catch (const TmaFail&) {
     return false;
   }

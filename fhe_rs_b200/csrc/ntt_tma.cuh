@@ -21,7 +21,9 @@
 // 64-bit words, the unit-stride round 128-bit pairs, both without bank conflicts.
 #pragma once
 #include <cuda.h>
+#include <type_traits>
 
+#include "engine.hpp"
 #include "ntt.cuh"
 
 namespace fhe_b200 {
@@ -93,6 +95,25 @@ __device__ __forceinline__ void load_2d(u32 dst, const CUtensorMap* tm, u32 c0, 
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
       ::"r"(dst), "l"(tm), "r"(c0), "r"(c1), "r"(bar)
       : "memory");
+}
+// a contiguous global -> shared copy (16-byte aligned, a multiple of 16 bytes) completing on mbarrier `bar`
+__device__ __forceinline__ void load_1d(u32 dst, const void* src, u32 bytes, u32 bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
+               : "memory");
+}
+// the key tiles of (limb j, TC-coefficient tile tau) of a key pair [limb][digit][N]: digit d of k0 / k1 lands at
+// dst0 / dst1 + d * TC * 8.  2 * nd row segments of TC words, all completing on `bar`.
+template <u32 TC>
+__device__ __forceinline__ void load_key_tiles(u32 dst0, u32 dst1, const u64* k0, const u64* k1, u32 j, u32 tau,
+                                               u32 nd, u32 logn, u32 bar) {
+  mbar_expect_tx(bar, 2 * nd * TC * 8);
+  const size_t row0 = ((size_t)j * nd << logn) + (size_t)tau * TC;
+  for (u32 d = 0; d < nd; d++) {
+    const size_t off = row0 + ((size_t)d << logn);
+    load_1d(dst0 + d * TC * 8, k0 + off, TC * 8, bar);
+    load_1d(dst1 + d * TC * 8, k1 + off, TC * 8, bar);
+  }
 }
 __device__ __forceinline__ void store_2d(const CUtensorMap* tm, u32 c0, u32 c1, u32 src) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%1, %2}], [%3];" ::"l"(tm), "r"(c0),
@@ -871,8 +892,10 @@ __global__ void __launch_bounds__(TensorRowsCfg<RLOG, STAGES>::NT + 32, MINB)
 // (key_switching_key.rs:256-268: out{0,1} = base{0,1} + sum_d NTT_j(digit_d) * k{0,1}[j][d]).  Every digit of one
 // (ciphertext, limb j) is transformed modulo the same q_j, so all of them share the rows-pass twiddles of (j, tau) and
 // the key tiles of (j, tau); the cols pass has left them in adjacent rows (digit-adjacent layout, [ct][j][d][N]).
-//   work item = (limb j, 128-coefficient tile tau, ciphertext ct), ct innermost: twiddles and the two key tiles of
-//   (j, tau) ({128, n_dig} boxes) are staged once per run of ciphertexts; the n_dig digit tiles of each item arrive
+//   work item = (limb j, 128-coefficient tile tau, ciphertext ct), ct innermost: twiddles are staged once per (j, tau)
+//   and the two key tiles of (j, tau) (2 n_dig row segments of 1 KiB, from the key pair the ciphertext's slot names)
+//   once per run of ciphertexts with the same (j, tau) and the same key (Keys = OneKey: the {128, n_dig} boxes of the
+//   key's tensor maps; Keys = KeyTable: the pair the ciphertext's slot names); the n_dig digit tiles of each item arrive
 //   through a ring of STAGES buffers.  Per item: the six small-stride forward stages on each digit tile (16 threads per
 //   tile, 16 tiles side by side, lazy outputs in [0,4q_j) as the unfused pass leaves them), a CTA barrier, then one
 //   thread per (output, coefficient) accumulates sum_d digit_d * key_d with Acc192, adds the base and reduces once.
@@ -900,10 +923,15 @@ struct KsRowsCfg {
   }
 };
 
-template <int STAGES, int MINB>
+// the keys of a launch with one key: its tensor maps (tm_k0, tm_k1), every ciphertext in slot 0
+struct OneKey {};
+__device__ __forceinline__ u32 key_slot(const OneKey&, u32) { return 0; }
+
+template <int STAGES, int MINB, class Keys>
 __global__ void __launch_bounds__(KsRowsCfg<STAGES>::NT + 32, MINB)
     ks_rows_mac_tma_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_k0,
-                           const __grid_constant__ CUtensorMap tm_k1, const KsRowsArgs A) {
+                           const __grid_constant__ CUtensorMap tm_k1, const KsRowsArgs A,
+                           const __grid_constant__ Keys K) {
   using namespace tma;
   using Cfg = KsRowsCfg<STAGES>;
   constexpr u32 R = Cfg::R, TC = Cfg::TC, NT = Cfg::NT, TILE_BYTES = Cfg::TILE_BYTES, GROUPS = Cfg::GROUPS;
@@ -981,24 +1009,33 @@ __global__ void __launch_bounds__(KsRowsCfg<STAGES>::NT + 32, MINB)
   TileWalk w;
   w.init(lo, A.cts);
   bool fresh = true;
-  u32 key_phase = 0;
+  u32 key_phase = 0, cur_slot = 0;
   const LimbDev* Mp = A.limbs;
   u64 p = 0, p2 = 0;
   const u32 logn1 = A.logn - 6;
   for (u32 i = 0; i < n; i++) {
     const u32 j = w.jt / A.tiles_per_row, tau = w.jt - j * A.tiles_per_row;
-    const bool new_keys = fresh;
+    const u32 slot = key_slot(K, w.p);
+    const bool new_keys = fresh || slot != cur_slot;
+    if (new_keys) {
+      // new (limb, tile position) or new key: the key tiles replace the previous ones
+      cur_slot = slot;
+      if (i) consumer_sync<NT>();   // nobody still reads the previous twiddles or key tiles
+      if (tid == 0) {
+        if constexpr (std::is_same<Keys, OneKey>::value) {
+          mbar_expect_tx(bar_key, 2 * nd * TC * 8);
+          load_2d(k0_base, &tm_k0, tau * TC, j * nd, bar_key);
+          load_2d(k1_base, &tm_k1, tau * TC, j * nd, bar_key);
+        } else {
+          load_key_tiles<TC>(k0_base, k1_base, K.k0[slot], K.k1[slot], j, tau, nd, A.logn, bar_key);
+        }
+      }
+    }
     if (fresh) {
-      // new (limb, tile position): its key tiles and 63R twiddle pairs replace the previous ones
+      // new (limb, tile position): its 63R twiddle pairs replace the previous ones
       Mp = A.limbs + A.ids[j];
       p = Mp->p;
       p2 = Mp->p2;
-      if (i) consumer_sync<NT>();   // nobody still reads the previous twiddles or key tiles
-      if (tid == 0) {
-        mbar_expect_tx(bar_key, 2 * nd * TC * 8);
-        load_2d(k0_base, &tm_k0, tau * TC, j * nd, bar_key);
-        load_2d(k1_base, &tm_k1, tau * TC, j * nd, bar_key);
-      }
       const u32 row0 = tau * R;
 #pragma unroll
       for (int tl = 0; tl < 6; tl++) {

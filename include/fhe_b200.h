@@ -477,6 +477,41 @@ int fhe_b200_switch_down(fhe_b200_batch* b, void* stream);
  * out (2 parts, NTT, ksk level) = (sum_i NTT(d_i) * c0_i, sum_i NTT(d_i) * c1_i) */
 int fhe_b200_key_switch(const fhe_b200_batch* pb, uint32_t part, const fhe_b200_ksk* k,
                         fhe_b200_batch* out2, void* stream);
+/* ---- per-ciphertext keys ----------------------------------------------------------------------------
+ * A server that answers many clients holds one relinearization, Galois or expansion key per client.  The _keyed
+ * calls below take a list of key handles and, in key_index (host memory, read during the call only), one u32 per
+ * ciphertext of the batch naming its key: entry j of the output is, word for word, what the single-key call gives on
+ * entry j alone with keys[key_index[j]].  An index may repeat, a key may go unused and a handle may be listed more
+ * than once.
+ * What stays shared by the whole batch: the levels, the Galois exponent, the expansion size and mod_switch.  Each
+ * key is checked as the single-key call checks it, and all keys of one call (for expand: of one expansion level) must
+ * have the same key level, digit count and base.  INVALID_ARGUMENT: a NULL key list, key or index, n_keys == 0, an
+ * index >= n_keys, keys that differ in key level, digit count or base; every other error is the single-key call's.
+ * Every check runs before anything is enqueued: a refused call writes nothing and keeps no device memory.  Streams
+ * and chunks behave as in the single-key calls.  The digit transforms of a key switch do not depend on the key; its
+ * inner product stages each run of ciphertexts with the same key once, and a chunk with more than 64 distinct keys
+ * takes one inner-product launch per range of at most 64.  With one key the calls launch exactly the single-key
+ * calls' kernels. */
+/* fhe_b200_key_switch of entry j with keys[key_index[j]] */
+int fhe_b200_key_switch_keyed(const fhe_b200_batch* pb, uint32_t part, const fhe_b200_ksk* const* keys,
+                              uint32_t n_keys, const uint32_t* key_index, fhe_b200_batch* out2, void* stream);
+/* fhe_b200_relinearize of entry j with rks[key_index[j]] */
+int fhe_b200_relinearize_keyed(const fhe_b200_batch* ct3, const fhe_b200_ksk* const* rks, uint32_t n_keys,
+                               const uint32_t* key_index, fhe_b200_batch* out2, void* stream);
+/* fhe_b200_mul_relin of entry j with rks[key_index[j]] (Multiplicator::default of each key) */
+int fhe_b200_mul_relin_keyed(const fhe_b200_batch* a, const fhe_b200_batch* b, const fhe_b200_ksk* const* rks,
+                             uint32_t n_keys, const uint32_t* key_index, int mod_switch, fhe_b200_batch* out2,
+                             void* stream);
+/* fhe_b200_galois of entry j with gks[key_index[j]]; the exponent is shared, so every key must be for it (the caller
+ * vouches for that, as for fhe_b200_galois) */
+int fhe_b200_galois_keyed(const fhe_b200_batch* ct, uint32_t exponent, const fhe_b200_ksk* const* gks,
+                          uint32_t n_keys, const uint32_t* key_index, fhe_b200_batch* out, void* stream);
+/* fhe_b200_expand of every query with its own key set: gks[s * n_gks + l] is the key of expansion level l of key set
+ * s, set_index[q] (one per query, Q = ct.count) the key set of query q.  Entry i*Q + q of out is output i of query q
+ * expanded with key set set_index[q].  n_gks below the expansion level, n_sets == 0 or a NULL set_index ->
+ * INVALID_ARGUMENT. */
+int fhe_b200_expand_keyed(const fhe_b200_batch* ct, uint32_t size, const fhe_b200_ksk* const* gks, uint32_t n_gks,
+                          uint32_t n_sets, const uint32_t* set_index, fhe_b200_batch* out, void* stream);
 /* rq::scaler::Scaler::scale with the level's multiplication scalers (rq/scaler.rs:55-127):
  * which = 0: extender (level basis -> multiplication basis, factor 1),
  * which = 1: down scaler (multiplication basis -> level basis, factor t/Q).

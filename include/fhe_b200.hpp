@@ -934,6 +934,124 @@ class Multiplicator {
   bool mod_switch_ = false;
 };
 
+// ---- per-ciphertext keys (the fhe_b200_*_keyed entry points): index[j] names the key of ciphertext j (for
+// expands_keyed: of query j), and output j is what the single-key method gives on ciphertext j with that key
+namespace keyed_detail {
+inline void check_index(const std::vector<uint32_t>& index, uint32_t count) {
+  if (index.size() != count) throw Error(FHE_B200_INVALID_ARGUMENT, "expected one key index per ciphertext");
+}
+template <class K, class F>
+std::vector<const fhe_b200_ksk*> handles(const std::vector<const K*>& keys, F ksk_of) {
+  std::vector<const fhe_b200_ksk*> h;
+  for (const K* k : keys) h.push_back(k ? ksk_of(*k) : nullptr);
+  if (h.empty()) h.push_back(nullptr);   // n_keys = 0: refused by the call
+  return h;
+}
+inline std::vector<const GaloisKey*> galois_of(const std::vector<const EvaluationKey*>& eks, uint32_t exponent) {
+  std::vector<const GaloisKey*> g;
+  for (const EvaluationKey* ek : eks) {
+    auto it = ek->galois_keys().find(exponent);
+    if (it == ek->galois_keys().end())
+      throw Error(FHE_B200_INVALID_ARGUMENT, "EvaluationKeyError: rotation not supported by this key");
+    g.push_back(it->second.get());
+  }
+  return g;
+}
+}  // namespace keyed_detail
+
+inline Ciphertext key_switch_keyed(const Ciphertext& p, uint32_t part, const std::vector<const KeySwitchingKey*>& ksks,
+                                   const std::vector<uint32_t>& index) {
+  keyed_detail::check_index(index, p.count());
+  const auto h = keyed_detail::handles(ksks, [](const KeySwitchingKey& k) { return k.handle(); });
+  Ciphertext out(p.par(), p.count(), 2, ksks.empty() || !ksks[0] ? p.level() : ksks[0]->ksk_level(),
+                 Representation::Ntt, p.stream());
+  check(fhe_b200_key_switch_keyed(p.handle(), part, h.data(), (uint32_t)ksks.size(), index.data(), out.handle(),
+                                  p.stream()));
+  return out;
+}
+inline Ciphertext relinearizes_keyed(const Ciphertext& ct, const std::vector<const RelinearizationKey*>& rks,
+                                     const std::vector<uint32_t>& index) {
+  keyed_detail::check_index(index, ct.count());
+  const auto h = keyed_detail::handles(rks, [](const RelinearizationKey& k) { return k.ksk->handle(); });
+  Ciphertext out(ct.par(), ct.count(), 2, ct.level(), Representation::Ntt, ct.stream());
+  check(fhe_b200_relinearize_keyed(ct.handle(), h.data(), (uint32_t)rks.size(), index.data(), out.handle(), ct.stream()));
+  return out;
+}
+// Multiplicator::default(rks[index[j]]).multiply of pair j, with enable_mod_switching when mod_switch
+inline Ciphertext multiply_keyed(const Ciphertext& a, const Ciphertext& b, const std::vector<const RelinearizationKey*>& rks,
+                                 const std::vector<uint32_t>& index, bool mod_switch = false) {
+  keyed_detail::check_index(index, a.count());
+  const auto h = keyed_detail::handles(rks, [](const RelinearizationKey& k) { return k.ksk->handle(); });
+  Ciphertext out(a.par(), a.count(), 2, a.level() + (mod_switch ? 1 : 0), Representation::Ntt, a.stream());
+  check(fhe_b200_mul_relin_keyed(a.handle(), b.handle(), h.data(), (uint32_t)rks.size(), index.data(),
+                                 mod_switch ? 1 : 0, out.handle(), a.stream()));
+  return out;
+}
+// every key must be for the same exponent
+inline Ciphertext galois_keyed(const Ciphertext& ct, const std::vector<const GaloisKey*>& gks,
+                               const std::vector<uint32_t>& index) {
+  keyed_detail::check_index(index, ct.count());
+  for (const GaloisKey* g : gks)
+    if (g && gks[0] && g->exponent != gks[0]->exponent)
+      throw Error(FHE_B200_INVALID_ARGUMENT, "the Galois keys of one call must share their exponent");
+  const auto h = keyed_detail::handles(gks, [](const GaloisKey& k) { return k.ksk->handle(); });
+  Ciphertext out(ct.par(), ct.count(), 2, ct.level(), Representation::Ntt, ct.stream());
+  check(fhe_b200_galois_keyed(ct.handle(), gks.empty() || !gks[0] ? 1 : gks[0]->exponent, h.data(),
+                              (uint32_t)gks.size(), index.data(), out.handle(), ct.stream()));
+  return out;
+}
+inline Ciphertext rotates_columns_by_keyed(const Ciphertext& ct, const std::vector<const EvaluationKey*>& eks,
+                                           const std::vector<uint32_t>& index, uint32_t i) {
+  uint64_t e = 1, m = 2 * ct.par()->degree();   // evaluation_key.rs:278-286
+  for (uint32_t k = 0; k < i; k++) e = e * 3 % m;
+  return galois_keyed(ct, keyed_detail::galois_of(eks, (uint32_t)e), index);
+}
+inline Ciphertext rotates_rows_keyed(const Ciphertext& ct, const std::vector<const EvaluationKey*>& eks,
+                                     const std::vector<uint32_t>& index) {
+  return galois_keyed(ct, keyed_detail::galois_of(eks, 2 * (uint32_t)ct.par()->degree() - 1), index);
+}
+// EvaluationKey::expands of query q with eks[index[q]]: `size` batches, batch i holding output i of every query
+inline std::vector<Ciphertext> expands_keyed(const Ciphertext& ct, const std::vector<const EvaluationKey*>& eks,
+                                             const std::vector<uint32_t>& index, uint32_t size) {
+  const uint32_t n = (uint32_t)ct.par()->degree();
+  if (size == 0 || size > n) throw Error(FHE_B200_INVALID_ARGUMENT, "EvaluationKeyError: InvalidExpansionSize");
+  keyed_detail::check_index(index, ct.count());
+  uint32_t level = 0;
+  while ((1u << level) < size) level++;
+  std::vector<const fhe_b200_ksk*> keys((size_t)level * eks.size() + 1, nullptr);
+  for (size_t s = 0; s < eks.size(); s++)
+    for (uint32_t l = 0; l < level; l++) {
+      auto it = eks[s]->galois_keys().find((n >> l) + 1);
+      if (it != eks[s]->galois_keys().end()) keys[s * level + l] = it->second->ksk->handle();
+    }
+  Ciphertext whole(ct.par(), size * ct.count(), 2, ct.level(), Representation::Ntt, ct.stream());
+  check(fhe_b200_expand_keyed(ct.handle(), size, keys.data(), level, (uint32_t)eks.size(), index.data(), whole.handle(),
+                              ct.stream()));
+  const uint32_t q = ct.count();
+  std::vector<Ciphertext> out;
+  out.reserve(size);
+  for (uint32_t i = 0; i < size; i++) out.push_back(whole.take(i * q, q));
+  return out;
+}
+// &cts[j] * &rgsws[index[j]] (rgsw_ciphertext.rs:122-155): two keyed key switches and an add
+inline Ciphertext external_products_keyed(const Ciphertext& cts, const std::vector<const RGSWCiphertext*>& rgsws,
+                                          const std::vector<uint32_t>& index) {
+  for (const RGSWCiphertext* r : rgsws)
+    if (r && r->ksk0->ciphertext_level() != cts.level())
+      throw Error(FHE_B200_INVALID_LEVEL, "Ciphertext and RGSWCiphertext must have the same level");
+  if (cts.len() != 2) throw Error(FHE_B200_BAD_POLY_COUNT, "Ciphertext must have two parts");
+  std::vector<const KeySwitchingKey*> k0, k1;
+  for (const RGSWCiphertext* r : rgsws) {
+    k0.push_back(r ? r->ksk0.get() : nullptr);
+    k1.push_back(r ? r->ksk1.get() : nullptr);
+  }
+  Ciphertext pb = cts.clone();
+  pb.into_power_basis();
+  Ciphertext out = key_switch_keyed(pb, 0, k0, index);
+  out += key_switch_keyed(pb, 1, k1, index);
+  return out;
+}
+
 }  // namespace bfv
 
 // fhe::mbfv (multiparty BFV, crates/fhe/src/mbfv).  WARNING: experimental, incomplete and not audited, as the
