@@ -106,6 +106,9 @@ SYMBOLS = {
     "fhe_b200_mul_relin_keyed": (_i, [_vp, _vp, _pp, _u32, _pu32, _i, _vp, _vp]),
     "fhe_b200_galois_keyed": (_i, [_vp, _u32, _pp, _u32, _pu32, _vp, _vp]),
     "fhe_b200_expand_keyed": (_i, [_vp, _u32, _pp, _u32, _u32, _pu32, _vp, _vp]),
+    "fhe_b200_galois_many": (_i, [_vp, _pu32, _pp, _pu32, _u32, _pu32, _vp, _vp]),
+    "fhe_b200_inner_sum": (_i, [_vp, _pp, _u32, _vp, _vp]),
+    "fhe_b200_inner_sum_keyed": (_i, [_vp, _pp, _u32, _u32, _pu32, _vp, _vp]),
     "fhe_b200_scale": (_i, [_vp, _i, _vp, _vp]),
     "fhe_b200_poly_packed_bytes": (_i, [_vp, _u32, C.POINTER(C.c_size_t)]),
     "fhe_b200_batch_packed_bytes": (_i, [_vp, C.POINTER(C.c_size_t)]),

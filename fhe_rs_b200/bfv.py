@@ -26,7 +26,8 @@ __all__ = ["BfvParameters", "BfvParametersBuilder", "Ciphertext", "KeySwitchingK
            "Encoding", "Plaintext", "PlaintextVec", "SecretKey", "PublicKey", "EvaluationKeyBuilder",
            "transcode_bidirectional", "transcode_to_bytes", "transcode_from_bytes", "key_switch_keyed",
            "relinearizes_keyed", "multiply_keyed", "galois_keyed", "rotates_columns_by_keyed", "rotates_rows_keyed",
-           "expands_keyed", "expands_batch_keyed", "external_products_keyed"]
+           "expands_keyed", "expands_batch_keyed", "external_products_keyed", "galois_many",
+           "computes_inner_sum_keyed"]
 
 
 def _release(free_name: str, handle) -> None:
@@ -1126,15 +1127,14 @@ class EvaluationKey:
 
     def computes_inner_sum(self, ct: Ciphertext) -> Ciphertext:
         """EvaluationKey::computes_inner_sum (evaluation_key.rs:56-100)."""
+        return computes_inner_sum_keyed(ct, [self], [0] * ct.count)
+
+    def inner_sum_keys(self) -> "List[GaloisKey]":
+        """the keys of the inner sum's steps: column rotations by 1, 2, 4, ..., N/4, then the row rotation"""
         if not self.supports_inner_sum():
             raise FheError(_capi.INVALID_ARGUMENT, "EvaluationKeyError: inner sum not supported by this key")
-        out = ct.clone()
-        i = 1
-        while i < self.par.degree() // 2:
-            out += self.gk[pow(3, i, 2 * self.par.degree())].relinearize(out)
-            i *= 2
-        out += self.gk[2 * self.par.degree() - 1].relinearize(out)
-        return out
+        n = self.par.degree()
+        return [self.gk[pow(3, 1 << l, 2 * n)] for l in range(n.bit_length() - 2)] + [self.gk[2 * n - 1]]
 
     def supports_expansion(self, level: int) -> bool:  # evaluation_key.rs:175-189
         n = self.par.degree()
@@ -1175,6 +1175,21 @@ class EvaluationKey:
         if e not in self.gk:
             raise FheError(_capi.INVALID_ARGUMENT, "EvaluationKeyError: column rotation not supported by this key")
         return self.gk[e].relinearize(ct)
+
+    def rotates_columns_by_many(self, ct: Ciphertext, steps: Sequence[int]) -> Ciphertext:
+        """rotates_columns_by(ct_q, steps[i]) for every step and every ciphertext of ct (Q = ct.count) in one device call
+        (fhe_b200_galois_many): entry i*Q + q of the result is ciphertext q rotated by steps[i]"""
+        two_n = 2 * self.par.degree()
+        exps = [pow(3, int(i), two_n) for i in steps]
+        for i, e in zip(steps, exps):
+            if e not in self.gk:
+                raise FheError(_capi.INVALID_ARGUMENT,
+                               "EvaluationKeyError: column rotation by %d not supported by this key" % i)
+        keys = sorted(set(exps))
+        gks = [self.gk[e] for e in keys]
+        q = ct.count
+        index = [keys.index(e) for e in exps for _ in range(q)]
+        return galois_many(ct, gks, index, [j for _ in exps for j in range(q)])
 
 
 class EvaluationKeyBuilder:
@@ -1504,6 +1519,41 @@ def galois_keyed(ct: Ciphertext, gks: Sequence["GaloisKey"], index) -> Ciphertex
     args = _keyed_args([g.ksk for g in gks], index, ct.count)
     out = ct._like()
     check(_capi.lib().fhe_b200_galois_keyed(ct._h, gks[0].exponent if gks else 1, *args, out._h, ct.stream))
+    return out
+
+
+def galois_many(ct: Ciphertext, gks: Sequence["GaloisKey"], index, source=None) -> Ciphertext:
+    """GaloisKey.relinearize of ciphertext source[j] (j when source is None) with gks[index[j]], each key with its own
+    exponent: one device call for many rotations of one ciphertext or of many (fhe_b200_galois_many)"""
+    count = ct.count
+    if source is not None:
+        src = np.ascontiguousarray(np.asarray(source, dtype=np.int64).reshape(-1))
+        if src.size and (src.min() < 0 or src.max() > 0xFFFFFFFF):
+            raise FheError(_capi.INVALID_ARGUMENT, "source index out of range")
+        count = src.size
+        sp = (C.c_uint32 * max(1, src.size))(*[int(v) for v in src])
+    else:
+        sp = None
+    keys, n, ix = _keyed_args([g.ksk for g in gks], index, count)
+    exps = (C.c_uint32 * max(1, len(gks)))(*[int(g.exponent) & 0xFFFFFFFF for g in gks])
+    out = Ciphertext(ct.par, max(count, 1), 2, ct.level, NTT, ct.stream)
+    check(_capi.lib().fhe_b200_galois_many(ct._h, sp, keys, exps, n, ix, out._h, ct.stream))
+    return out
+
+
+def computes_inner_sum_keyed(ct: Ciphertext, eks: Sequence["EvaluationKey"], index) -> Ciphertext:
+    """EvaluationKey.computes_inner_sum of ciphertext j with eks[index[j]] (evaluation_key.rs:56-100), one device call
+    (fhe_b200_inner_sum_keyed; fhe_b200_inner_sum for a single key)"""
+    sets = [ek.inner_sum_keys() for ek in eks]
+    _, _, ix = _keyed_args([], index, ct.count)
+    n_gks = ct.par.degree().bit_length() - 1
+    arr = (C.c_void_p * max(1, n_gks * len(sets)))(*[g.ksk._h.value for gs in sets for g in gs])
+    keys = C.cast(arr, C.POINTER(C.c_void_p))
+    out = ct._like()
+    if len(sets) == 1:
+        check(_capi.lib().fhe_b200_inner_sum(ct._h, keys, n_gks, out._h, ct.stream))
+    else:
+        check(_capi.lib().fhe_b200_inner_sum_keyed(ct._h, keys, n_gks, len(sets), ix, out._h, ct.stream))
     return out
 
 

@@ -75,7 +75,7 @@ struct DeviceGuard {
 
 // The owner of a handle's immutable device tables: `put` uploads a vector on the owner's device and keeps the
 // allocation until the owner goes.  Not thread-safe: the parameter set calls put only while it holds its mutex (the
-// lazy tables of level(), perm() and expansion_monomial_dev()); the other owners fill theirs before their handle is
+// lazy tables of level() and expansion_monomial_dev()); the other owners fill theirs before their handle is
 // handed out.
 class DeviceTables {
  public:
@@ -201,7 +201,6 @@ struct fhe_b200_params {
   mutable cudaStream_t side[4] = {nullptr, nullptr, nullptr, nullptr};
   mutable std::mutex mu;
   mutable std::map<u32, std::unique_ptr<LevelData>> levels;
-  mutable std::map<u32, int*> perms;
 
   explicit fhe_b200_params(int dev) : device(dev), uploads(dev) {}
 
@@ -295,28 +294,6 @@ struct fhe_b200_params {
     auto* raw = d.get();
     levels[lv] = std::move(d);
     return *raw;
-  }
-
-  // SubstitutionExponent::new (rq/mod.rs:99-121) folded with ctx.bitrev into one gather table:
-  // out[bitrev(j)] = in[bitrev((j*e + (e-1)/2) mod N)]
-  const int* perm(u32 exponent) const {
-    std::lock_guard<std::mutex> g(mu);
-    auto it = perms.find(exponent);
-    if (it != perms.end()) return it->second;
-    std::vector<int> p(N);
-    auto brev = [&](u32 x) {
-      u32 r = 0;
-      for (u32 b = 0; b < logn; b++) r |= ((x >> b) & 1) << (logn - 1 - b);
-      return r;
-    };
-    u64 power = (exponent - 1) / 2;
-    for (u32 j = 0; j < N; j++) {
-      p[brev(j)] = (int)brev((u32)(power & (N - 1)));
-      power += exponent;
-    }
-    int* d = uploads.put(p);
-    perms[exponent] = d;
-    return d;
   }
 
   // The expansion monomial -x^(N - 2^l) of EvaluationKey (evaluation_key.rs:465-474) at level `lv`, NTT words [L][N].
@@ -602,13 +579,17 @@ void switch_down_polys(const fhe_b200_params* par, u32 level, u64* d, u32 polys,
 }
 
 // The keys of a key switch: ciphertext c of the call uses keys[index[c]], or keys[0] when index is null (the
-// single-key entry points).  Every key has the levels, digit count and base of keys[0] (check_keys).
+// single-key entry points).  Every key has the levels, digit count and base of keys[0] (check_keys).  A Galois call
+// also gives each key's exponent (reduced mod 2N) and may name each output's source ciphertext.
 struct KeySet {
   const fhe_b200_ksk* const* keys;
   u32 n;
-  const u32* index;   // host memory, one entry per ciphertext; nullable
+  const u32* index;            // host memory, one entry per ciphertext; nullable
+  const u32* exps = nullptr;   // Galois calls: exps[k] is the exponent of keys[k]
+  const u32* source = nullptr; // Galois calls, host memory, one entry per output; nullable (output c reads input c)
   // the same keys for the ciphertexts from c0 on
-  KeySet from(u32 c0) const { return {keys, n, index ? index + c0 : nullptr}; }
+  KeySet from(u32 c0) const { return {keys, n, index ? index + c0 : nullptr, exps, source ? source + c0 : nullptr}; }
+  u32 key_of(u32 c) const { return index ? index[c] : 0; }
 };
 
 // The inner-product launches of `cts` ciphertexts: consecutive ranges of at most kKeyPairs distinct keys (a handle
@@ -727,20 +708,27 @@ void key_switch_apply(const fhe_b200_params* par, const KeySet& K, const u64* c2
   }
 }
 
-// GaloisKey::relinearize (galois_key.rs:63-86) of n 2-part NTT ciphertexts [n][2][L][N] at `src` into `dst` (same
-// layout), on one stream: the chunk body of fhe_b200_galois and of every level of fhe_b200_expand.
-void galois_range(const fhe_b200_params* par, const LevelData& lv, const int* perm, const KeySet& gk,
-                  const u64* src, u64* dst, u32 n, cudaStream_t st) {
+// GaloisKey::relinearize (galois_key.rs:63-86) of n 2-part NTT ciphertexts into `dst` ([n][2][L][N]), on one stream:
+// the chunk body of every Galois call.  Output c reads ciphertext gk.source[c] of `src` (src0 + c without a source
+// list) and uses the exponent of its key.  sum: one inner-sum step, dst = src + galois(src) (dst must not alias src):
+// the substitution kernel writes (sigma(c0) + c0, c1) to dst and the key switch's in-place add finishes the step.
+void galois_range(const fhe_b200_params* par, const LevelData& lv, const KeySet& gk, const u64* src, u32 src0, u64* dst,
+                  u32 n, bool sum, cudaStream_t st) {
   const size_t row = (size_t)1 << par->logn, L = lv.L;
+  std::vector<u32> exps(n), source(n);
+  for (u32 c = 0; c < n; c++) {
+    exps[c] = gk.exps[gk.key_of(c)];
+    source[c] = gk.source ? gk.source[c] : src0 + c;
+  }
   Workspace ws(par, st);
-  u64* s = ws.words((size_t)n * 2 * L * row);
+  u64* s = sum ? nullptr : ws.words((size_t)n * 2 * L * row);
   u64* c2 = ws.words((size_t)n * L * row);
   // galois_key.rs:66: substitute both parts; part 1 becomes the key-switch input
-  launch_gather(src, s, (size_t)n * 2 * L, perm, par->logn, st);
-  FHE_CUDA(cudaMemcpy2DAsync(c2, L * row * 8, s + L * row, 2 * L * row * 8, L * row * 8, n, cudaMemcpyDeviceToDevice, st));
+  launch_substitute_ntt(src, 2 * L * row, sum ? dst : s, 2 * L * row, c2, L * row, exps.data(), source.data(), n,
+                        (u32)L, sum, lv.ctx_ids, par->d_limbs, par->logn, st);
   launch_ntt(c2, c2, n * (u32)L, lv.ctx_ids, par->d_limbs, par->logn, true, 1, false, st);
-  // galois_key.rs:67 + :78: out0 = key_switch0 + substitute(ct[0]); out1 = key_switch1
-  key_switch_apply(par, gk, c2, n, dst, 2, s, ws, st);
+  // galois_key.rs:67 + :78: out0 = key_switch0 + substitute(ct[0]); out1 = key_switch1 (sum: both added in place)
+  key_switch_apply(par, gk, c2, n, dst, sum ? 1 : 2, s, ws, st);
 }
 
 // extend -> tensor -> scale down of bfv/ops/mul.rs:192-206 for `cts` ciphertext pairs.
@@ -1874,12 +1862,12 @@ int fhe_b200_galois_keys_generate(const fhe_b200_secret_key* sk, const uint32_t*
   }
   DeviceGuard g(par);
   const LevelData& cl = par->level(ciphertext_level);
-  std::vector<const int*> perms(n_keys);
-  for (u32 k = 0; k < n_keys; k++) perms[k] = par->perm(exps[k]);
-  // x = s substituted by the exponent (galois_key.rs:40-46), a gather of the NTT words
+  // x = s substituted by the exponent (galois_key.rs:40-46), a permutation of the NTT words
   generate_keys(sk, n_keys, ciphertext_level, key_level, variance, seed_words(seed),
-                [&](u32 k, u64* x, cudaStream_t st) { launch_gather(sk->s.d, x, cl.L, perms[k], par->logn, st); }, out,
-                (cudaStream_t)stream);
+                [&](u32 k, u64* x, cudaStream_t st) {
+                  launch_substitute_ntt(sk->s.d, 0, x, 0, nullptr, 0, &exps[k], nullptr, 1, cl.L, false, cl.ctx_ids,
+                                        par->d_limbs, par->logn, st);
+                }, out, (cudaStream_t)stream);
   API_END
 }
 
@@ -2630,7 +2618,8 @@ int fhe_b200_substitute(const fhe_b200_batch* in, uint32_t exponent, fhe_b200_ba
   DeviceGuard g(par);
   const size_t rows = (size_t)in->count * in->parts * in->limbs;
   if (in->repr == FHE_B200_NTT)   // rq/mod.rs:360-389: a permutation of the bit-reversed evaluation points
-    launch_gather(in->d, out->d, rows, par->perm(exponent), par->logn, (cudaStream_t)stream);
+    launch_substitute_ntt(in->d, 0, out->d, 0, nullptr, 0, &exponent, nullptr, 1, (u32)rows, false, ids_of(in),
+                          par->d_limbs, par->logn, (cudaStream_t)stream);
   else                            // rq/mod.rs:390-408: a signed permutation of the coefficients
     launch_substitute_power(in->d, out->d, rows, exponent, ids_of(in), par->d_limbs, par->logn, (cudaStream_t)stream);
   FHE_CUDA(cudaGetLastError());
@@ -2638,25 +2627,41 @@ int fhe_b200_substitute(const fhe_b200_batch* in, uint32_t exponent, fhe_b200_ba
   API_END
 }
 
-static void galois_run(const fhe_b200_batch* ct, uint32_t exponent, const KeySet& gk, fhe_b200_batch* out,
-                       void* stream) {
+// SubstitutionExponent::new (rq/mod.rs:99-121) of each key's exponent
+static std::vector<u32> galois_exponents(const fhe_b200_params* par, const u32* exponents, u32 n_keys) {
+  std::vector<u32> e(n_keys);
+  for (u32 k = 0; k < n_keys; k++) {
+    e[k] = exponents[k] % (2 * par->N);
+    REQUIRE(e[k] & 1, FHE_B200_INVALID_EXPONENT, "InvalidSubstitutionExponent: " + std::to_string(exponents[k]));
+  }
+  return e;
+}
+
+// output j = GaloisKey::relinearize of ciphertext gk.source[j] (j without a source list) with key gk.key_of(j) for
+// its exponent gk.exps[key]
+static void galois_run(const fhe_b200_batch* ct, KeySet gk, fhe_b200_batch* out, void* stream) {
   REQUIRE(ct && gk.keys[0] && out && ct != out, FHE_B200_INVALID_ARGUMENT, "null or aliased argument");
   check_same(ct, out);
   REQUIRE(!ct->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
   REQUIRE(ct->parts == 2 && out->parts == 2, FHE_B200_BAD_POLY_COUNT, "InvalidPolynomialCount: expected 2");
-  REQUIRE(ct->count == out->count, FHE_B200_INVALID_ARGUMENT, "batch sizes differ");
+  if (gk.source)
+    for (u32 j = 0; j < out->count; j++)
+      REQUIRE(gk.source[j] < ct->count, FHE_B200_INVALID_ARGUMENT, "source " + std::to_string(gk.source[j]) +
+                                                                       " of output " + std::to_string(j) +
+                                                                       " beyond the batch");
+  else
+    REQUIRE(ct->count == out->count, FHE_B200_INVALID_ARGUMENT, "batch sizes differ");
   need_repr(ct, FHE_B200_NTT);
-  check_ksks(gk, ct->par, ct->level, ct->count);
+  check_ksks(gk, ct->par, ct->level, out->count);
   const fhe_b200_params* par = ct->par;
-  exponent %= 2 * par->N;
-  REQUIRE(exponent & 1, FHE_B200_INVALID_EXPONENT, "InvalidSubstitutionExponent");
+  const std::vector<u32> exps = galois_exponents(par, gk.exps, gk.n);
+  gk.exps = exps.data();
   DeviceGuard g(par);
   const LevelData& lv = par->level(ct->level);
   const size_t W = ct->words_per_ct();
-  const int* perm = par->perm(exponent);
-  ChunkRunner chunks(par, ct->count, (cudaStream_t)stream);
+  ChunkRunner chunks(par, out->count, (cudaStream_t)stream);
   chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
-    galois_range(par, lv, perm, gk.from(c0), ct->d + c0 * W, out->d + c0 * W, n, st);
+    galois_range(par, lv, gk.from(c0), ct->d, c0, out->d + c0 * W, n, false, st);
   });
   FHE_CUDA(cudaGetLastError());
   out->repr = FHE_B200_NTT;
@@ -2665,14 +2670,101 @@ static void galois_run(const fhe_b200_batch* ct, uint32_t exponent, const KeySet
 int fhe_b200_galois(const fhe_b200_batch* ct, uint32_t exponent, const fhe_b200_ksk* gk, fhe_b200_batch* out,
                     void* stream) {
   API_BEGIN
-  galois_run(ct, exponent, {&gk, 1, nullptr}, out, stream);
+  galois_run(ct, {&gk, 1, nullptr, &exponent}, out, stream);
   API_END
 }
 
 int fhe_b200_galois_keyed(const fhe_b200_batch* ct, uint32_t exponent, const fhe_b200_ksk* const* gks, uint32_t n_keys,
                           const uint32_t* key_index, fhe_b200_batch* out, void* stream) {
   API_BEGIN
-  galois_run(ct, exponent, key_list(gks, n_keys, key_index), out, stream);
+  KeySet K = key_list(gks, n_keys, key_index);
+  const std::vector<u32> exps(n_keys, exponent);
+  K.exps = exps.data();
+  galois_run(ct, K, out, stream);
+  API_END
+}
+
+int fhe_b200_galois_many(const fhe_b200_batch* ct, const uint32_t* source, const fhe_b200_ksk* const* gks,
+                         const uint32_t* exponents, uint32_t n_keys, const uint32_t* key_index, fhe_b200_batch* out,
+                         void* stream) {
+  API_BEGIN
+  KeySet K = key_list(gks, n_keys, key_index);
+  REQUIRE(exponents, FHE_B200_INVALID_ARGUMENT, "null exponent list");
+  REQUIRE(ct && out && ct != out && out->d != ct->d, FHE_B200_INVALID_ARGUMENT, "null or aliased argument");
+  K.exps = exponents;
+  K.source = source;
+  galois_run(ct, K, out, stream);
+  API_END
+}
+
+// EvaluationKey::computes_inner_sum (evaluation_key.rs:56-100) of every ciphertext: gks[s * n_gks + l] is the key of
+// step l of key set s (column rotations by 1, 2, 4, ..., N/4, then the row rotation), set_index[c] (nullable: set 0)
+// the key set of ciphertext c.  Step l of a chunk is one Galois call in sum mode, from the previous step's output; the
+// steps alternate between `out` and one scratch buffer so that the last lands in `out`.
+static void inner_sum_run(const fhe_b200_batch* ct, const fhe_b200_ksk* const* gks, uint32_t n_gks, uint32_t n_sets,
+                          const uint32_t* set_index, fhe_b200_batch* out, void* stream) {
+  REQUIRE(ct && out && gks, FHE_B200_INVALID_ARGUMENT, "null argument");
+  REQUIRE(ct != out && out->d != ct->d, FHE_B200_INVALID_ARGUMENT, "out must not alias ct");
+  const fhe_b200_params* par = ct->par;
+  REQUIRE(n_gks == par->logn, FHE_B200_INVALID_ARGUMENT,
+          "EvaluationKeyError: an inner sum takes log2 N = " + std::to_string(par->logn) + " keys per set, got " +
+              std::to_string(n_gks));
+  check_same(ct, out);
+  REQUIRE(!ct->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
+  REQUIRE(ct->parts == 2 && out->parts == 2, FHE_B200_BAD_POLY_COUNT, "InvalidPolynomialCount: expected 2");
+  REQUIRE(ct->count == out->count, FHE_B200_INVALID_ARGUMENT, "batch sizes differ");
+  need_repr(ct, FHE_B200_NTT);
+  const u32 Q = ct->count, steps = n_gks, m = 2 * par->N;
+  // the exponent of step l: 3^(2^l) mod 2N (evaluation_key.rs:278-286), then 2N - 1 (:118)
+  std::vector<u32> step_exp(steps);
+  u64 e = 3;
+  for (u32 l = 0; l + 1 < steps; l++) {
+    step_exp[l] = (u32)e;
+    e = e * e % m;
+  }
+  step_exp[steps - 1] = m - 1;
+  std::vector<std::vector<const fhe_b200_ksk*>> keys(steps, std::vector<const fhe_b200_ksk*>(n_sets));
+  std::vector<std::vector<u32>> exps(steps);
+  for (u32 l = 0; l < steps; l++) {
+    for (u32 k = 0; k < n_sets; k++) {
+      keys[l][k] = gks[(size_t)k * n_gks + l];
+      REQUIRE(keys[l][k], FHE_B200_INVALID_ARGUMENT,
+              "EvaluationKeyError: Missing GaloisKey { element: " + std::to_string(step_exp[l]) + " }");
+    }
+    exps[l].assign(n_sets, step_exp[l]);
+    check_ksks({keys[l].data(), n_sets, set_index}, par, ct->level, Q);
+  }
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(ct->level);
+  const size_t W = ct->words_per_ct();
+  ChunkRunner chunks(par, Q, (cudaStream_t)stream);
+  chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace ws(par, st);
+    u64* buf[2] = {out->d + c0 * W, ws.words(n * W)};
+    const u64* src = ct->d + c0 * W;
+    for (u32 l = 0; l < steps; l++) {
+      u64* dst = buf[(steps - 1 - l) & 1];
+      const KeySet K{keys[l].data(), n_sets, set_index ? set_index + c0 : nullptr, exps[l].data()};
+      galois_range(par, lv, K, src, 0, dst, n, true, st);
+      src = dst;
+    }
+  });
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
+}
+
+int fhe_b200_inner_sum(const fhe_b200_batch* ct, const fhe_b200_ksk* const* gks, uint32_t n_gks, fhe_b200_batch* out,
+                       void* stream) {
+  API_BEGIN
+  inner_sum_run(ct, gks, n_gks, 1, nullptr, out, stream);
+  API_END
+}
+
+int fhe_b200_inner_sum_keyed(const fhe_b200_batch* ct, const fhe_b200_ksk* const* gks, uint32_t n_gks, uint32_t n_sets,
+                             const uint32_t* set_index, fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  REQUIRE(n_sets && set_index, FHE_B200_INVALID_ARGUMENT, "null key set index, or no key sets");
+  inner_sum_run(ct, gks, n_gks, n_sets, set_index, out, stream);
   API_END
 }
 
@@ -2721,12 +2813,12 @@ static void expand_run(const fhe_b200_batch* ct, uint32_t size, const fhe_b200_k
   cudaStream_t user = (cudaStream_t)stream;
   const LevelData& lv = par->level(ct->level);
   const size_t W = ct->words_per_ct();
-  // tables first: building one allocates and uploads synchronously, which must not happen between enqueued levels
-  std::vector<const int*> perms(level);
+  // monomials first: building one allocates and uploads synchronously, which must not happen between enqueued levels
   std::vector<const ulonglong2*> monos(level);
+  std::vector<std::vector<u32>> exps(level);
   for (u32 l = 0; l < level; l++) {
-    perms[l] = par->perm((par->N >> l) + 1);
     monos[l] = par->expansion_monomial_dev(ct->level, l);
+    exps[l].assign(n_sets, (par->N >> l) + 1);
   }
   // index-major order: entry i*Q + q of `out` is output i of query q, so the outputs 0 .. step-1 of every query are
   // the contiguous region [0, step*Q) and the ones a level adds, step .. 2*step-1, the region right after it
@@ -2739,11 +2831,11 @@ static void expand_run(const fhe_b200_batch* ct, uint32_t size, const fhe_b200_k
     const u32 step = 1u << l, pairs = step * Q, n_hi = (std::min(2 * step, size) - step) * Q;
     u64* hi = out->d + (size_t)pairs * W;
     ChunkRunner chunks(par, pairs, user);
-    const KeySet K{keys[l].data(), n_sets, set_index ? index[l].data() : nullptr};
+    const KeySet K{keys[l].data(), n_sets, set_index ? index[l].data() : nullptr, exps[l].data()};
     chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
       const u32 e = c0 + n, mid = std::min(std::max(c0, n_hi), e);
-      if (mid > c0) galois_range(par, lv, perms[l], K.from(c0), out->d + c0 * W, hi + c0 * W, mid - c0, st);
-      if (e > mid) galois_range(par, lv, perms[l], K.from(mid), out->d + mid * W, spill + (mid - n_hi) * W, e - mid, st);
+      if (mid > c0) galois_range(par, lv, K.from(c0), out->d, c0, hi + c0 * W, mid - c0, false, st);
+      if (e > mid) galois_range(par, lv, K.from(mid), out->d, mid, spill + (mid - n_hi) * W, e - mid, false, st);
     });
     launch_expand_butterfly(out->d, hi, spill, pairs, n_hi, monos[l], lv.ctx_ids, par->d_limbs, par->logn, user);
   }

@@ -181,8 +181,23 @@ bool launch_key_switch_tma(const u64* c2, u64* inter, const std::vector<KeyRange
 // in [polys][N] -> out [polys][n_dig][N]
 void launch_decompose(const u64* in, u64* out, size_t polys, u32 n_dig, u32 log_base, u32 logn, cudaStream_t st);
 
-// NTT-domain substitution gather (rq/mod.rs:368-377): out[row][t] = in[row][perm[t]]
+// out[row][t] = in[row][perm[t]] (the SIMD decoder's slot map)
 void launch_gather(const u64* in, u64* out, size_t n_rows, const int* perm, u32 logn, cudaStream_t st);
+// The substitutions of one launch, carried in its kernel parameters: ciphertexts ct0[r] .. ct0[r+1]-1 of the launch
+// (run r) use exponent[r] and read sources src0[r], src0[r] + 1, ...  A call with more runs takes more launches.
+constexpr u32 kSubstRuns = 64;
+struct SubstTable {
+  u32 n;
+  u32 ct0[kSubstRuns], exponent[kSubstRuns], src0[kSubstRuns];
+};
+// Poly::substitute of NTT rows (rq/mod.rs:360-389) for `cts` ciphertexts: ciphertext c reads ciphertext source[c]
+// (c when source is null) of `in`, L rows per part, and uses exponent[c] (odd, < 2N); host arrays.
+//  sum == false: out0 + c*out0_stride = sigma(part 0); out1 (nullable) + c*out1_stride = sigma(part 1).
+//  sum == true (2-part): out0 + c*out0_stride = (sigma(c0) + c0, c1), out1 = sigma(c1).  ids/limbs: the rows' moduli.
+// Every word stays in [0, q) when the input's are.  No table, allocation or host synchronisation.
+void launch_substitute_ntt(const u64* in, size_t in_stride, u64* out0, size_t out0_stride, u64* out1,
+                           size_t out1_stride, const u32* exponent, const u32* source, u32 cts, u32 L, bool sum,
+                           const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st);
 // Poly<PowerBasis>::substitute (rq/mod.rs:390-408): signed coefficient scatter x^j -> x^(j*exponent)
 void launch_substitute_power(const u64* in, u64* out, size_t n_rows, u32 exponent, const RowIds& ids,
                              const LimbDev* limbs, u32 logn, cudaStream_t st);

@@ -924,6 +924,50 @@ __global__ void gather_kernel(const u64* in, u64* out, size_t n_words, const int
   out[i] = in[(row << logn) + perm[t]];
 }
 
+// Poly::substitute, Ntt branch (rq/mod.rs:360-389), with SubstitutionExponent::new (:99-121) and the bit reversal of
+// the evaluation points folded into the index: out[brev(j)] = in[brev((j*e + (e-1)/2) mod N)].  One CTA row (blockIdx.y)
+// per ciphertext; its exponent and source come from the run table (SubstTable).  The 2-part form writes
+// sigma(c0) to out0 and sigma(c1) to out1 in one pass; the inner-sum form writes out0 = (sigma(c0) + c0, c1) instead.
+struct SubstArgs {
+  SubstTable T;
+  const u64* in;
+  u64 *out0, *out1;
+  size_t in_stride, out0_stride, out1_stride;   // words per ciphertext
+  u32 L, logn;
+  int sum;
+  const LimbDev* limbs;
+  unsigned short ids[kMaxPos];
+};
+__global__ void subst_kernel(SubstArgs A) {
+  const u32 N = 1u << A.logn;
+  const size_t w = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= ((size_t)A.L << A.logn)) return;
+  const u32 c = blockIdx.y;
+  const SubstTable& T = A.T;
+  u32 lo = 0, hi = T.n;   // the run holding c: the last r with T.ct0[r] <= c
+  while (hi - lo > 1) {
+    const u32 mid = (lo + hi) >> 1;
+    if (T.ct0[mid] <= c) lo = mid;
+    else hi = mid;
+  }
+  const u32 e = T.exponent[lo];
+  const u64* src = A.in + (size_t)(T.src0[lo] + (c - T.ct0[lo])) * A.in_stride;
+  const u32 o = (u32)w & (N - 1);
+  const size_t row = w - o;
+  const u32 j = __brev(o) >> (32 - A.logn);
+  const u32 s = __brev((j * e + ((e - 1) >> 1)) & (N - 1)) >> (32 - A.logn);   // mod 2^32 keeps the low logn bits
+  const size_t part1 = (size_t)A.L << A.logn;
+  u64 v0 = src[row + s];
+  u64* d0 = A.out0 + (size_t)blockIdx.y * A.out0_stride;
+  if (A.sum) {
+    const u64 p = A.limbs[A.ids[row >> A.logn]].p;
+    v0 = csub(v0 + src[w], p);
+    d0[part1 + w] = src[part1 + w];
+  }
+  d0[w] = v0;
+  if (A.out1) A.out1[(size_t)blockIdx.y * A.out1_stride + w] = src[part1 + row + s];
+}
+
 // Poly::substitute, PowerBasis branch (rq/mod.rs:390-408): coefficient j of x^j moves to x^(j*e mod 2N), i.e. to slot
 // (j*e) & (N-1), negated when bit N of j*e is set (x^N = -1).  e is odd, so the map is a bijection: a scatter in which
 // every output word is written exactly once (reads coalesced, writes strided by e).
@@ -1957,6 +2001,41 @@ void launch_gather(const u64* in, u64* out, size_t n_rows, const int* perm, u32 
   if (!n) return;
   gather_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(in, out, n, perm, logn);
   g_launches++;
+}
+
+void launch_substitute_ntt(const u64* in, size_t in_stride, u64* out0, size_t out0_stride, u64* out1,
+                           size_t out1_stride, const u32* exponent, const u32* source, u32 cts, u32 L, bool sum,
+                           const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st) {
+  const size_t words = (size_t)L << logn;
+  if (!words || !cts) return;
+  SubstArgs A;
+  std::memset(&A, 0, sizeof(A));
+  A.in = in; A.in_stride = in_stride;
+  A.out1 = out1; A.out0_stride = out0_stride; A.out1_stride = out1_stride;
+  A.L = L; A.logn = logn; A.sum = sum ? 1 : 0; A.limbs = limbs;
+  copy_ids(A.ids, ids);
+  const dim3 block(256);
+  u32 c0 = 0;   // first ciphertext of the pending launch
+  auto flush = [&](u32 end) {
+    A.out0 = out0 + (size_t)c0 * out0_stride;
+    A.out1 = out1 ? out1 + (size_t)c0 * out1_stride : nullptr;
+    subst_kernel<<<dim3((unsigned)((words + 255) / 256), end - c0), block, 0, st>>>(A);
+    g_launches++;
+    A.T.n = 0;
+    c0 = end;
+  };
+  for (u32 c = 0; c < cts; c++) {
+    if (c - c0 == 65535) flush(c);   // gridDim.y
+    const u32 e = exponent[c], s = source ? source[c] : c;
+    const u32 r = A.T.n;
+    if (r && A.T.exponent[r - 1] == e && A.T.src0[r - 1] + (c - c0 - A.T.ct0[r - 1]) == s) continue;   // extends run r-1
+    if (r == kSubstRuns) flush(c);
+    A.T.ct0[A.T.n] = c - c0;
+    A.T.exponent[A.T.n] = e;
+    A.T.src0[A.T.n] = s;
+    A.T.n++;
+  }
+  flush(cts);
 }
 
 void launch_substitute_power(const u64* in, u64* out, size_t n_rows, u32 exponent, const RowIds& ids,

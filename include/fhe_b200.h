@@ -512,6 +512,32 @@ int fhe_b200_galois_keyed(const fhe_b200_batch* ct, uint32_t exponent, const fhe
  * INVALID_ARGUMENT. */
 int fhe_b200_expand_keyed(const fhe_b200_batch* ct, uint32_t size, const fhe_b200_ksk* const* gks, uint32_t n_gks,
                           uint32_t n_sets, const uint32_t* set_index, fhe_b200_batch* out, void* stream);
+/* ---- per-ciphertext Galois exponents --------------------------------------------------------------------
+ * Many rotations in one call: of one ciphertext by many steps, or of many ciphertexts by their own steps.  gks[k] is
+ * the Galois key for exponents[k] (the caller vouches that they match, as for fhe_b200_galois); entry j of out is, word
+ * for word, fhe_b200_galois(ct[src_j], exponents[key_index[j]], gks[key_index[j]]) with src_j = source[j], or j when
+ * source is NULL (then ct.count must equal out.count).  source and key_index are host memory with out.count entries,
+ * read during the call only.  Each exponent is reduced mod 2N; an even one -> INVALID_EXPONENT.  INVALID_ARGUMENT: a
+ * NULL key list, key, exponent list or index, n_keys == 0, key_index[j] >= n_keys, source[j] >= ct.count, out aliasing
+ * ct, keys that differ in key level, digit count or base.  Every other error is fhe_b200_galois's, and every check runs
+ * before anything is enqueued.  The substitution reads each output's exponent and source from its kernel parameters: no
+ * table is built, nothing is allocated beyond the stream-ordered scratch and nothing is synchronised. */
+int fhe_b200_galois_many(const fhe_b200_batch* ct, const uint32_t* source, const fhe_b200_ksk* const* gks,
+                         const uint32_t* exponents, uint32_t n_keys, const uint32_t* key_index, fhe_b200_batch* out,
+                         void* stream);
+/* EvaluationKey::computes_inner_sum (keys/evaluation_key.rs:56-100) of every ciphertext of ct into out (same shape,
+ * must not alias ct; ct is left unchanged; out becomes NTT).  gks holds n_gks = log2 N keys: the Galois keys of the
+ * column rotations by 1, 2, 4, ..., N/4 (exponents 3^i mod 2N), then of the row rotation (2N - 1); any other n_gks or a
+ * NULL key -> INVALID_ARGUMENT.  Levels and leveled keys as in fhe_b200_galois.  Each step is one substitution kernel
+ * that also forms sigma(c0) + c0 and one key switch that adds in place: no separate add launch, no host
+ * synchronisation between steps. */
+int fhe_b200_inner_sum(const fhe_b200_batch* ct, const fhe_b200_ksk* const* gks, uint32_t n_gks, fhe_b200_batch* out,
+                       void* stream);
+/* fhe_b200_inner_sum of every ciphertext with its own key set: gks[s * n_gks + l] is the key of step l of key set s
+ * and set_index[c] the key set of ciphertext c (host memory, ct.count entries).  The keys of one step must share their
+ * key level, digit count and base.  n_sets == 0, a NULL set_index or set_index[c] >= n_sets -> INVALID_ARGUMENT. */
+int fhe_b200_inner_sum_keyed(const fhe_b200_batch* ct, const fhe_b200_ksk* const* gks, uint32_t n_gks, uint32_t n_sets,
+                             const uint32_t* set_index, fhe_b200_batch* out, void* stream);
 /* rq::scaler::Scaler::scale with the level's multiplication scalers (rq/scaler.rs:55-127):
  * which = 0: extender (level basis -> multiplication basis, factor 1),
  * which = 1: down scaler (multiplication basis -> level basis, factor t/Q).

@@ -708,13 +708,47 @@ class EvaluationKey {
     for (uint32_t i = 1; i < n / 2; i *= 2) ok = ok && gk_.count(column_exponent(i)) != 0;
     return ok;
   }
-  // EvaluationKey::computes_inner_sum (evaluation_key.rs:56-100)
-  Ciphertext computes_inner_sum(const Ciphertext& ct) const {
+  // the keys of the inner sum's log2 N steps: column rotations by 1, 2, 4, ..., N/4, then the row rotation
+  std::vector<const fhe_b200_ksk*> inner_sum_keys() const {
     if (!supports_inner_sum()) throw Error(FHE_B200_INVALID_ARGUMENT, "EvaluationKeyError: inner sum not supported by this key");
     const uint32_t n = (uint32_t)par_->degree();
-    Ciphertext out = ct.clone();
-    for (uint32_t i = 1; i < n / 2; i *= 2) out += at(column_exponent(i)).relinearize(out);
-    out += at(2 * n - 1).relinearize(out);
+    std::vector<const fhe_b200_ksk*> keys;
+    for (uint32_t i = 1; i < n / 2; i *= 2) keys.push_back(at(column_exponent(i)).ksk->handle());
+    keys.push_back(at(2 * n - 1).ksk->handle());
+    return keys;
+  }
+  // EvaluationKey::computes_inner_sum (evaluation_key.rs:56-100) of every ciphertext of ct, one device call
+  Ciphertext computes_inner_sum(const Ciphertext& ct) const {
+    const std::vector<const fhe_b200_ksk*> keys = inner_sum_keys();
+    Ciphertext out(ct.par(), ct.count(), 2, ct.level(), Representation::Ntt, ct.stream());
+    check(fhe_b200_inner_sum(ct.handle(), keys.data(), (uint32_t)keys.size(), out.handle(), ct.stream()));
+    return out;
+  }
+  // rotates_columns_by(ct_q, steps[i]) for every step and every ciphertext of ct (Q = ct.count()) in one device call
+  // (fhe_b200_galois_many): entry i*Q + q of the result is ciphertext q rotated by steps[i]
+  Ciphertext rotates_columns_by_many(const Ciphertext& ct, const std::vector<uint32_t>& steps) const {
+    std::vector<const fhe_b200_ksk*> keys;
+    std::vector<uint32_t> exps, index, source;
+    const uint32_t q = ct.count();
+    for (uint32_t i : steps) {
+      const uint32_t e = column_exponent(i);
+      const GaloisKey& gk = at(e);
+      uint32_t k = 0;
+      while (k < exps.size() && exps[k] != e) k++;
+      if (k == exps.size()) {
+        exps.push_back(e);
+        keys.push_back(gk.ksk->handle());
+      }
+      for (uint32_t j = 0; j < q; j++) {
+        index.push_back(k);
+        source.push_back(j);
+      }
+    }
+    if (keys.empty()) keys.push_back(nullptr);   // no steps: refused by the call
+    Ciphertext out(ct.par(), std::max<uint32_t>((uint32_t)index.size(), 1), 2, ct.level(), Representation::Ntt,
+                   ct.stream());
+    check(fhe_b200_galois_many(ct.handle(), source.data(), keys.data(), exps.data(), (uint32_t)exps.size(),
+                               index.data(), out.handle(), ct.stream()));
     return out;
   }
   // evaluation_key.rs:175-189
@@ -1009,6 +1043,38 @@ inline Ciphertext rotates_columns_by_keyed(const Ciphertext& ct, const std::vect
 inline Ciphertext rotates_rows_keyed(const Ciphertext& ct, const std::vector<const EvaluationKey*>& eks,
                                      const std::vector<uint32_t>& index) {
   return galois_keyed(ct, keyed_detail::galois_of(eks, 2 * (uint32_t)ct.par()->degree() - 1), index);
+}
+// GaloisKey::relinearize of ciphertext source[j] (j when source is empty) with gks[index[j]], each key with its own
+// exponent (fhe_b200_galois_many)
+inline Ciphertext galois_many(const Ciphertext& ct, const std::vector<const GaloisKey*>& gks,
+                              const std::vector<uint32_t>& index, const std::vector<uint32_t>& source = {}) {
+  const uint32_t count = source.empty() ? ct.count() : (uint32_t)source.size();
+  keyed_detail::check_index(index, count);
+  const auto h = keyed_detail::handles(gks, [](const GaloisKey& k) { return k.ksk->handle(); });
+  std::vector<uint32_t> exps;
+  for (const GaloisKey* g : gks) exps.push_back(g ? g->exponent : 1);
+  if (exps.empty()) exps.push_back(1);
+  Ciphertext out(ct.par(), std::max<uint32_t>(count, 1), 2, ct.level(), Representation::Ntt, ct.stream());
+  check(fhe_b200_galois_many(ct.handle(), source.empty() ? nullptr : source.data(), h.data(), exps.data(),
+                             (uint32_t)gks.size(), index.data(), out.handle(), ct.stream()));
+  return out;
+}
+// EvaluationKey::computes_inner_sum of ciphertext j with eks[index[j]] (fhe_b200_inner_sum_keyed)
+inline Ciphertext computes_inner_sum_keyed(const Ciphertext& ct, const std::vector<const EvaluationKey*>& eks,
+                                           const std::vector<uint32_t>& index) {
+  keyed_detail::check_index(index, ct.count());
+  std::vector<const fhe_b200_ksk*> keys;
+  uint32_t n_gks = 0;
+  for (const EvaluationKey* ek : eks) {
+    const std::vector<const fhe_b200_ksk*> k = ek->inner_sum_keys();
+    n_gks = (uint32_t)k.size();
+    keys.insert(keys.end(), k.begin(), k.end());
+  }
+  if (keys.empty()) keys.push_back(nullptr);
+  Ciphertext out(ct.par(), ct.count(), 2, ct.level(), Representation::Ntt, ct.stream());
+  check(fhe_b200_inner_sum_keyed(ct.handle(), keys.data(), n_gks, (uint32_t)eks.size(), index.data(), out.handle(),
+                                 ct.stream()));
+  return out;
 }
 // EvaluationKey::expands of query q with eks[index[q]]: `size` batches, batch i holding output i of every query
 inline std::vector<Ciphertext> expands_keyed(const Ciphertext& ct, const std::vector<const EvaluationKey*>& eks,
