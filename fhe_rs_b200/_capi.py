@@ -109,6 +109,9 @@ SYMBOLS = {
     "fhe_b200_galois_many": (_i, [_vp, _pu32, _pp, _pu32, _u32, _pu32, _vp, _vp]),
     "fhe_b200_inner_sum": (_i, [_vp, _pp, _u32, _vp, _vp]),
     "fhe_b200_inner_sum_keyed": (_i, [_vp, _pp, _u32, _u32, _pu32, _vp, _vp]),
+    "fhe_b200_batch_sum": (_i, [_vp, _u32, _i, _vp, _vp]),
+    "fhe_b200_dot_product": (_i, [_vp, _vp, _u32, _vp, _vp, _vp]),
+    "fhe_b200_dot_product_keyed": (_i, [_vp, _vp, _u32, _pp, _u32, _pu32, _vp, _vp]),
     "fhe_b200_scale": (_i, [_vp, _i, _vp, _vp]),
     "fhe_b200_poly_packed_bytes": (_i, [_vp, _u32, C.POINTER(C.c_size_t)]),
     "fhe_b200_batch_packed_bytes": (_i, [_vp, C.POINTER(C.c_size_t)]),
@@ -119,6 +122,7 @@ SYMBOLS = {
     "fhe_b200_fold": (_i, [_vp, _u32, _u32, _vp, _vp]),
     "fhe_b200_sync": (_i, [_vp]),
     "fhe_b200_launch_count": (_u64, []),
+    "fhe_b200_ntt_row_count": (_u64, [_i]),
     "fhe_b200_debug_scaler_tables": (_i, [_vp, _u32, _i, _pu32, _pu32, _pu32] + [_vp] * 8),
     "fhe_b200_debug_ntt_tables": (_i, [_vp, _u64, _vp, _vp, _vp, _vp, _pu64]),
     "fhe_b200_debug_expansion_monomial": (_i, [_vp, _u32, _u32, _vp]),

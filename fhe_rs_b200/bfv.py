@@ -27,7 +27,7 @@ __all__ = ["BfvParameters", "BfvParametersBuilder", "Ciphertext", "KeySwitchingK
            "transcode_bidirectional", "transcode_to_bytes", "transcode_from_bytes", "key_switch_keyed",
            "relinearizes_keyed", "multiply_keyed", "galois_keyed", "rotates_columns_by_keyed", "rotates_rows_keyed",
            "expands_keyed", "expands_batch_keyed", "external_products_keyed", "galois_many",
-           "computes_inner_sum_keyed"]
+           "computes_inner_sum_keyed", "dot_product", "dot_product_keyed"]
 
 
 def _release(free_name: str, handle) -> None:
@@ -242,7 +242,7 @@ class Ciphertext:
         h = C.c_void_p()
         f = _capi.lib().fhe_b200_batch_alloc_mul_basis if mul_basis else _capi.lib().fhe_b200_batch_alloc
         check(f(par._h, count, parts, level, repr, C.byref(h)))
-        self._h, self.par, self.stream = h, par, stream
+        self._h, self.par, self.stream, self.mul_basis = h, par, stream, mul_basis
 
     def __del__(self):
         h, self._h = getattr(self, "_h", None), None
@@ -446,6 +446,23 @@ class Ciphertext:
         out = self.clone()
         check(_capi.lib().fhe_b200_neg(out._h, out.stream))
         return out
+
+    def sum(self, n_terms: Optional[int] = None, out: Optional["Ciphertext"] = None) -> "Ciphertext":
+        """Ciphertext += folded over runs (bfv/ops/mod.rs:54-69): entry g of the result is the sum of entries
+        g*n_terms .. g*n_terms + n_terms - 1.  n_terms None sums the whole batch into one ciphertext.  The result
+        has this batch's parts, level, representation and basis (the multiplication basis included).  With `out`, the
+        sums are added to out's entries and out is returned.  One device call (fhe_b200_batch_sum)."""
+        count = self.count
+        n = count if n_terms is None else int(n_terms)
+        if n <= 0 or count % n:
+            raise FheError(_capi.INVALID_ARGUMENT, "a batch of %d entries does not split into runs of %s" % (count, n_terms))
+        if out is None:
+            c, p, lv, _, r = self._info()
+            res = Ciphertext(self.par, c // n, p, lv, r, self.stream, self.mul_basis)
+        else:
+            res = out
+        check(_capi.lib().fhe_b200_batch_sum(self._h, n, 0 if out is None else 1, res._h, self.stream))
+        return res
 
     def __mul__(self, rhs: "Ciphertext") -> "Ciphertext":
         """&Ciphertext * &Ciphertext, no relinearization (ops/mod.rs:259-358): n x m parts -> n + m - 1 parts."""
@@ -1611,4 +1628,39 @@ def external_products_keyed(cts: Ciphertext, rgsws: Sequence["RGSWCiphertext"], 
     pb = cts.clone().into_power_basis()
     out = key_switch_keyed(pb, 0, [r.ksk0 for r in rgsws], index)
     out += key_switch_keyed(pb, 1, [r.ksk1 for r in rgsws], index)
+    return out
+
+
+# ---- dot products of ciphertext vectors (examples/mulpir.rs:176-183): sum_i a[i] * b[i] with one relinearization
+# and one switch_to_level per group, in one device call.
+
+def _dot_groups(a: Ciphertext, b: Ciphertext, n_terms: int) -> int:
+    n = int(n_terms)
+    count = max(a.count, b.count)
+    if n <= 0 or count % n:
+        raise FheError(_capi.INVALID_ARGUMENT, "DotProductError::OperandCountMismatch: %d entries, n_terms %s"
+                       % (count, n_terms))
+    return count // n
+
+
+def dot_product(a: Ciphertext, b: Ciphertext, n_terms: int, rk: Optional[RelinearizationKey] = None,
+                level: Optional[int] = None) -> Ciphertext:
+    """out[g] = sum_{i < n_terms} a[g*n_terms + i] * b[g*n_terms + i], relinearized with `rk` (3 parts without one)
+    and switched to `level` (default: the operands' level).  Either operand may hold n_terms entries only, shared by
+    every group.  Words equal the reference's loop of mul, +=, relinearizes and switch_to_level (fhe_b200_dot_product)."""
+    groups = _dot_groups(a, b, n_terms)
+    out = Ciphertext(a.par, groups, 2 if rk is not None else 3, a.level if level is None else level, NTT, a.stream)
+    check(_capi.lib().fhe_b200_dot_product(a._h, b._h, int(n_terms), rk.ksk._h if rk is not None else None, out._h,
+                                           a.stream))
+    return out
+
+
+def dot_product_keyed(a: Ciphertext, b: Ciphertext, n_terms: int, rks: Sequence[RelinearizationKey], index,
+                      level: Optional[int] = None) -> Ciphertext:
+    """dot_product with group g relinearized by rks[index[g]]: one key index per group, not per term
+    (fhe_b200_dot_product_keyed)"""
+    groups = _dot_groups(a, b, n_terms)
+    args = _keyed_args([rk.ksk for rk in rks], index, groups)
+    out = Ciphertext(a.par, groups, 2, a.level if level is None else level, NTT, a.stream)
+    check(_capi.lib().fhe_b200_dot_product_keyed(a._h, b._h, int(n_terms), *args, out._h, a.stream))
     return out

@@ -839,6 +839,7 @@ extern "C" {
 const char* fhe_b200_version(void) { return "fhe_b200 0.1 (sm_90a)"; }
 const char* fhe_b200_last_error(void) { return g_last_error.c_str(); }
 uint64_t fhe_b200_launch_count(void) { return g_launches.load(); }
+uint64_t fhe_b200_ntt_row_count(int inverse) { return g_ntt_rows[inverse ? 1 : 0].load(); }
 
 static int params_build(int device, uint32_t degree, const std::vector<u64>& moduli, const uint8_t* pt,
                         uint32_t pt_len, const uint64_t* psi, fhe_b200_params** out) {
@@ -1241,6 +1242,28 @@ int fhe_b200_dot_product_scalar(const fhe_b200_batch* cts, const fhe_b200_batch*
              cts->par->d_limbs, cts->par->logn, (cudaStream_t)stream);
   FHE_CUDA(cudaGetLastError());
   out->repr = FHE_B200_NTT;
+  API_END
+}
+
+// AddAssign<&Ciphertext> (ops/mod.rs:54-69) folded over each run of n_terms entries, from out[g] or from
+// Ciphertext::zero: one segment_sum launch for the whole batch.  It holds no scratch, so it needs no chunks.
+int fhe_b200_batch_sum(const fhe_b200_batch* in, uint32_t n_terms, int accumulate, fhe_b200_batch* out,
+                       void* stream) {
+  API_BEGIN
+  REQUIRE(in && out && in != out, FHE_B200_INVALID_ARGUMENT, "null or aliased argument");
+  REQUIRE(n_terms > 0, FHE_B200_INVALID_ARGUMENT, "a sum takes at least one term");
+  REQUIRE(in->count == (size_t)out->count * n_terms, FHE_B200_INVALID_ARGUMENT,
+          "the input must hold n_terms entries per output entry");
+  REQUIRE(in->par == out->par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch: batches use different parameters");
+  REQUIRE(in->parts == out->parts, FHE_B200_BAD_POLY_COUNT, "input and output part counts differ");
+  check_same(in, out);
+  if (accumulate) need_repr(out, in->repr);
+  DeviceGuard g(in->par);
+  const size_t W = in->words_per_ct();
+  launch_segment_sum(in->d, W, n_terms, out->d, W, nullptr, 0, in->parts * in->limbs, out->count, W, accumulate != 0,
+                     ids_of(in), in->par->d_limbs, in->par->logn, (cudaStream_t)stream);
+  FHE_CUDA(cudaGetLastError());
+  out->repr = in->repr;
   API_END
 }
 
@@ -2470,6 +2493,104 @@ int fhe_b200_mul_relin_keyed(const fhe_b200_batch* a, const fhe_b200_batch* b, c
                              void* stream) {
   API_BEGIN
   mul_relin_run(a, b, key_list(rks, n_keys, key_index), mod_switch, out2, stream);
+  API_END
+}
+
+// out[g] = switch_to_level(out.level, relinearizes(sum_i a[g*n + i] * b[g*n + i])) (examples/mulpir.rs:176-183; rk
+// null: the 3-part sum).  An operand of n_terms entries is shared by every group.  The chunks run over groups, so the
+// terms of one group stay on one stream; inside a chunk, slices of at most chunk_size() products go through mul_core
+// (power basis, no forward NTT) and segment_sum adds them into the group accumulator.  The NTT is linear on canonical
+// residues, so transforming the sum once gives the words of the reference's sum of transformed products; c2 stays in
+// power basis for the key switch, as in mul_relin.
+static void dot_product_run(const fhe_b200_batch* a, const fhe_b200_batch* b, uint32_t n_terms, const KeySet* rk,
+                            fhe_b200_batch* out, void* stream) {
+  REQUIRE(a && b && out && a != out && b != out, FHE_B200_INVALID_ARGUMENT, "null or aliased argument");
+  REQUIRE(!rk || rk->keys[0], FHE_B200_INVALID_ARGUMENT, "null key");
+  REQUIRE(a->par == b->par && a->par == out->par, FHE_B200_CONTEXT_MISMATCH,
+          "ParameterMismatch: batches use different parameters");
+  REQUIRE(!a->mul_basis && !b->mul_basis && !out->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
+  const u32 P = rk ? 2 : 3;
+  REQUIRE(a->parts == 2 && b->parts == 2 && out->parts == P, FHE_B200_BAD_POLY_COUNT,
+          rk ? "MultiplicationPolynomialCount: expected 2 x 2 -> 2" : "MultiplicationPolynomialCount: expected 2 x 2 -> 3");
+  const size_t total = (size_t)out->count * n_terms;
+  REQUIRE(n_terms > 0 && (a->count == total || a->count == n_terms) && (b->count == total || b->count == n_terms),
+          FHE_B200_INVALID_ARGUMENT, "DotProductError::OperandCountMismatch");
+  REQUIRE(a->level == b->level, FHE_B200_INVALID_LEVEL, "InvalidLevel: operands are at different levels");
+  REQUIRE(out->level >= a->level, FHE_B200_INVALID_LEVEL, "InvalidLevel: output below the operand level");
+  need_repr(a, FHE_B200_NTT);
+  need_repr(b, FHE_B200_NTT);
+  if (rk) check_ksks(*rk, a->par, a->level, out->count);
+  const fhe_b200_params* par = a->par;
+  DeviceGuard g(par);
+  const LevelData& lv = par->level(a->level);
+  const LevelData& ol = par->level(out->level);
+  const u32 L = lv.L, logn = par->logn, S = chunk_size();
+  const size_t row = (size_t)1 << logn, W = 2 * L * row, Wo = P * ol.L * row;
+  ChunkRunner chunks(par, out->count, (cudaStream_t)stream, std::max(1u, S / n_terms));
+  chunks.run([&](u32 g0, u32 ng, cudaStream_t st) {
+    Workspace ws(par, st);
+    // terms of one group per slice: a chunk of several groups holds at most S products and takes one slice
+    const u32 tps = ng > 1 ? n_terms : std::min(S, n_terms);
+    // the products of the chunk's terms [i0, i0 + m) of each group: a shared operand is repeated ng times
+    auto operand = [&](const fhe_b200_batch* x, u32 i0) -> const u64* {
+      if (x->count == total) return x->d + ((size_t)g0 * n_terms + i0) * W;
+      if (ng == 1) return x->d + (size_t)i0 * W;
+      const size_t run = (size_t)n_terms * W;
+      u64* rep = ws.words(ng * run);
+      FHE_CUDA(cudaMemcpyAsync(rep, x->d, run * 8, cudaMemcpyDeviceToDevice, st));
+      for (u32 k = 1; k < ng; k *= 2)
+        FHE_CUDA(cudaMemcpyAsync(rep + k * run, rep, std::min(k, ng - k) * run * 8, cudaMemcpyDeviceToDevice, st));
+      return rep;
+    };
+    const bool direct = out->level == a->level;
+    u64* o = direct ? out->d + (size_t)g0 * Wo : ws.words(ng * P * L * row);
+    u64* c2 = rk ? ws.words(ng * L * row) : nullptr;
+    u64* prod = ws.words((size_t)ng * tps * 3 * L * row);
+    for (u32 i0 = 0; i0 < n_terms; i0 += tps) {
+      const u32 m = std::min(tps, n_terms - i0);
+      {
+        Workspace slice(par, st);
+        mul_core(par, lv, operand(a, i0), operand(b, i0), ng * m, prod, nullptr, 0, slice, st);
+      }
+      // (c0, c1[, c2]) into o, c2 into its own buffer when it is relinearized
+      launch_segment_sum(prod, 3 * L * row, m, o, P * L * row, c2, L * row, P * L, ng, 3 * L * row, i0 > 0,
+                         lv.ctx_ids, par->d_limbs, logn, st);
+    }
+    if (rk) {
+      // relinearization_key.rs:70-103 on the sum: (c0, c1) to NTT, c2 switched from the power basis
+      launch_ntt(o, o, ng * 2 * L, lv.ctx_ids, par->d_limbs, logn, false, 1, false, st);
+      key_switch_apply(par, rk->from(g0), c2, ng, o, 1, nullptr, ws, st);
+      if (!direct) launch_ntt(o, o, ng * 2 * L, lv.ctx_ids, par->d_limbs, logn, true, 1, false, st);
+    }
+    // Ciphertext::switch_to_level (ciphertext.rs:164-186): each switch_down goes through the power basis; the
+    // transforms between two of them cancel (backward(forward(x)) == x for reduced x), so only the last one runs
+    u64* cur = o;
+    for (u32 l = a->level; l < out->level; l++) {
+      const LevelData& from = par->level(l);
+      u64* nxt = l + 1 == out->level ? out->d + (size_t)g0 * Wo : ws.words(ng * P * (from.L - 1) * row);
+      launch_switch_down(from.sd, cur, nxt, ng * P, from.L, from.ctx_ids, par->d_limbs, logn, st);
+      cur = nxt;
+    }
+    if (!rk || !direct) launch_ntt(cur, cur, ng * P * ol.L, ol.ctx_ids, par->d_limbs, logn, false, 1, false, st);
+  });
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
+}
+
+int fhe_b200_dot_product(const fhe_b200_batch* a, const fhe_b200_batch* b, uint32_t n_terms, const fhe_b200_ksk* rk,
+                         fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  const KeySet K{&rk, 1, nullptr};
+  dot_product_run(a, b, n_terms, rk ? &K : nullptr, out, stream);
+  API_END
+}
+
+int fhe_b200_dot_product_keyed(const fhe_b200_batch* a, const fhe_b200_batch* b, uint32_t n_terms,
+                               const fhe_b200_ksk* const* rks, uint32_t n_keys, const uint32_t* key_index,
+                               fhe_b200_batch* out, void* stream) {
+  API_BEGIN
+  const KeySet K = key_list(rks, n_keys, key_index);
+  dot_product_run(a, b, n_terms, &K, out, stream);
   API_END
 }
 

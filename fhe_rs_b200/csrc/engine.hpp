@@ -10,6 +10,8 @@
 namespace fhe_b200 {
 
 extern std::atomic<unsigned long long> g_launches;
+// rows transformed by launch_ntt so far: [0] forward, [1] inverse (fhe_b200_ntt_row_count)
+extern std::atomic<unsigned long long> g_ntt_rows[2];
 
 // The FHE_B200_* environment switches (DESIGN.md, appendix), read once per process by switches() (ntt.cu).  Every
 // value the appendix lists is set by a bit-for-bit rerun test.
@@ -294,6 +296,14 @@ constexpr u32 kSumGroup = 64;
 void launch_shares_sum(const u64* const* src, u32 n_src, size_t src_stride, const u64* base, size_t base_stride,
                        u64* out, size_t out_stride, u32 items, size_t item_words, const RowIds& ids,
                        const LimbDev* limbs, u32 logn, cudaStream_t st, size_t out_row = 0);
+// Segment sums (AddAssign folded over runs, bfv/ops/mod.rs:54-69): for g < groups, out item g = (accumulate ? out item
+// g : 0) + sum_{i < n_terms} in item g * n_terms + i.  An item is item_words words of rows of limb (row %
+// limbs_per_poly); input item j starts at in + j * in_stride.  Rows r < split_rows of out item g are at out0 +
+// g * out0_stride + r * N, the others at out1 + g * out1_stride + (r - split_rows) * N (split_rows = item_words / N:
+// one output).  Every input word is read once and every output word reduced and written once.
+void launch_segment_sum(const u64* in, size_t in_stride, u32 n_terms, u64* out0, size_t out0_stride, u64* out1,
+                        size_t out1_stride, u32 split_rows, u32 groups, size_t item_words, bool accumulate,
+                        const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st);
 
 // bit (un)packing of power-basis rows (fhe-util/src/lib.rs:71-146): row r of `rows` uses nbits[r % limbs] bits per
 // coefficient; packed row r starts at byte  (r / limbs) * poly_bytes + offs[r % limbs]

@@ -1597,6 +1597,55 @@ __global__ void shares_sum_kernel(SumArgs A) {
       make_ulonglong2(reduce128_limb(lo0, hi0, M), reduce128_limb(lo1, hi1, M));
 }
 
+struct SegSumArgs {
+  const u64* in;               // input item j at in + j * in_stride
+  u64 *out0, *out1;            // rows r < split_rows of out item g at out0 + g * out0_stride + r * N, the rest in out1
+  size_t in_stride, out0_stride, out1_stride, item_words;
+  u32 n_terms, groups, split_rows, logn, limbs_per_poly, accumulate;
+  const LimbDev* limbs;
+  unsigned short ids[kMaxPos];
+};
+// out[g] = (accumulate ? out[g] : 0) + sum_i in[g * n_terms + i], two words per thread.  The words are canonical
+// (< 2^62), so the 128-bit sum with a carry count holds any n_terms < 2^32 (< 2^94) and is reduced once.  Memory
+// bound: four terms (eight words) in flight per trip; the branch on the row only picks the output buffer.
+__global__ void segment_sum_kernel(SegSumArgs A) {
+  const size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 2;
+  if (i >= (size_t)A.groups * A.item_words) return;
+  const size_t g = i / A.item_words, w = i % A.item_words;
+  const u32 r = (u32)(w >> A.logn), c = (u32)w & ((1u << A.logn) - 1);
+  const LimbDev& M = A.limbs[A.ids[r % A.limbs_per_poly]];
+  u64* o = r < A.split_rows ? A.out0 + g * A.out0_stride + ((size_t)r << A.logn) + c
+                            : A.out1 + g * A.out1_stride + ((size_t)(r - A.split_rows) << A.logn) + c;
+  u64 lo0 = 0, lo1 = 0, hi0 = 0, hi1 = 0;
+  if (A.accumulate) {
+    const ulonglong2 b = *reinterpret_cast<const ulonglong2*>(o);
+    lo0 = b.x;
+    lo1 = b.y;
+  }
+  const u64* p = A.in + g * A.n_terms * A.in_stride + w;
+  u32 k = 0;
+  for (; k + 4 <= A.n_terms; k += 4) {
+    ulonglong2 v[4];
+#pragma unroll
+    for (int j = 0; j < 4; j++) v[j] = *reinterpret_cast<const ulonglong2*>(p + (size_t)(k + j) * A.in_stride);
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      lo0 += v[j].x;
+      hi0 += lo0 < v[j].x;
+      lo1 += v[j].y;
+      hi1 += lo1 < v[j].y;
+    }
+  }
+  for (; k < A.n_terms; k++) {
+    const ulonglong2 v = *reinterpret_cast<const ulonglong2*>(p + (size_t)k * A.in_stride);
+    lo0 += v.x;
+    hi0 += lo0 < v.x;
+    lo1 += v.y;
+    hi1 += lo1 < v.y;
+  }
+  *reinterpret_cast<ulonglong2*>(o) = make_ulonglong2(reduce128_limb(lo0, hi0, M), reduce128_limb(lo1, hi1, M));
+}
+
 void copy_ids(unsigned short* dst, const RowIds& ids) {
   for (int i = 0; i < kMaxPos; i++) dst[i] = ids.ids[i];
 }
@@ -1659,6 +1708,21 @@ void launch_shares_sum(const u64* const* src, u32 n_src, size_t src_stride, cons
     shares_sum_kernel<<<(unsigned)((total / 2 + 255) / 256), 256, 0, st>>>(A);
     g_launches++;
   }
+}
+
+void launch_segment_sum(const u64* in, size_t in_stride, u32 n_terms, u64* out0, size_t out0_stride, u64* out1,
+                        size_t out1_stride, u32 split_rows, u32 groups, size_t item_words, bool accumulate,
+                        const RowIds& ids, const LimbDev* limbs, u32 logn, cudaStream_t st) {
+  const size_t total = (size_t)groups * item_words;
+  if (!total) return;
+  SegSumArgs A;
+  A.in = in; A.out0 = out0; A.out1 = out1;
+  A.in_stride = in_stride; A.out0_stride = out0_stride; A.out1_stride = out1_stride; A.item_words = item_words;
+  A.n_terms = n_terms; A.groups = groups; A.split_rows = split_rows; A.logn = logn;
+  A.limbs_per_poly = ids.limbs_per_poly; A.accumulate = accumulate ? 1 : 0; A.limbs = limbs;
+  copy_ids(A.ids, ids);
+  segment_sum_kernel<<<(unsigned)((total / 2 + 255) / 256), 256, 0, st>>>(A);
+  g_launches++;
 }
 
 void launch_encode_load(const u64* staged, u64* coeffs, u32 n_pt, size_t n_values, const u32* inv_map, bool is_signed,

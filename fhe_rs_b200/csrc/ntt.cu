@@ -16,6 +16,7 @@
 namespace fhe_b200 {
 
 std::atomic<unsigned long long> g_launches{0};
+std::atomic<unsigned long long> g_ntt_rows[2] = {{0}, {0}};
 
 const Switches& switches() {
   static const Switches s = [] {
@@ -487,6 +488,7 @@ void launch_ntt(const u64* in, u64* out, u32 n_rows, const RowIds& ids, const Li
                 bool inverse, u32 in_div, bool reduce_on_load, cudaStream_t st, bool lazy_out, bool digit_adjacent,
                 u32 n_dig) {
   if (n_rows == 0) return;
+  g_ntt_rows[inverse ? 1 : 0].fetch_add(n_rows, std::memory_order_relaxed);
   NttArgs a;
   a.in = in;
   a.out = out;

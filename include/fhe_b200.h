@@ -538,6 +538,40 @@ int fhe_b200_inner_sum(const fhe_b200_batch* ct, const fhe_b200_ksk* const* gks,
  * key level, digit count and base.  n_sets == 0, a NULL set_index or set_index[c] >= n_sets -> INVALID_ARGUMENT. */
 int fhe_b200_inner_sum_keyed(const fhe_b200_batch* ct, const fhe_b200_ksk* const* gks, uint32_t n_gks, uint32_t n_sets,
                              const uint32_t* set_index, fhe_b200_batch* out, void* stream);
+/* ---- sums over many ciphertexts --------------------------------------------------------------------------
+ * A run is n_terms consecutive entries: run g of a batch is entries g*n_terms .. g*n_terms + n_terms - 1, and an output
+ * batch of out.count entries takes one run each.  Every check runs before anything is enqueued. */
+/* Ciphertext += &Ciphertext (bfv/ops/mod.rs:54-69) folded over each run, from Ciphertext::zero (accumulate == 0) or
+ * from out's own entries: out[g] = (accumulate ? out[g] : 0) + sum_{i < n_terms} in[g*n_terms + i], for g < out.count.
+ * Any part count, either representation, and batches over the multiplication basis; out takes in's representation.
+ * Errors: in.count != out.count * n_terms, n_terms == 0, a NULL argument or out == in -> INVALID_ARGUMENT; parts that
+ * differ -> BAD_POLY_COUNT; levels that differ -> INVALID_LEVEL; another parameter set, or one batch over the
+ * multiplication basis and the other not -> CONTEXT_MISMATCH; accumulate into an out of the other representation ->
+ * INVALID_REPRESENTATION.  One kernel: each output word is accumulated in 128 bits and reduced once, so n_terms may
+ * reach 2^32 - 1.  The voting tally of examples/voting.rs:142-147 is one call with n_terms = the number of ballots. */
+int fhe_b200_batch_sum(const fhe_b200_batch* in, uint32_t n_terms, int accumulate, fhe_b200_batch* out, void* stream);
+/* The dot product of two ciphertext vectors, one relinearization per run (examples/mulpir.rs:176-183):
+ *   out[g] = switch_to_level(out.level, relinearizes(sum_{i < n_terms} a[g*n_terms + i] * b[g*n_terms + i]))
+ * Each term is &Ciphertext * &Ciphertext (bfv/ops/mod.rs:259-358) of two 2-part NTT ciphertexts, the sum is AddAssign
+ * (ops/mod.rs:54-69) from Ciphertext::zero.  rk == NULL: no relinearization, out is 3-part; otherwise out is 2-part,
+ * RelinearizationKey::relinearizes (relinearization_key.rs:70-103), with keys at another key level as in
+ * fhe_b200_relinearize.  out.level > a.level applies Ciphertext::switch_to_level (ciphertext.rs:164-186) to the result.
+ * Either operand may hold n_terms entries only, shared by every group, or out.count * n_terms (the rule of
+ * fhe_b200_dot_product_scalar).  The words equal the reference's loop of mul, +=, relinearizes and switch_to_level.
+ * Errors: operand parts other than 2 x 2, or out parts other than 3 (no key) / 2 -> BAD_POLY_COUNT; counts that fit
+ * neither rule, n_terms == 0, a NULL argument, out aliasing an operand -> INVALID_ARGUMENT; operands at different
+ * levels, out.level below a.level -> INVALID_LEVEL; POWER_BASIS operands -> INVALID_REPRESENTATION; another parameter
+ * set or a multiplication-basis batch -> CONTEXT_MISMATCH; the key as fhe_b200_relinearize checks it.
+ * The products are summed before their forward NTT (linear on canonical residues), so each group transforms 2 parts
+ * (with a key) or 3 instead of 3 per term, and c2 goes from the power basis straight into the key switch. */
+int fhe_b200_dot_product(const fhe_b200_batch* a, const fhe_b200_batch* b, uint32_t n_terms, const fhe_b200_ksk* rk,
+                         fhe_b200_batch* out, void* stream);
+/* fhe_b200_dot_product with group g relinearized by rks[key_index[g]]: many clients' MulPIR responses in one call.
+ * key_index holds one u32 per group (out.count entries, host memory), not per term; the key rules and errors are those
+ * of the other _keyed calls above. */
+int fhe_b200_dot_product_keyed(const fhe_b200_batch* a, const fhe_b200_batch* b, uint32_t n_terms,
+                               const fhe_b200_ksk* const* rks, uint32_t n_keys, const uint32_t* key_index,
+                               fhe_b200_batch* out, void* stream);
 /* rq::scaler::Scaler::scale with the level's multiplication scalers (rq/scaler.rs:55-127):
  * which = 0: extender (level basis -> multiplication basis, factor 1),
  * which = 1: down scaler (multiplication basis -> level basis, factor t/Q).
@@ -603,6 +637,10 @@ int fhe_b200_fold(const fhe_b200_batch* ct, uint32_t in_bits, uint32_t out_bits,
 int fhe_b200_sync(void* stream);
 /* kernels launched by this library in the calling process so far (bench.py "gpu_launches") */
 uint64_t fhe_b200_launch_count(void);
+/* polynomial rows (one limb of one polynomial) transformed by the batched NTT so far in the calling process:
+ * inverse == 0 forward, otherwise inverse.  Transforms fused into other kernels (the tensor product, the key switch
+ * digits) are not counted. */
+uint64_t fhe_b200_ntt_row_count(int inverse);
 
 /* ---- inspection of the host precompute (CPU-only tests of the parameter builder) -------
  * RnsScaler tables (rns/scaler.rs:52-73) of the level's extender (which=0), down scaler

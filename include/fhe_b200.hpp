@@ -1076,6 +1076,47 @@ inline Ciphertext computes_inner_sum_keyed(const Ciphertext& ct, const std::vect
                                  ct.stream()));
   return out;
 }
+// Ciphertext += folded over runs of n_terms entries (bfv/ops/mod.rs:54-69; n_terms 0: the whole batch), one
+// ciphertext per run (fhe_b200_batch_sum)
+inline Ciphertext batch_sum(const Ciphertext& in, uint32_t n_terms = 0) {
+  const uint32_t n = n_terms ? n_terms : in.count();
+  if (n == 0 || in.count() % n)
+    throw Error(FHE_B200_INVALID_ARGUMENT, "a batch of " + std::to_string(in.count()) + " entries does not split into runs of " +
+                                              std::to_string(n_terms));
+  Ciphertext out(in.par(), in.count() / n, in.len(), in.level(), in.representation(), in.stream());
+  check(fhe_b200_batch_sum(in.handle(), n, 0, out.handle(), in.stream()));
+  return out;
+}
+namespace keyed_detail {
+inline uint32_t dot_groups(const Ciphertext& a, const Ciphertext& b, uint32_t n_terms) {
+  const uint32_t count = std::max(a.count(), b.count());
+  if (n_terms == 0 || count % n_terms)
+    throw Error(FHE_B200_INVALID_ARGUMENT, "DotProductError::OperandCountMismatch");
+  return count / n_terms;
+}
+}  // namespace keyed_detail
+// sum_{i<n_terms} a[g*n_terms+i] * b[g*n_terms+i] for every group g, relinearized with rk (3 parts when rk is null) and
+// switched to `level` (-1: the operands' level); an operand of n_terms entries is shared (fhe_b200_dot_product)
+inline Ciphertext dot_product(const Ciphertext& a, const Ciphertext& b, uint32_t n_terms,
+                              const RelinearizationKey* rk = nullptr, int level = -1) {
+  const uint32_t groups = keyed_detail::dot_groups(a, b, n_terms);
+  Ciphertext out(a.par(), groups, rk ? 2 : 3, level < 0 ? a.level() : (uint32_t)level, Representation::Ntt, a.stream());
+  check(fhe_b200_dot_product(a.handle(), b.handle(), n_terms, rk ? rk->ksk->handle() : nullptr, out.handle(),
+                             a.stream()));
+  return out;
+}
+// dot_product with group g relinearized by rks[index[g]] (fhe_b200_dot_product_keyed)
+inline Ciphertext dot_product_keyed(const Ciphertext& a, const Ciphertext& b, uint32_t n_terms,
+                                    const std::vector<const RelinearizationKey*>& rks, const std::vector<uint32_t>& index,
+                                    int level = -1) {
+  const uint32_t groups = keyed_detail::dot_groups(a, b, n_terms);
+  keyed_detail::check_index(index, groups);
+  const auto h = keyed_detail::handles(rks, [](const RelinearizationKey& k) { return k.ksk->handle(); });
+  Ciphertext out(a.par(), groups, 2, level < 0 ? a.level() : (uint32_t)level, Representation::Ntt, a.stream());
+  check(fhe_b200_dot_product_keyed(a.handle(), b.handle(), n_terms, h.data(), (uint32_t)rks.size(), index.data(),
+                                   out.handle(), a.stream()));
+  return out;
+}
 // EvaluationKey::expands of query q with eks[index[q]]: `size` batches, batch i holding output i of every query
 inline std::vector<Ciphertext> expands_keyed(const Ciphertext& ct, const std::vector<const EvaluationKey*>& eks,
                                              const std::vector<uint32_t>& index, uint32_t size) {
