@@ -13,7 +13,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Dict, List, Optional, Sequence
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -26,7 +26,7 @@ __all__ = ["BfvParameters", "BfvParametersBuilder", "Ciphertext", "KeySwitchingK
            "Encoding", "Plaintext", "PlaintextVec", "SecretKey", "PublicKey", "EvaluationKeyBuilder",
            "transcode_bidirectional", "transcode_to_bytes", "transcode_from_bytes", "key_switch_keyed",
            "relinearizes_keyed", "multiply_keyed", "galois_keyed", "rotates_columns_by_keyed", "rotates_rows_keyed",
-           "expands_keyed", "expands_batch_keyed", "external_products_keyed", "galois_many",
+           "expands_keyed", "expands_batch_keyed", "external_products_keyed", "galois_many", "galois_many_hoisted",
            "computes_inner_sum_keyed", "dot_product", "dot_product_keyed"]
 
 
@@ -1196,6 +1196,14 @@ class EvaluationKey:
     def rotates_columns_by_many(self, ct: Ciphertext, steps: Sequence[int]) -> Ciphertext:
         """rotates_columns_by(ct_q, steps[i]) for every step and every ciphertext of ct (Q = ct.count) in one device call
         (fhe_b200_galois_many): entry i*Q + q of the result is ciphertext q rotated by steps[i]"""
+        return galois_many(ct, *self._many_args(ct, steps))
+
+    def rotates_columns_by_many_hoisted(self, ct: Ciphertext, steps: Sequence[int]) -> Ciphertext:
+        """rotates_columns_by_many, word for word, with each ciphertext's rotations computed from one digit
+        decomposition of it when it has two or more (fhe_b200_galois_many_hoisted)"""
+        return galois_many_hoisted(ct, *self._many_args(ct, steps))[0]
+
+    def _many_args(self, ct: Ciphertext, steps: Sequence[int]):
         two_n = 2 * self.par.degree()
         exps = [pow(3, int(i), two_n) for i in steps]
         for i, e in zip(steps, exps):
@@ -1206,7 +1214,7 @@ class EvaluationKey:
         gks = [self.gk[e] for e in keys]
         q = ct.count
         index = [keys.index(e) for e in exps for _ in range(q)]
-        return galois_many(ct, gks, index, [j for _ in exps for j in range(q)])
+        return gks, index, [j for _ in exps for j in range(q)]
 
 
 class EvaluationKeyBuilder:
@@ -1542,6 +1550,17 @@ def galois_keyed(ct: Ciphertext, gks: Sequence["GaloisKey"], index) -> Ciphertex
 def galois_many(ct: Ciphertext, gks: Sequence["GaloisKey"], index, source=None) -> Ciphertext:
     """GaloisKey.relinearize of ciphertext source[j] (j when source is None) with gks[index[j]], each key with its own
     exponent: one device call for many rotations of one ciphertext or of many (fhe_b200_galois_many)"""
+    return _galois_many(ct, gks, index, source, False)[0]
+
+
+def galois_many_hoisted(ct: Ciphertext, gks: Sequence["GaloisKey"], index, source=None) -> Tuple[Ciphertext, int]:
+    """galois_many, word for word, with the rotations of each source ciphertext that has two or more outputs computed
+    from one digit decomposition of its c1 (fhe_b200_galois_many_hoisted).  Returns the result and how many outputs
+    were hoisted.  Synchronises the stream once when any source has two or more outputs."""
+    return _galois_many(ct, gks, index, source, True)
+
+
+def _galois_many(ct, gks, index, source, hoisted):
     count = ct.count
     if source is not None:
         src = np.ascontiguousarray(np.asarray(source, dtype=np.int64).reshape(-1))
@@ -1554,8 +1573,13 @@ def galois_many(ct: Ciphertext, gks: Sequence["GaloisKey"], index, source=None) 
     keys, n, ix = _keyed_args([g.ksk for g in gks], index, count)
     exps = (C.c_uint32 * max(1, len(gks)))(*[int(g.exponent) & 0xFFFFFFFF for g in gks])
     out = Ciphertext(ct.par, max(count, 1), 2, ct.level, NTT, ct.stream)
-    check(_capi.lib().fhe_b200_galois_many(ct._h, sp, keys, exps, n, ix, out._h, ct.stream))
-    return out
+    if not hoisted:
+        check(_capi.lib().fhe_b200_galois_many(ct._h, sp, keys, exps, n, ix, out._h, ct.stream))
+        return out, 0
+    n_hoisted = C.c_uint32(0)
+    check(_capi.lib().fhe_b200_galois_many_hoisted(ct._h, sp, keys, exps, n, ix, out._h, C.byref(n_hoisted),
+                                                   ct.stream))
+    return out, n_hoisted.value
 
 
 def computes_inner_sum_keyed(ct: Ciphertext, eks: Sequence["EvaluationKey"], index) -> Ciphertext:

@@ -623,6 +623,18 @@ std::vector<KeyRange> key_ranges(const KeySet& K, u32 cts) {
   return out;
 }
 
+// Whether the digit transforms reduce their input on load.  The reference lazily reduces the digit modulo q_j before
+// its lazy transform; the forward butterflies accept any input below 4*q_j, so the reduction on load is only needed
+// when a digit (< max q_i) can reach 4 * min q_j (mixed modulus sizes).  The digits are those of the ciphertext level
+// (n_dig = its L), the rows those of the key level.
+bool digit_reduce(const fhe_b200_params* par, const fhe_b200_ksk* k) {
+  const u64 qmax = par->level(k->ct_level).q_max, qmin = par->level(k->ksk_level).q_min;
+  // The lifts of plaintext words (LevelData::lift_reduce) test only t > 4 * q_min - 1: the butterflies take [0, 4p)
+  // for any modulus, down to q_min = 193 < 2^8 (tests/test_gpu_client_edges.py).  The extra clause here changes the
+  // choice only when every modulus of the key level is below 2^10, which needs N <= 64.
+  return qmax > 4 * qmin - 1 || qmin < (1ull << 8);
+}
+
 // KeySwitchingKey::key_switch core on a contiguous power-basis buffer c2 [cts][L][N]
 // (key_switching_key.rs:241-270): out0/out1 (+ optional bases), rows (ct, j) at (ct*out_ct_rows + j).  The digit
 // transforms do not depend on the key; the inner product runs once per key range (key_ranges).
@@ -641,15 +653,8 @@ void key_switch_core(const fhe_b200_params* par, const KeySet& K, const u64* c2,
     launch_decompose(c2, dig, cts, L, k->log_base, par->logn, st);
     launch_ntt(dig, inter, cts * L, kl.ctx_ids, par->d_limbs, par->logn, false, 1, false, st, true);
   } else {
-  // digit broadcast (rq/mod.rs:563-586), then NTT of every (digit, limb) row.  The reference lazily reduces the
-  // digit modulo q_j before its lazy transform; the forward butterflies accept any input below 4*q_j, so the
-  // reduction on load is only needed when a digit (< max q_i) can reach 4 * min q_j (mixed modulus sizes).  The
-  // digits are those of the ciphertext level (n_dig = its L), the rows those of the key level.
-  const u64 qmax = par->level(k->ct_level).q_max, qmin = kl.q_min;
-  // The lifts of plaintext words (LevelData::lift_reduce) test only t > 4 * q_min - 1: the butterflies take [0, 4p)
-  // for any modulus, down to q_min = 193 < 2^8 (tests/test_gpu_client_edges.py).  The extra clause here changes the
-  // choice only when every modulus of the key level is below 2^10, which needs N <= 64.
-  const bool reduce = qmax > 4 * qmin - 1 || qmin < (1ull << 8);
+  // digit broadcast (rq/mod.rs:563-586), then NTT of every (digit, limb) row
+  const bool reduce = digit_reduce(par, k);
   // forward_vt_lazy (rq/mod.rs:580): the digits stay in [0,4q_j); the lazy accumulator of the inner product takes
   // any 64-bit operand and reduces once
   // with the TMA kernels the transform deposits the digits of one (ciphertext, limb) in adjacent rows, which the
@@ -667,6 +672,9 @@ void key_switch_core(const fhe_b200_params* par, const KeySet& K, const u64* c2,
   launch_ksmac(inter, ranges, base0, base1, out0, out1, L, Lk, out_ct_rows, kl.ctx_ids, par->d_limbs, par->logn, st,
                adjacent);
 }
+
+void key_switch_leveled_tail(const fhe_b200_params* par, const fhe_b200_ksk* k, u64* cur, u32 cts, u64* out,
+                             int base_mode, u64* base, Workspace& ws, cudaStream_t st);
 
 // key switch + the reference's post-processing (relinearization_key.rs:88-95, galois_key.rs:69-76):
 // when the key lives at a lower level number than the ciphertext (more moduli), the (c0, c1) pair is
@@ -687,6 +695,16 @@ void key_switch_apply(const fhe_b200_params* par, const KeySet& K, const u64* c2
   }
   u64* cur = ws.words((size_t)cts * 2 * Lk * row);
   key_switch_core(par, K, c2, cts, nullptr, nullptr, cur, cur + Lk * row, 2 * Lk, ws, st);
+  key_switch_leveled_tail(par, k, cur, cts, out, base_mode, base, ws, st);
+}
+
+// The tail of key_switch_apply for a leveled key: cur [cts][2][Lk][N] (NTT, the key level) is taken to power basis,
+// switched down to the ciphertext level, transformed back and written to or added into out as base_mode says.
+void key_switch_leveled_tail(const fhe_b200_params* par, const fhe_b200_ksk* k, u64* cur, u32 cts, u64* out,
+                             int base_mode, u64* base, Workspace& ws, cudaStream_t st) {
+  const LevelData& cl = par->level(k->ct_level);
+  const u32 L = cl.L, Lk = k->Lk, logn = par->logn;
+  const size_t row = (size_t)1 << logn;
   const LevelData& kl = par->level(k->ksk_level);
   launch_ntt(cur, cur, cts * 2 * Lk, kl.ctx_ids, par->d_limbs, logn, true, 1, false, st);
   for (u32 lv = k->ksk_level; lv < k->ct_level; lv++) {  // Poly::switch_down_to, rq/mod.rs:498-507
@@ -2758,9 +2776,8 @@ static std::vector<u32> galois_exponents(const fhe_b200_params* par, const u32* 
   return e;
 }
 
-// output j = GaloisKey::relinearize of ciphertext gk.source[j] (j without a source list) with key gk.key_of(j) for
-// its exponent gk.exps[key]
-static void galois_run(const fhe_b200_batch* ct, KeySet gk, fhe_b200_batch* out, void* stream) {
+// the argument checks of every Galois call; returns the exponents of gk.exps reduced mod 2N
+static std::vector<u32> galois_check(const fhe_b200_batch* ct, const KeySet& gk, const fhe_b200_batch* out) {
   REQUIRE(ct && gk.keys[0] && out && ct != out, FHE_B200_INVALID_ARGUMENT, "null or aliased argument");
   check_same(ct, out);
   REQUIRE(!ct->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
@@ -2774,16 +2791,26 @@ static void galois_run(const fhe_b200_batch* ct, KeySet gk, fhe_b200_batch* out,
     REQUIRE(ct->count == out->count, FHE_B200_INVALID_ARGUMENT, "batch sizes differ");
   need_repr(ct, FHE_B200_NTT);
   check_ksks(gk, ct->par, ct->level, out->count);
+  return galois_exponents(ct->par, gk.exps, gk.n);
+}
+
+// output j = GaloisKey::relinearize of ciphertext gk.source[j] (j without a source list) with key gk.key_of(j) for
+// its exponent gk.exps[key] (reduced), after galois_check
+static void galois_chunks(const fhe_b200_batch* ct, const KeySet& gk, fhe_b200_batch* out, cudaStream_t stream) {
   const fhe_b200_params* par = ct->par;
-  const std::vector<u32> exps = galois_exponents(par, gk.exps, gk.n);
-  gk.exps = exps.data();
-  DeviceGuard g(par);
   const LevelData& lv = par->level(ct->level);
   const size_t W = ct->words_per_ct();
-  ChunkRunner chunks(par, out->count, (cudaStream_t)stream);
+  ChunkRunner chunks(par, out->count, stream);
   chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
     galois_range(par, lv, gk.from(c0), ct->d, c0, out->d + c0 * W, n, false, st);
   });
+}
+
+static void galois_run(const fhe_b200_batch* ct, KeySet gk, fhe_b200_batch* out, void* stream) {
+  const std::vector<u32> exps = galois_check(ct, gk, out);
+  gk.exps = exps.data();
+  DeviceGuard g(ct->par);
+  galois_chunks(ct, gk, out, (cudaStream_t)stream);
   FHE_CUDA(cudaGetLastError());
   out->repr = FHE_B200_NTT;
 }
@@ -2815,6 +2842,177 @@ int fhe_b200_galois_many(const fhe_b200_batch* ct, const uint32_t* source, const
   K.exps = exponents;
   K.source = source;
   galois_run(ct, K, out, stream);
+  API_END
+}
+
+// Item i of `in` ([n][words]) to item dst[i] of `out`: one copy per run of consecutive destinations.
+static void scatter_items(const u64* in, u64* out, size_t words, const u32* dst, u32 n, cudaStream_t st) {
+  for (u32 i = 0, e; i < n; i = e) {
+    for (e = i + 1; e < n && dst[e] == dst[e - 1] + 1; e++) {}
+    FHE_CUDA(cudaMemcpyAsync(out + dst[i] * words, in + i * words, (e - i) * words * sizeof(u64),
+                             cudaMemcpyDeviceToDevice, st));
+  }
+}
+
+// The hoisted outputs [c0, c0 + n) of `outs` (output indices, ordered by source) as kernel entries: each distinct
+// source gets a digit slot and each distinct exponent a correction row, in order of first use.
+struct HoistPlan {
+  std::vector<HoistOut> h;
+  std::vector<u32> sources, exps;
+  HoistPlan(const KeySet& gk, const std::vector<u32>& outs, u32 c0, u32 n) {
+    for (u32 i = 0; i < n; i++) {
+      const u32 j = outs[c0 + i], s = gk.source ? gk.source[j] : j;
+      const fhe_b200_ksk* k = gk.keys[gk.key_of(j)];
+      const u32 e = gk.exps[gk.key_of(j)];
+      u32 slot = (u32)sources.size(), m = 0;
+      if (slot && sources.back() == s) slot--;
+      else sources.push_back(s);
+      while (m < exps.size() && exps[m] != e) m++;
+      if (m == exps.size()) exps.push_back(e);
+      h.push_back({k->k0, k->k1, e, slot, s, m, j});
+    }
+  }
+};
+
+// The power-basis c1 of the plan's sources: x [slot][L][N], canonical (the reference's c2 before its substitution)
+static u64* hoist_c1(const fhe_b200_params* par, const LevelData& lv, const fhe_b200_batch* ct,
+                     const std::vector<u32>& sources, Workspace& ws, cudaStream_t st) {
+  const size_t rowb = ((size_t)lv.L << par->logn) * sizeof(u64), W = ct->words_per_ct();
+  const u32 n = (u32)sources.size();
+  u64* x = ws.words(((size_t)n * lv.L) << par->logn);
+  for (u32 i = 0, e; i < n; i = e) {   // one 2-D copy per run of consecutive sources
+    for (e = i + 1; e < n && sources[e] == sources[e - 1] + 1; e++) {}
+    FHE_CUDA(cudaMemcpy2DAsync((char*)x + i * rowb, rowb, ct->d + sources[i] * W + ((size_t)lv.L << par->logn),
+                               W * sizeof(u64), rowb, e - i, cudaMemcpyDeviceToDevice, st));
+  }
+  launch_ntt(x, x, n * lv.L, lv.ctx_ids, par->d_limbs, par->logn, true, 1, false, st);
+  return x;
+}
+
+// fhe_b200_galois_many_hoisted after galois_check; returns how many outputs the hoisted kernels computed
+static u32 galois_hoisted(const fhe_b200_batch* ct, const KeySet& gk, fhe_b200_batch* out, cudaStream_t user) {
+  const fhe_b200_params* par = ct->par;
+  const fhe_b200_ksk* k = gk.keys[0];
+  const LevelData& lv = par->level(ct->level);
+  const LevelData& kl = par->level(k->ksk_level);
+  const u32 L = lv.L, Lk = k->Lk, logn = par->logn, count = out->count;
+  const size_t row = (size_t)1 << logn, W = ct->words_per_ct();
+  auto src_of = [&](u32 j) { return gk.source ? gk.source[j] : j; };
+  // candidates: the outputs of sources with two or more outputs, by (source, key) so that outputs sharing either
+  // are neighbours in the kernels' order.  Base-2^b digits of q - x are not a function of those of x: no candidates.
+  std::vector<u32> uses(ct->count), cand;
+  for (u32 j = 0; j < count; j++) uses[src_of(j)]++;
+  for (u32 j = 0; j < count && !k->log_base; j++)
+    if (uses[src_of(j)] >= 2) cand.push_back(j);
+  if (cand.empty()) {
+    galois_chunks(ct, gk, out, user);
+    return 0;
+  }
+  std::stable_sort(cand.begin(), cand.end(), [&](u32 a, u32 b) {
+    return src_of(a) != src_of(b) ? src_of(a) < src_of(b) : gk.key_of(a) < gk.key_of(b);
+  });
+  const u32 nc = (u32)cand.size();
+  // the zero check: an output whose exponent negates a position where c1 has a zero residue takes galois_range
+  std::vector<u32> zero(nc);
+  {
+    Workspace ws(par, user);
+    u32* flags = (u32*)ws.words((nc + 1) / 2);
+    FHE_CUDA(cudaMemsetAsync(flags, 0, nc * sizeof(u32), user));
+    {
+      ChunkRunner chunks(par, nc, user);
+      chunks.run([&](u32 c0, u32 n, cudaStream_t st) {
+        Workspace cws(par, st);
+        const HoistPlan P(gk, cand, c0, n);
+        const u64* x = hoist_c1(par, lv, ct, P.sources, cws, st);
+        launch_hoist_zero(P.h.data(), n, x, flags + c0, L, logn, st);
+      });
+    }
+    FHE_CUDA(cudaMemcpyAsync(zero.data(), flags, nc * sizeof(u32), cudaMemcpyDeviceToHost, user));
+    FHE_CUDA(cudaStreamSynchronize(user));   // the one synchronisation of the call
+  }
+  std::vector<u32> hoisted, rest, rest_key, rest_src;
+  std::vector<bool> is_hoisted(count);
+  for (u32 i = 0; i < nc; i++)
+    if (!zero[i]) {
+      hoisted.push_back(cand[i]);
+      is_hoisted[cand[i]] = true;
+    }
+  for (u32 j = 0; j < count; j++)
+    if (!is_hoisted[j]) {
+      rest.push_back(j);
+      rest_key.push_back(gk.key_of(j));
+      rest_src.push_back(src_of(j));
+    }
+  const u32 nh = (u32)hoisted.size(), nr = (u32)rest.size();
+  const bool reduce = digit_reduce(par, k);
+  ChunkRunner(par, nh, user).run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace ws(par, st);
+    const HoistPlan P(gk, hoisted, c0, n);
+    const u32 ns = (u32)P.sources.size(), ne = (u32)P.exps.size();
+    const u64* x = hoist_c1(par, lv, ct, P.sources, ws, st);
+    // D_k[j] = NTT_j(lazy(x_k)): key_switch_core's unfused digit transform, in the layout it would choose
+    u64* D = ws.words(((size_t)ns * L * Lk) << logn);
+    const bool adjacent = Lk > 1 && ntt_uses_tma(ns * L * Lk, kl.ctx_ids, logn, Lk, x, D);
+    launch_ntt(x, D, ns * L * Lk, kl.ctx_ids, par->d_limbs, logn, false, Lk, reduce, st, true, adjacent, L);
+    // M_e[j] = NTT_j(N_e) of every exponent of the chunk
+    u64* Mrows = ws.words(((size_t)ne * Lk) << logn);
+    launch_negation_rows(Mrows, P.exps.data(), ne, Lk, logn, st);
+    launch_ntt(Mrows, Mrows, ne * Lk, kl.ctx_ids, par->d_limbs, logn, false, 1, false, st);
+    if (Lk == L) {   // galois_key.rs:78: sigma(c0) is added in the kernel, which writes every output in place
+      launch_hoist_mac(P.h.data(), n, D, adjacent, Mrows, ct->d, W, out->d, W, L, Lk, kl.ctx_ids, par->d_limbs,
+                       logn, st);
+      return;
+    }
+    // leveled key (galois_key.rs:69-76): the Lk-limb pairs take key_switch_apply's tail with sigma(c0) as its base
+    std::vector<HoistOut> h = P.h;
+    std::vector<u32> exps(n), srcs(n), dst(n);
+    for (u32 i = 0; i < n; i++) {
+      exps[i] = h[i].exponent;
+      srcs[i] = h[i].src_ct;
+      dst[i] = h[i].dst;
+      h[i].dst = i;
+    }
+    u64* cur = ws.words(((size_t)n * 2 * Lk) << logn);
+    launch_hoist_mac(h.data(), n, D, adjacent, Mrows, nullptr, 0, cur, 2 * Lk * row, L, Lk, kl.ctx_ids, par->d_limbs,
+                     logn, st);
+    u64* s = ws.words(n * W);
+    u64* res = ws.words(n * W);
+    launch_substitute_ntt(ct->d, W, s, W, nullptr, 0, exps.data(), srcs.data(), n, L, false, lv.ctx_ids,
+                          par->d_limbs, logn, st);
+    key_switch_leveled_tail(par, k, cur, n, res, 2, s, ws, st);
+    scatter_items(res, out->d, W, dst.data(), n, st);
+  });
+  // every other output: galois_many's path, into place when the chunk's outputs are consecutive
+  const KeySet R{gk.keys, gk.n, rest_key.data(), gk.exps, rest_src.data()};
+  ChunkRunner(par, nr, user).run([&](u32 c0, u32 n, cudaStream_t st) {
+    if (rest[c0 + n - 1] - rest[c0] == n - 1) {
+      galois_range(par, lv, R.from(c0), ct->d, 0, out->d + rest[c0] * W, n, false, st);
+      return;
+    }
+    Workspace ws(par, st);
+    u64* tmp = ws.words(n * W);
+    galois_range(par, lv, R.from(c0), ct->d, 0, tmp, n, false, st);
+    scatter_items(tmp, out->d, W, rest.data() + c0, n, st);
+  });
+  return nh;
+}
+
+int fhe_b200_galois_many_hoisted(const fhe_b200_batch* ct, const uint32_t* source, const fhe_b200_ksk* const* gks,
+                                 const uint32_t* exponents, uint32_t n_keys, const uint32_t* key_index,
+                                 fhe_b200_batch* out, uint32_t* n_hoisted, void* stream) {
+  API_BEGIN
+  KeySet K = key_list(gks, n_keys, key_index);
+  REQUIRE(exponents, FHE_B200_INVALID_ARGUMENT, "null exponent list");
+  REQUIRE(ct && out && ct != out && out->d != ct->d, FHE_B200_INVALID_ARGUMENT, "null or aliased argument");
+  K.exps = exponents;
+  K.source = source;
+  const std::vector<u32> exps = galois_check(ct, K, out);
+  K.exps = exps.data();
+  DeviceGuard g(ct->par);
+  const u32 h = galois_hoisted(ct, K, out, (cudaStream_t)stream);
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
+  if (n_hoisted) *n_hoisted = h;
   API_END
 }
 

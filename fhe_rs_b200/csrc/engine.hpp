@@ -204,6 +204,30 @@ void launch_substitute_ntt(const u64* in, size_t in_stride, u64* out0, size_t ou
 void launch_substitute_power(const u64* in, u64* out, size_t n_rows, u32 exponent, const RowIds& ids,
                              const LimbDev* limbs, u32 logn, cudaStream_t st);
 
+// ---- hoisted rotations (DESIGN §8): many Galois key switches of one ciphertext from one digit decomposition of c1.
+// One hoisted output: its key pair ([Lk][n_dig][N] each), exponent (odd, < 2N), the slot of its source's digits and
+// power-basis c1 in the call's buffers, its source ciphertext in the batch, its correction row and where it is written.
+struct HoistOut {
+  const u64 *k0, *k1;
+  u32 exponent, src, src_ct, mrow, dst;
+};
+// flags[i] = 1 when output i's substitution negates a position s >= 1 at which some residue row of its source's c1 is
+// zero: x [slot][L][N] power basis, canonical; output i negates s when (s * exponent mod 2N) >= N.  Writes only 1s (the
+// caller clears the flags).
+void launch_hoist_zero(const HoistOut* outs, u32 n, const u64* x, u32* flags, u32 L, u32 logn, cudaStream_t st);
+// out [m][Lk][N] power basis: row (m, j) is N_e of exponent exps[m] in every limb j, 1 at each destination x^d whose
+// source x^s has (s * e mod 2N) >= N (the negated coefficients of rq/mod.rs:390-408), 0 elsewhere
+void launch_negation_rows(u64* out, const u32* exps, u32 n_exp, u32 Lk, u32 logn, cudaStream_t st);
+// The key switch of sigma_e(c1) from the digit transforms of c1 (key_switching_key.rs:256-268 with the identity of
+// DESIGN §8): for output i with source slot s, exponent e and correction row m, limb j < Lk,
+//   out_p[j] = sum_{k < L} key_p,k[j] (.) pi_e(D_k[j]) + M_m[j] (.) sum_{k < L} [q_k]_{q_j} key_p,k[j]   (+ sigma_e(c0)[j])
+// D: digits [slot][L][Lk][N] (lazy NTT words), or [slot][Lk][L][N] when `adjacent`; mrows: [m][Lk][N] NTT of N_e,
+// canonical.  Output i's rows (p, j) go to out + dst * out_stride + (p * Lk + j) * N.  c0 (nullable, Lk == L): the
+// batch, whose part 0 of ciphertext src_ct (at c0 + src_ct * c0_stride) is added through pi_e.  ids: the key level's.
+void launch_hoist_mac(const HoistOut* outs, u32 n, const u64* D, bool adjacent, const u64* mrows, const u64* c0,
+                      size_t c0_stride, u64* out, size_t out_stride, u32 L, u32 Lk, const RowIds& ids,
+                      const LimbDev* limbs, u32 logn, cudaStream_t st);
+
 // Poly<PowerBasis>::switch_down (rq/mod.rs:433-492): in [polys][L][N] -> out [polys][L-1][N]
 struct SwitchDownDev {
   u64 q_last, q_last_half;

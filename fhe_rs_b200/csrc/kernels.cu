@@ -991,6 +991,95 @@ __global__ void substitute_power_kernel(SubstPowerArgs A) {
   A.out[(row << A.logn) + (power & (N - 1))] = (power & N) ? csub(p - v, p) : v;   // Modulus::sub(0, v) / add(0, v)
 }
 
+// ------------------------------------------------------------------ hoisted rotations (DESIGN §8)
+// The outputs of one launch, carried in its kernel parameters (HoistOut without the key pointers, which go to the
+// KeyTable).  96 outputs keep the MAC kernel's parameters under 4 KiB.
+constexpr u32 kHoistOuts = 96;
+struct HoistTable {
+  u32 n;
+  u32 exponent[kHoistOuts], src_ct[kHoistOuts], dst[kHoistOuts];
+  unsigned short src[kHoistOuts], mrow[kHoistOuts];
+};
+
+// the source word of NTT position o under exponent e: pi_e of subst_kernel
+__device__ __forceinline__ u32 subst_source(u32 o, u32 e, u32 logn) {
+  const u32 j = __brev(o) >> (32 - logn);
+  return __brev((j * e + ((e - 1) >> 1)) & ((1u << logn) - 1)) >> (32 - logn);
+}
+
+// One CTA row (blockIdx.y) per output, one thread per coefficient s of its source's c1; only the positions the
+// exponent negates read the L residues.
+__global__ void hoist_zero_kernel(const __grid_constant__ HoistTable T, const u64* x, u32* flags, u32 L, u32 logn) {
+  const u32 N = 1u << logn, s = blockIdx.x * blockDim.x + threadIdx.x, i = blockIdx.y;
+  if (s == 0 || s >= N || !((s * T.exponent[i]) & N)) return;   // mod 2^32 keeps bit logn of s*e exact
+  const u64* r = x + (((size_t)T.src[i] * L) << logn) + s;
+  bool zero = false;
+  for (u32 k = 0; k < L; k++) zero |= r[(size_t)k << logn] == 0;
+  if (zero) flags[i] = 1;
+}
+
+// Row (m, j) of N_e: thread s writes destination (s * e) mod N, so every word is written once.
+__global__ void negation_rows_kernel(const __grid_constant__ HoistTable T, u64* out, u32 Lk, u32 logn) {
+  const u32 N = 1u << logn, s = blockIdx.x * blockDim.x + threadIdx.x, m = blockIdx.y;
+  if (s >= N) return;
+  const u32 power = s * T.exponent[m];
+  u64* row = out + (((size_t)m * Lk) << logn) + (power & (N - 1));
+  for (u32 j = 0; j < Lk; j++) row[(size_t)j << logn] = (power & N) ? 1 : 0;
+}
+
+struct HoistMacArgs {
+  HoistTable T;
+  KeyTable keys;
+  const u64 *D, *mrows, *c0;
+  u64* out;
+  size_t c0_stride, out_stride;
+  u32 L, Lk, logn, adjacent;
+  const LimbDev* limbs;
+  unsigned short ids[kMaxPos];
+};
+// One thread per (coefficient o, output i = blockIdx.y, limb j = blockIdx.z), limb outermost: at any time the resident
+// CTAs work on one limb of consecutive outputs, which the caller orders by (source, key), so the L digit rows of a
+// source's limb j (3.7 MB at set C) and the key rows of a repeated key are read from L2 by every output that uses
+// them.  pi_e permutes the words of each aligned group of 32 among themselves, so a warp's digit reads stay one 256-byte
+// segment.  The correction sum_k [q_k]_{q_j} key_p,k[j] is accumulated beside the inner product from the key words
+// already in registers, reduced, and multiplied by the correction row once.
+__global__ void hoist_mac_kernel(const __grid_constant__ HoistMacArgs A) {
+  __shared__ u64 qk[kMaxPos];
+  const u32 N = 1u << A.logn, i = blockIdx.y, j = blockIdx.z;
+  const LimbDev& M = A.limbs[A.ids[j]];
+  if (threadIdx.x < A.L) qk[threadIdx.x] = A.limbs[A.ids[threadIdx.x]].p % M.p;   // [q_k]_{q_j}
+  __syncthreads();
+  const u32 o = blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= N) return;
+  const u32 s = subst_source(o, A.T.exponent[i], A.logn);
+  const u64* d = A.adjacent ? A.D + ((((size_t)A.T.src[i] * A.Lk + j) * A.L) << A.logn) + s
+                            : A.D + ((((size_t)A.T.src[i] * A.L) * A.Lk + j) << A.logn) + s;
+  const size_t dstride = A.adjacent ? (size_t)1 << A.logn : (size_t)A.Lk << A.logn;
+  const u32 slot = key_slot(A.keys, i);
+  const u64* k0 = A.keys.k0[slot] + (((size_t)j * A.L) << A.logn) + o;
+  const u64* k1 = A.keys.k1[slot] + (((size_t)j * A.L) << A.logn) + o;
+  Acc192 a0, a1, h0, h1;
+  a0.clear();
+  a1.clear();
+  h0.clear();
+  h1.clear();
+#pragma unroll 2
+  for (u32 k = 0; k < A.L; k++) {
+    const u64 t = d[k * dstride], x = __ldg(k0 + ((size_t)k << A.logn)), y = __ldg(k1 + ((size_t)k << A.logn));
+    a0.mac(t, x);
+    a1.mac(t, y);
+    h0.mac(qk[k], x);
+    h1.mac(qk[k], y);
+  }
+  const u64 m = A.mrows[(((size_t)A.T.mrow[i] * A.Lk + j) << A.logn) + o];
+  a0.mac(h0.reduce(M), m);
+  a1.mac(h1.reduce(M), m);
+  if (A.c0) a0.add64(A.c0[A.T.src_ct[i] * A.c0_stride + ((size_t)j << A.logn) + s]);
+  u64* out = A.out + A.T.dst[i] * A.out_stride + ((size_t)j << A.logn) + o;
+  out[0] = a0.reduce(M);
+  out[(size_t)A.Lk << A.logn] = a1.reduce(M);
+}
+
 struct SwitchDownArgs {
   SwitchDownDev S;
   const u64* in;
@@ -2111,6 +2200,77 @@ void launch_substitute_power(const u64* in, u64* out, size_t n_rows, u32 exponen
   if (!A.n_words) return;
   substitute_power_kernel<<<(unsigned)((A.n_words + 255) / 256), 256, 0, st>>>(A);
   g_launches++;
+}
+
+// the outputs [i0, i0 + T.n) of `outs` as a launch table
+static void hoist_table(HoistTable& T, const HoistOut* outs, u32 i0, u32 n) {
+  std::memset(&T, 0, sizeof(T));
+  T.n = n;
+  for (u32 i = 0; i < n; i++) {
+    const HoistOut& h = outs[i0 + i];
+    T.exponent[i] = h.exponent;
+    T.src_ct[i] = h.src_ct;
+    T.dst[i] = h.dst;
+    T.src[i] = (unsigned short)h.src;
+    T.mrow[i] = (unsigned short)h.mrow;
+  }
+}
+
+void launch_hoist_zero(const HoistOut* outs, u32 n, const u64* x, u32* flags, u32 L, u32 logn, cudaStream_t st) {
+  const u32 N = 1u << logn;
+  HoistTable T;
+  for (u32 i0 = 0; i0 < n; i0 += kHoistOuts) {
+    hoist_table(T, outs, i0, std::min(kHoistOuts, n - i0));
+    hoist_zero_kernel<<<dim3((N + 255) / 256, T.n), 256, 0, st>>>(T, x, flags + i0, L, logn);
+    g_launches++;
+  }
+}
+
+void launch_negation_rows(u64* out, const u32* exps, u32 n_exp, u32 Lk, u32 logn, cudaStream_t st) {
+  const u32 N = 1u << logn;
+  HoistTable T;
+  for (u32 m0 = 0; m0 < n_exp; m0 += kHoistOuts) {
+    std::memset(&T, 0, sizeof(T));
+    T.n = std::min(kHoistOuts, n_exp - m0);
+    for (u32 m = 0; m < T.n; m++) T.exponent[m] = exps[m0 + m];
+    negation_rows_kernel<<<dim3((N + 255) / 256, T.n), 256, 0, st>>>(T, out + (((size_t)m0 * Lk) << logn), Lk, logn);
+    g_launches++;
+  }
+}
+
+void launch_hoist_mac(const HoistOut* outs, u32 n, const u64* D, bool adjacent, const u64* mrows, const u64* c0,
+                      size_t c0_stride, u64* out, size_t out_stride, u32 L, u32 Lk, const RowIds& ids,
+                      const LimbDev* limbs, u32 logn, cudaStream_t st) {
+  const u32 N = 1u << logn;
+  HoistMacArgs A;
+  std::memset(&A, 0, sizeof(A));
+  A.D = D; A.mrows = mrows; A.c0 = c0; A.out = out; A.c0_stride = c0_stride; A.out_stride = out_stride;
+  A.L = L; A.Lk = Lk; A.logn = logn; A.adjacent = adjacent ? 1 : 0; A.limbs = limbs;
+  copy_ids(A.ids, ids);
+  // one launch per run of at most kHoistOuts outputs and kKeyPairs distinct keys
+  u32 i0 = 0;
+  auto flush = [&](u32 end) {
+    hoist_table(A.T, outs, i0, end - i0);
+    hoist_mac_kernel<<<dim3((N + 255) / 256, A.T.n, Lk), 256, 0, st>>>(A);
+    g_launches++;
+    std::memset(&A.keys, 0, sizeof(A.keys));
+    i0 = end;
+  };
+  for (u32 i = 0; i < n; i++) {
+    u32 s = 0;
+    while (s < A.keys.n && A.keys.k0[s] != outs[i].k0) s++;
+    if (i - i0 == kHoistOuts || (s == A.keys.n && s == kKeyPairs)) {
+      flush(i);
+      s = 0;
+    }
+    if (s == A.keys.n) {
+      A.keys.k0[s] = outs[i].k0;
+      A.keys.k1[s] = outs[i].k1;
+      A.keys.n++;
+    }
+    A.keys.slot[i - i0] = (unsigned char)s;
+  }
+  if (n > i0) flush(n);
 }
 
 void launch_pack(const PackDev& P, const u64* words, unsigned char* bytes, size_t n_rows, u32 logn, cudaStream_t st) {

@@ -525,6 +525,25 @@ int fhe_b200_expand_keyed(const fhe_b200_batch* ct, uint32_t size, const fhe_b20
 int fhe_b200_galois_many(const fhe_b200_batch* ct, const uint32_t* source, const fhe_b200_ksk* const* gks,
                          const uint32_t* exponents, uint32_t n_keys, const uint32_t* key_index, fhe_b200_batch* out,
                          void* stream);
+/* fhe_b200_galois_many with hoisting: the same arguments, checks and error codes, and entry j of out is word for word
+ * entry j of fhe_b200_galois_many.  The outputs of a source ciphertext that has two or more outputs share one digit
+ * decomposition of its c1: its L x Lk digit transforms (rq/mod.rs:563-586) run once, and each output's key switch
+ * (key_switching_key.rs:241-270, galois_key.rs:63-86) reads them through the NTT-domain permutation of its exponent
+ * (rq/mod.rs:360-389).  The reference's digits of sigma(c1) differ from sigma applied to the digits of c1 by q_k at the
+ * coefficients the substitution negates (rq/mod.rs:390-408); the kernel adds that difference back, which is exact
+ * except where such a coefficient's residue is zero.  The outputs whose exponent negates a position s >= 1 at which
+ * some residue of their source's c1 is zero, the outputs of sources with one output, and every output of a call whose
+ * keys have a base-2^b decomposition (log_base != 0) take fhe_b200_galois_many's path.
+ * n_hoisted (host memory, nullable) receives how many outputs were computed from shared digits.
+ * Synchronisation: when any output is a candidate for hoisting, the call synchronises `stream` once, after the zero
+ * check and before the first output is computed, to read the check on the host.  A call that hoists nothing (every
+ * source used once, or base-2^b keys) does not synchronise.
+ * Scratch: stream-ordered, per hoisted source of a chunk L x Lk x N words of digits plus L x N of its power-basis c1
+ * (51 MB at N = 2^15 with 14 moduli), and per distinct exponent of a chunk Lk x N words; a chunk holds at most
+ * FHE_B200_CHUNK outputs.  Nothing outlives the call. */
+int fhe_b200_galois_many_hoisted(const fhe_b200_batch* ct, const uint32_t* source, const fhe_b200_ksk* const* gks,
+                                 const uint32_t* exponents, uint32_t n_keys, const uint32_t* key_index,
+                                 fhe_b200_batch* out, uint32_t* n_hoisted, void* stream);
 /* EvaluationKey::computes_inner_sum (keys/evaluation_key.rs:56-100) of every ciphertext of ct into out (same shape,
  * must not alias ct; ct is left unchanged; out becomes NTT).  gks holds n_gks = log2 N keys: the Galois keys of the
  * column rotations by 1, 2, 4, ..., N/4 (exponents 3^i mod 2N), then of the row rotation (2N - 1); any other n_gks or a

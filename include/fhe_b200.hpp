@@ -727,6 +727,16 @@ class EvaluationKey {
   // rotates_columns_by(ct_q, steps[i]) for every step and every ciphertext of ct (Q = ct.count()) in one device call
   // (fhe_b200_galois_many): entry i*Q + q of the result is ciphertext q rotated by steps[i]
   Ciphertext rotates_columns_by_many(const Ciphertext& ct, const std::vector<uint32_t>& steps) const {
+    return rotates_many(ct, steps, false);
+  }
+  // rotates_columns_by_many, word for word, with each ciphertext's rotations computed from one digit decomposition of
+  // it when it has two or more (fhe_b200_galois_many_hoisted; synchronises ct's stream once when it hoists)
+  Ciphertext rotates_columns_by_many_hoisted(const Ciphertext& ct, const std::vector<uint32_t>& steps) const {
+    return rotates_many(ct, steps, true);
+  }
+
+ private:
+  Ciphertext rotates_many(const Ciphertext& ct, const std::vector<uint32_t>& steps, bool hoisted) const {
     std::vector<const fhe_b200_ksk*> keys;
     std::vector<uint32_t> exps, index, source;
     const uint32_t q = ct.count();
@@ -747,10 +757,16 @@ class EvaluationKey {
     if (keys.empty()) keys.push_back(nullptr);   // no steps: refused by the call
     Ciphertext out(ct.par(), std::max<uint32_t>((uint32_t)index.size(), 1), 2, ct.level(), Representation::Ntt,
                    ct.stream());
-    check(fhe_b200_galois_many(ct.handle(), source.data(), keys.data(), exps.data(), (uint32_t)exps.size(),
-                               index.data(), out.handle(), ct.stream()));
+    if (hoisted)
+      check(fhe_b200_galois_many_hoisted(ct.handle(), source.data(), keys.data(), exps.data(), (uint32_t)exps.size(),
+                                         index.data(), out.handle(), nullptr, ct.stream()));
+    else
+      check(fhe_b200_galois_many(ct.handle(), source.data(), keys.data(), exps.data(), (uint32_t)exps.size(),
+                                 index.data(), out.handle(), ct.stream()));
     return out;
   }
+
+ public:
   // evaluation_key.rs:175-189
   bool supports_expansion(uint32_t level) const {
     const uint32_t n = (uint32_t)par_->degree();
@@ -1057,6 +1073,22 @@ inline Ciphertext galois_many(const Ciphertext& ct, const std::vector<const Galo
   Ciphertext out(ct.par(), std::max<uint32_t>(count, 1), 2, ct.level(), Representation::Ntt, ct.stream());
   check(fhe_b200_galois_many(ct.handle(), source.empty() ? nullptr : source.data(), h.data(), exps.data(),
                              (uint32_t)gks.size(), index.data(), out.handle(), ct.stream()));
+  return out;
+}
+// galois_many, word for word, with the rotations of each source that has two or more outputs computed from one digit
+// decomposition of its c1 (fhe_b200_galois_many_hoisted); *n_hoisted (when given) receives how many were
+inline Ciphertext galois_many_hoisted(const Ciphertext& ct, const std::vector<const GaloisKey*>& gks,
+                                      const std::vector<uint32_t>& index, const std::vector<uint32_t>& source = {},
+                                      uint32_t* n_hoisted = nullptr) {
+  const uint32_t count = source.empty() ? ct.count() : (uint32_t)source.size();
+  keyed_detail::check_index(index, count);
+  const auto h = keyed_detail::handles(gks, [](const GaloisKey& k) { return k.ksk->handle(); });
+  std::vector<uint32_t> exps;
+  for (const GaloisKey* g : gks) exps.push_back(g ? g->exponent : 1);
+  if (exps.empty()) exps.push_back(1);
+  Ciphertext out(ct.par(), std::max<uint32_t>(count, 1), 2, ct.level(), Representation::Ntt, ct.stream());
+  check(fhe_b200_galois_many_hoisted(ct.handle(), source.empty() ? nullptr : source.data(), h.data(), exps.data(),
+                                     (uint32_t)gks.size(), index.data(), out.handle(), n_hoisted, ct.stream()));
   return out;
 }
 // EvaluationKey::computes_inner_sum of ciphertext j with eks[index[j]] (fhe_b200_inner_sum_keyed)
