@@ -108,6 +108,7 @@ SYMBOLS = {
     "fhe_b200_expand_keyed": (_i, [_vp, _u32, _pp, _u32, _u32, _pu32, _vp, _vp]),
     "fhe_b200_galois_many": (_i, [_vp, _pu32, _pp, _pu32, _u32, _pu32, _vp, _vp]),
     "fhe_b200_galois_many_hoisted": (_i, [_vp, _pu32, _pp, _pu32, _u32, _pu32, _vp, _pu32, _vp]),
+    "fhe_b200_linear_transform": (_i, [_vp, _vp, _u32, _u32, _pp, _pu32, _u32, _vp, _pu32, _vp]),
     "fhe_b200_inner_sum": (_i, [_vp, _pp, _u32, _vp, _vp]),
     "fhe_b200_inner_sum_keyed": (_i, [_vp, _pp, _u32, _u32, _pu32, _vp, _vp]),
     "fhe_b200_batch_sum": (_i, [_vp, _u32, _i, _vp, _vp]),

@@ -27,6 +27,7 @@ __all__ = ["BfvParameters", "BfvParametersBuilder", "Ciphertext", "KeySwitchingK
            "transcode_bidirectional", "transcode_to_bytes", "transcode_from_bytes", "key_switch_keyed",
            "relinearizes_keyed", "multiply_keyed", "galois_keyed", "rotates_columns_by_keyed", "rotates_rows_keyed",
            "expands_keyed", "expands_batch_keyed", "external_products_keyed", "galois_many", "galois_many_hoisted",
+           "linear_transform", "linear_transform_steps", "encode_diagonals",
            "computes_inner_sum_keyed", "dot_product", "dot_product_keyed"]
 
 
@@ -1203,6 +1204,21 @@ class EvaluationKey:
         decomposition of it when it has two or more (fhe_b200_galois_many_hoisted)"""
         return galois_many_hoisted(ct, *self._many_args(ct, steps))[0]
 
+    def linear_transform(self, ct: Ciphertext, diags: "PlaintextVec", baby: int,
+                         n_diags: Optional[int] = None) -> Ciphertext:
+        """sum_k diag_k (.) rotates_columns_by(ct, k) of every ciphertext by baby-step/giant-step diagonals in one
+        device call (fhe_b200_linear_transform); `diags` from encode_diagonals"""
+        n = _n_diags(ct, diags, n_diags)
+        two_n = 2 * self.par.degree()
+        gks = []
+        for i in linear_transform_steps(n, baby):
+            e = pow(3, i, two_n)
+            if e not in self.gk:
+                raise FheError(_capi.INVALID_ARGUMENT,
+                               "EvaluationKeyError: column rotation by %d not supported by this key" % i)
+            gks.append(self.gk[e])
+        return linear_transform(ct, diags, baby, gks, n)[0]
+
     def _many_args(self, ct: Ciphertext, steps: Sequence[int]):
         two_n = 2 * self.par.degree()
         exps = [pow(3, int(i), two_n) for i in steps]
@@ -1580,6 +1596,87 @@ def _galois_many(ct, gks, index, source, hoisted):
     check(_capi.lib().fhe_b200_galois_many_hoisted(ct._h, sp, keys, exps, n, ix, out._h, C.byref(n_hoisted),
                                                    ct.stream))
     return out, n_hoisted.value
+
+
+def linear_transform_steps(n_diags: int, baby: int) -> List[int]:
+    """the column rotation steps a linear transform of n_diags diagonals with baby step `baby` needs keys for (to
+    enable in EvaluationKeyBuilder): the baby steps 1 .. baby - 1, then the giant steps baby, 2 baby, .."""
+    if not 1 <= baby <= n_diags:
+        raise FheError(_capi.INVALID_ARGUMENT, "the baby step must be 1 .. n_diags, got %d" % baby)
+    return list(range(1, baby)) + list(range(baby, n_diags, baby))
+
+
+def _n_diags(ct: Ciphertext, diags: "PlaintextVec", n_diags: Optional[int]) -> int:
+    if n_diags is not None:
+        return int(n_diags)
+    if getattr(diags, "n_diags", None) is not None:
+        return diags.n_diags
+    return len(diags)
+
+
+def linear_transform(ct: Ciphertext, diags: "PlaintextVec", baby: int, gks: Sequence["GaloisKey"],
+                     n_diags: Optional[int] = None) -> Tuple[Ciphertext, int]:
+    """out[c] = sum_g rot_{g baby}(sum_i diags[g baby + i] (.) rot_i(ct[c])) (rot_0 the identity) for every ciphertext
+    of ct, word for word the composition of rotates_columns_by, mul_plain and + (fhe_b200_linear_transform).  `diags`:
+    a PlaintextVec (or 1-part NTT batch) of n_diags diagonals shared by every ciphertext, or n_diags per ciphertext;
+    n_diags defaults to the count encode_diagonals recorded, else len(diags).  gks: Galois keys holding at least the
+    steps of linear_transform_steps.  Returns the result and how many (ciphertext, baby step) rotations were computed
+    unhoisted.  Synchronises the stream once when it hoists."""
+    batch = diags.batch if isinstance(diags, PlaintextVec) else diags
+    n = _n_diags(ct, diags, n_diags)
+    keys = (C.c_void_p * max(1, len(gks)))(*[g.ksk._h.value for g in gks])
+    exps = (C.c_uint32 * max(1, len(gks)))(*[int(g.exponent) & 0xFFFFFFFF for g in gks])
+    out = Ciphertext(ct.par, max(ct.count, 1), 2, ct.level, NTT, ct.stream)
+    n_fallback = C.c_uint32(0)
+    check(_capi.lib().fhe_b200_linear_transform(ct._h, batch._h, n, baby, C.cast(keys, C.POINTER(C.c_void_p)), exps,
+                                                len(gks), out._h, C.byref(n_fallback), ct.stream))
+    return out, n_fallback.value
+
+
+def diagonals(matrices, half: int, n_diags: int, baby: int) -> np.ndarray:
+    """the slot values encode_diagonals encodes, [count][n_diags][2 * half] uint64 (see there)"""
+    m = np.asarray(matrices)
+    if m.dtype.kind not in "iu":
+        raise FheError(_capi.INVALID_ARGUMENT, "expected integer matrices")
+    if m.ndim == 2:
+        m = np.stack([m, m])
+    if m.ndim == 3:
+        m = m[None]
+    if m.ndim != 4 or m.shape[1:] != (2, half, half):
+        raise FheError(_capi.INVALID_ARGUMENT, "expected (N/2) x (N/2) matrices: one, a pair (one per slot row), or "
+                       "a stack of pairs [count][2][N/2][N/2]")
+    if not 1 <= n_diags <= half or not 1 <= baby <= n_diags:
+        raise FheError(_capi.INVALID_ARGUMENT, "n_diags must be 1 .. N/2 and the baby step 1 .. n_diags")
+    r = np.arange(half)
+    k = np.arange(half)
+    # d[c][q][k][r] = M_cq[r][(r + k) mod half]
+    d = m[:, :, r[None, :], (r[None, :] + k[:, None]) % half]
+    if np.any(d[:, :, n_diags:] != 0):
+        raise FheError(_capi.INVALID_ARGUMENT, "a diagonal beyond the first n_diags = %d is not zero" % n_diags)
+    d = d[:, :, :n_diags]
+    for j in range(baby, n_diags):   # rotated right by the giant step g * baby of diagonal j
+        d[:, :, j] = np.roll(d[:, :, j], (j // baby) * baby, axis=-1)
+    return np.ascontiguousarray(d.transpose(0, 2, 1, 3).reshape(m.shape[0], n_diags, 2 * half))
+
+
+def encode_diagonals(par: BfvParameters, matrices, baby: int, level: int = 0,
+                     n_diags: Optional[int] = None) -> "PlaintextVec":
+    """The diagonals of a slot-wise linear map for linear_transform, SIMD-encoded on the device.  `matrices`: one
+    (N/2) x (N/2) integer matrix for both slot rows, a pair [2][N/2][N/2] (one per row), or a stack of pairs
+    [count][2][N/2][N/2] (one map per ciphertext); entries are taken mod t.  Diagonal k is M[r][(r + k) mod N/2] in
+    slot r of each row, rotated right by its giant step g * baby (k = g * baby + i) on the host; the result holds
+    diagonals 0 .. n_diags - 1 (default N/2) of each map in that order.  A non-zero diagonal from n_diags on is
+    refused."""
+    half = par.degree() // 2
+    n = half if n_diags is None else int(n_diags)
+    t = par.plaintext()
+    m = np.asarray(matrices)
+    if m.dtype.kind in "iu":
+        m = np.mod(m.astype(np.int64) if m.dtype.kind == "i" else m, t).astype(np.uint64)
+    d = diagonals(m, half, n, baby)
+    pv = PlaintextVec.try_encode(d.reshape(-1), Encoding.simd_at_level(level), par)
+    pv.n_diags = n
+    return pv
 
 
 def computes_inner_sum_keyed(ct: Ciphertext, eks: Sequence["EvaluationKey"], index) -> Ciphertext:

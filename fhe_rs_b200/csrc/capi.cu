@@ -3016,6 +3016,230 @@ int fhe_b200_galois_many_hoisted(const fhe_b200_batch* ct, const uint32_t* sourc
   API_END
 }
 
+// ---- linear transforms (DESIGN §3.4): out[c] = sum_g rot_{g b}(sum_i D[g b + i] (.) B_i(ct[c])), B_0 the identity
+struct LinearTransform {
+  const fhe_b200_batch *ct, *diags;
+  u32 n, b, G;
+  bool per_ct;
+  const fhe_b200_ksk* const* keys;
+  u32 n_keys;
+  const u32* exps;            // reduced, one per key
+  std::vector<u32> baby_key;  // [b]: the key of baby step i >= 1 (entry 0 unused)
+  std::vector<u32> giant_key; // [G]: the key of giant step g >= 1 (entry 0 unused)
+  size_t W() const { return ct->words_per_ct(); }
+  // GaloisKey::relinearize of items src[r] of `in` with keys key[r] into dst [m][W], at most chunk_size() at a time
+  void rotate(const u64* in, const std::vector<u32>& src, const std::vector<u32>& key, u64* dst, cudaStream_t st) const {
+    const fhe_b200_params* par = ct->par;
+    const u32 m = (u32)src.size(), step = chunk_size();
+    for (u32 r0 = 0; r0 < m; r0 += step)
+      galois_range(par, par->level(ct->level), KeySet{keys, n_keys, key.data() + r0, exps, src.data() + r0}, in, 0,
+                   dst + r0 * W(), std::min(step, m - r0), false, st);
+  }
+  // the giant steps of groups [g0, g0 + ng) of ciphertexts [c0, c0 + cts): P [cts][ng] holds their partial sums;
+  // out[c] = (g0 == 0 ? P[c][0] : out[c]) + sum over the other groups of rot_{g b}(P[c][g - g0]), through R [cts][ng]
+  void finish(u64* P, u64* R, u32 c0, u32 cts, u32 g0, u32 ng, u64* out, cudaStream_t st) const {
+    const fhe_b200_params* par = ct->par;
+    const u32 L = par->level(ct->level).L;
+    std::vector<u32> src, key;
+    for (u32 c = 0; c < cts; c++)
+      for (u32 gi = g0 ? 0 : 1; gi < ng; gi++) {
+        src.push_back(c * ng + gi);
+        key.push_back(giant_key[g0 + gi]);
+      }
+    u64* o = out + (size_t)c0 * W();
+    if (g0 == 0)
+      launch_segment_sum(P, ng * W(), 1, o, W(), nullptr, 0, 2 * L, cts, W(), false, ids_of(ct), par->d_limbs,
+                         par->logn, st);
+    if (src.empty()) return;
+    rotate(P, src, key, R, st);
+    launch_segment_sum(R, W(), (u32)src.size() / cts, o, W(), nullptr, 0, 2 * L, cts, W(), true, ids_of(ct),
+                       par->d_limbs, par->logn, st);
+  }
+  // groups per tile for a chunk of `cts` ciphertexts: a tile's giant rotations are at most chunk_size() outputs
+  u32 group_tile(u32 cts) const { return std::min(G, std::max(1u, chunk_size() / cts)); }
+  const u64* diag(u32 c, u32 k) const {
+    return diags->d + ((per_ct ? (size_t)c * n : 0) + k) * diags->words_per_ct();
+  }
+};
+
+// Keys at the ciphertext level without base-2^b digits: one hoisted decomposition per ciphertext and hoist_dot_kernel;
+// returns the (ciphertext, baby step) terms that took galois_range because of the zero check
+static u32 linear_transform_fused(const LinearTransform& T, fhe_b200_batch* out, cudaStream_t user) {
+  const fhe_b200_batch* ct = T.ct;
+  const fhe_b200_params* par = ct->par;
+  const LevelData& lv = par->level(ct->level);
+  const u32 L = lv.L, logn = par->logn, b = T.b, count = ct->count;
+  const size_t W = T.W();
+  std::vector<LtStep> steps(b);
+  std::vector<u32> exps(b, 1);
+  for (u32 i = 1; i < b; i++) {
+    const fhe_b200_ksk* k = T.keys[T.baby_key[i]];
+    exps[i] = T.exps[T.baby_key[i]];
+    steps[i] = {k->k0, k->k1, exps[i], 0};
+  }
+  auto c1_of = [&](u32 c0, u32 n, Workspace& ws, cudaStream_t st) {
+    std::vector<u32> src(n);
+    for (u32 c = 0; c < n; c++) src[c] = c0 + c;
+    return hoist_c1(par, lv, ct, src, ws, st);
+  };
+  // the zero check (DESIGN §8): term (c, i) falls back when exponent i negates a position where c1 has a zero residue
+  std::vector<u32> zero((size_t)count * (b - 1));
+  Workspace ws(par, user);
+  if (b > 1) {
+    u32* flags = (u32*)ws.words((zero.size() + 1) / 2);
+    FHE_CUDA(cudaMemsetAsync(flags, 0, zero.size() * sizeof(u32), user));
+    ChunkRunner(par, count, user).run([&](u32 c0, u32 n, cudaStream_t st) {
+      Workspace cws(par, st);
+      std::vector<HoistOut> h;
+      for (u32 c = 0; c < n; c++)
+        for (u32 i = 1; i < b; i++) h.push_back({steps[i].k0, steps[i].k1, exps[i], c, c0 + c, i, 0});
+      launch_hoist_zero(h.data(), (u32)h.size(), c1_of(c0, n, cws, st), flags + (size_t)c0 * (b - 1), L, logn, st);
+    });
+    FHE_CUDA(cudaMemcpyAsync(zero.data(), flags, zero.size() * sizeof(u32), cudaMemcpyDeviceToHost, user));
+    FHE_CUDA(cudaStreamSynchronize(user));   // the one synchronisation of the call
+  }
+  // the baby steps' keys and exponents, and M_e of each (DESIGN §8), for every chunk
+  LtStep* d_steps = (LtStep*)ws.words((b * sizeof(LtStep) + 7) / 8);
+  FHE_CUDA(cudaMemcpyAsync(d_steps, steps.data(), b * sizeof(LtStep), cudaMemcpyHostToDevice, user));
+  u64* mrows = ws.words(((size_t)b * L) << logn);
+  launch_negation_rows(mrows, exps.data(), b, L, logn, user);
+  launch_ntt(mrows, mrows, b * L, lv.ctx_ids, par->d_limbs, logn, false, 1, false, user);
+  const bool reduce = b > 1 && digit_reduce(par, T.keys[0]);
+  u32 n_fallback = 0;
+  for (u32 z : zero) n_fallback += z;
+  ChunkRunner(par, count, user, std::max(1u, chunk_size() / T.G)).run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace cws(par, st);
+    u64 *D = nullptr, *fb = nullptr;
+    int* d_fallback = nullptr;
+    bool adjacent = false;
+    if (b > 1) {
+      const u64* x = c1_of(c0, n, cws, st);
+      D = cws.words(((size_t)n * L * L) << logn);
+      adjacent = L > 1 && ntt_uses_tma(n * L * L, lv.ctx_ids, logn, L, x, D);
+      launch_ntt(x, D, n * L * L, lv.ctx_ids, par->d_limbs, logn, false, L, reduce, st, true, adjacent, L);
+      std::vector<int> fallback((size_t)n * b, -1);
+      std::vector<u32> src, key;
+      for (u32 c = 0; c < n; c++)
+        for (u32 i = 1; i < b; i++)
+          if (zero[(size_t)(c0 + c) * (b - 1) + i - 1]) {
+            fallback[(size_t)c * b + i] = (int)src.size();
+            src.push_back(c0 + c);
+            key.push_back(T.baby_key[i]);
+          }
+      if (!src.empty()) {
+        fb = cws.words(src.size() * W);
+        T.rotate(ct->d, src, key, fb, st);
+        d_fallback = (int*)cws.words((fallback.size() + 1) / 2);
+        FHE_CUDA(cudaMemcpyAsync(d_fallback, fallback.data(), fallback.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+      }
+    }
+    const u32 gt = T.group_tile(n);
+    u64* P = cws.words((size_t)n * gt * W);
+    u64* R = cws.words((size_t)n * gt * W);
+    for (u32 g0 = 0; g0 < T.G; g0 += gt) {
+      const u32 ng = std::min(gt, T.G - g0);
+      launch_hoist_dot(d_steps, d_fallback, fb, D, adjacent, mrows, ct->d + (size_t)c0 * W, W, n, T.diags->d, c0,
+                       T.per_ct, T.n, b, g0, ng, P, L, lv.ctx_ids, par->d_limbs, logn, st);
+      T.finish(P, R, c0, n, g0, ng, out->d, st);
+    }
+  });
+  return n_fallback;
+}
+
+// Leveled keys and base-2^b keys: the composition itself -- every baby-step rotation through galois_range, the
+// products and sums of each group through launch_dot, then the giant steps and the sum
+static u32 linear_transform_unfused(const LinearTransform& T, fhe_b200_batch* out, cudaStream_t user) {
+  const fhe_b200_batch* ct = T.ct;
+  const fhe_b200_params* par = ct->par;
+  const u32 b = T.b;
+  const size_t W = T.W();
+  ChunkRunner(par, ct->count, user, std::max(1u, chunk_size() / std::max(b, T.G))).run([&](u32 c0, u32 n, cudaStream_t st) {
+    Workspace cws(par, st);
+    // B [n][b]: ciphertext c, then its rotations by 1 .. b - 1
+    u64* B = cws.words((size_t)n * b * W);
+    FHE_CUDA(cudaMemcpy2DAsync(B, b * W * sizeof(u64), ct->d + (size_t)c0 * W, W * sizeof(u64), W * sizeof(u64), n,
+                               cudaMemcpyDeviceToDevice, st));
+    if (b > 1) {
+      std::vector<u32> src, key;
+      for (u32 c = 0; c < n; c++)
+        for (u32 i = 1; i < b; i++) {
+          src.push_back(c0 + c);
+          key.push_back(T.baby_key[i]);
+        }
+      u64* rot = cws.words(src.size() * W);
+      T.rotate(ct->d, src, key, rot, st);
+      FHE_CUDA(cudaMemcpy2DAsync(B + W, b * W * sizeof(u64), rot, (b - 1) * W * sizeof(u64), (b - 1) * W * sizeof(u64),
+                                 n, cudaMemcpyDeviceToDevice, st));
+    }
+    const u32 gt = T.group_tile(n);
+    u64* P = cws.words((size_t)n * gt * W);
+    u64* R = cws.words((size_t)n * gt * W);
+    for (u32 g0 = 0; g0 < T.G; g0 += gt) {
+      const u32 ng = std::min(gt, T.G - g0);
+      for (u32 c = 0; c < n; c++)
+        for (u32 gi = 0; gi < ng; gi++) {
+          const u32 first = (g0 + gi) * b, terms = std::min(b, T.n - first);
+          launch_dot(B + (size_t)c * b * W, T.diag(c0 + c, first), P + ((size_t)c * ng + gi) * W, 1, terms, 2, terms,
+                     terms, ids_of(ct), par->d_limbs, par->logn, st);
+        }
+      T.finish(P, R, c0, n, g0, ng, out->d, st);
+    }
+  });
+  return ct->count * (b - 1);
+}
+
+int fhe_b200_linear_transform(const fhe_b200_batch* ct, const fhe_b200_batch* diags, uint32_t n_diags, uint32_t baby,
+                              const fhe_b200_ksk* const* gks, const uint32_t* exponents, uint32_t n_keys,
+                              fhe_b200_batch* out, uint32_t* n_fallback, void* stream) {
+  API_BEGIN
+  REQUIRE(!n_keys || (gks && exponents), FHE_B200_INVALID_ARGUMENT, "null key list or exponents");
+  for (u32 i = 0; i < n_keys; i++) REQUIRE(gks[i], FHE_B200_INVALID_ARGUMENT, "null key");
+  REQUIRE(ct && diags && out && ct != out && out->d != ct->d && diags != out && diags->d != out->d,
+          FHE_B200_INVALID_ARGUMENT, "null or aliased argument");
+  check_same(ct, diags);
+  REQUIRE(ct->par == out->par, FHE_B200_CONTEXT_MISMATCH, "ParameterMismatch: batches use different parameters");
+  REQUIRE(ct->level == out->level, FHE_B200_INVALID_LEVEL, "InvalidLevel: operands are at different levels");
+  REQUIRE(!ct->mul_basis && !out->mul_basis, FHE_B200_CONTEXT_MISMATCH, "PolynomialContextMismatch");
+  REQUIRE(ct->parts == 2, FHE_B200_BAD_POLY_COUNT, "InvalidPolynomialCount: expected 2");
+  REQUIRE(out->parts == 2 && out->count == ct->count, FHE_B200_INVALID_ARGUMENT,
+          "the output must hold one 2-part ciphertext per input ciphertext");
+  REQUIRE(diags->parts == 1, FHE_B200_INVALID_ARGUMENT, "diagonals must hold one polynomial per entry");
+  const fhe_b200_params* par = ct->par;
+  REQUIRE(n_diags >= 1 && n_diags <= par->N / 2, FHE_B200_INVALID_ARGUMENT,
+          "n_diags must be 1 .. N/2, got " + std::to_string(n_diags));
+  REQUIRE(baby >= 1 && baby <= n_diags, FHE_B200_INVALID_ARGUMENT,
+          "the baby step must be 1 .. n_diags, got " + std::to_string(baby));
+  REQUIRE(diags->count == n_diags || diags->count == (size_t)ct->count * n_diags, FHE_B200_INVALID_ARGUMENT,
+          "diags must hold n_diags entries or n_diags per ciphertext");
+  need_repr(ct, FHE_B200_NTT);
+  need_repr(diags, FHE_B200_NTT);
+  const std::vector<u32> exps = galois_exponents(par, exponents, n_keys);
+  if (n_keys) check_ksks(KeySet{gks, n_keys, nullptr}, par, ct->level, 0);
+  LinearTransform T{ct, diags, n_diags, baby, (n_diags + baby - 1) / baby, diags->count != n_diags, gks, n_keys,
+                    exps.data(), std::vector<u32>(baby), std::vector<u32>()};
+  T.giant_key.resize(T.G);
+  // EvaluationKey::rotates_columns_by's key of each step (evaluation_key.rs:145-170, :278-286)
+  auto key_of_step = [&](u32 step) {
+    const u32 e = (u32)powmod_h(3, step, 2 * (u64)par->N);
+    for (u32 k = 0; k < n_keys; k++)
+      if (exps[k] == e) return k;
+    throw FheError(FHE_B200_INVALID_ARGUMENT,
+                   "EvaluationKeyError: column rotation by " + std::to_string(step) + " not supported by the key list");
+  };
+  for (u32 i = 1; i < baby; i++) T.baby_key[i] = key_of_step(i);
+  for (u32 g = 1; g < T.G; g++) T.giant_key[g] = key_of_step(g * baby);
+  DeviceGuard g(par);
+  // the one routing decision, from the keys: a transform that needs no key is the plaintext products alone
+  const fhe_b200_ksk* k = baby > 1 || T.G > 1 ? gks[0] : nullptr;
+  const bool fused = !k || (k->log_base == 0 && k->Lk == par->level(ct->level).L);
+  const u32 f = fused ? linear_transform_fused(T, out, (cudaStream_t)stream)
+                      : linear_transform_unfused(T, out, (cudaStream_t)stream);
+  FHE_CUDA(cudaGetLastError());
+  out->repr = FHE_B200_NTT;
+  if (n_fallback) *n_fallback = f;
+  API_END
+}
+
 // EvaluationKey::computes_inner_sum (evaluation_key.rs:56-100) of every ciphertext: gks[s * n_gks + l] is the key of
 // step l of key set s (column rotations by 1, 2, 4, ..., N/4, then the row rotation), set_index[c] (nullable: set 0)
 // the key set of ciphertext c.  Step l of a chunk is one Galois call in sum mode, from the previous step's output; the

@@ -228,6 +228,24 @@ void launch_hoist_mac(const HoistOut* outs, u32 n, const u64* D, bool adjacent, 
                       size_t c0_stride, u64* out, size_t out_stride, u32 L, u32 Lk, const RowIds& ids,
                       const LimbDev* limbs, u32 logn, cudaStream_t st);
 
+// ---- linear transforms (DESIGN §3.4): baby-step/giant-step diagonal products from one hoisted decomposition.
+// Baby step i >= 1 of a transform: its Galois key pair ([L][L][N] each) and exponent (3^i mod 2N).
+struct LtStep {
+  const u64 *k0, *k1;
+  u32 exponent, pad;
+};
+// The partial sums of giant groups [g0, g0 + n_groups) of `cts` ciphertexts, NTT, keys at the ciphertext level (L):
+//   out[c][g - g0][p] = sum_{i < baby, g*baby + i < n_diags} diag[g*baby + i] (.) T_i,p(ct[c])
+// T_0 = ct[c]; T_i (i >= 1) = GaloisKey::relinearize of ct[c] for steps[i] from the digits D of its c1 (layout of
+// launch_hoist_mac, slot c) and the correction rows mrows [baby][L][N] (row i: NTT of N_e of steps[i]), as
+// hoist_mac_kernel computes it -- or, when fallback (nullable, [cts][baby]) gives f >= 0 for (c, i), item f of fb.
+// ct, fb, out: items of ct_stride words; diag: [.][L][N], entry k of ciphertext c at (per_ct ? (diag_ct0 + c) *
+// n_diags : 0) + k.  Every word canonical.
+void launch_hoist_dot(const LtStep* steps, const int* fallback, const u64* fb, const u64* D, bool adjacent,
+                      const u64* mrows, const u64* ct, size_t ct_stride, u32 cts, const u64* diag, u32 diag_ct0,
+                      bool per_ct, u32 n_diags, u32 baby, u32 g0, u32 n_groups, u64* out, u32 L, const RowIds& ids,
+                      const LimbDev* limbs, u32 logn, cudaStream_t st);
+
 // Poly<PowerBasis>::switch_down (rq/mod.rs:433-492): in [polys][L][N] -> out [polys][L-1][N]
 struct SwitchDownDev {
   u64 q_last, q_last_half;

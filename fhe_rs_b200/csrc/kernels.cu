@@ -1080,6 +1080,124 @@ __global__ void hoist_mac_kernel(const __grid_constant__ HoistMacArgs A) {
   out[(size_t)A.Lk << A.logn] = a1.reduce(M);
 }
 
+// ------------------------------------------------------------------ linear transforms (DESIGN §3.4)
+constexpr u32 kDotCts = 2;      // ciphertexts per thread: each key word loaded serves this many digit rows
+constexpr u32 kDotGroups = 8;   // giant groups per thread: each baby-step term computed serves this many groups
+struct HoistDotArgs {
+  const LtStep* steps;
+  const int* fallback;
+  const u64 *D, *mrows, *ct, *diag, *fb;
+  u64* out;
+  size_t ct_stride;
+  u32 cts, ct_tiles, diag_ct0, per_ct, n_diags, baby, g0, n_groups, L, logn, adjacent;
+  const LimbDev* limbs;
+  unsigned short ids[kMaxPos];
+};
+// One thread per (coefficient o, limb j = blockIdx.z), kDotCts ciphertexts and kDotGroups giant groups
+// (blockIdx.x = group tile * ct_tiles + ciphertext tile, fastest): the CTAs resident at any time work on the same
+// coefficients and limb of every tile, so each key and digit word they share comes from HBM once and from L2 after.
+// Baby step i >= 1 is hoist_mac_kernel's key switch of sigma_i(c1) plus sigma_i(c0), computed once for the thread's
+// ciphertexts from one load of the key words; step 0 is the ciphertext itself.  Each term is reduced, multiplied by
+// the diagonal of every group of the tile that uses it and added into that group's partial sum; nothing per baby
+// step leaves the registers.
+__global__ void __launch_bounds__(256) hoist_dot_kernel(const __grid_constant__ HoistDotArgs A) {
+  __shared__ u64 qk[kMaxPos];
+  const u32 N = 1u << A.logn, j = blockIdx.z;
+  const u32 gt = (blockIdx.x / A.ct_tiles) * kDotGroups, t0 = (blockIdx.x % A.ct_tiles) * kDotCts;
+  const LimbDev& M = A.limbs[A.ids[j]];
+  for (u32 k = threadIdx.x; k < A.L; k += blockDim.x) qk[k] = A.limbs[A.ids[k]].p % M.p;   // [q_k]_{q_j}
+  __syncthreads();
+  const u32 o = blockIdx.y * blockDim.x + threadIdx.x;
+  if (o >= N) return;
+  const u32 nt = min(kDotCts, A.cts - t0), ng = min(kDotGroups, A.n_groups - gt), g1 = A.g0 + gt;
+  // the tile's first group is full unless it is the last: baby steps beyond its terms serve no group of the tile
+  const u32 steps = min(A.baby, A.n_diags - g1 * A.baby);
+  const size_t row = (size_t)1 << A.logn, jo = ((size_t)j << A.logn) + o, part1 = (size_t)A.L << A.logn;
+  const size_t dstride = A.adjacent ? row : (size_t)A.L << A.logn, plane = ((size_t)A.L * A.L) << A.logn;
+  const size_t dbase = A.adjacent ? ((size_t)j * A.L) << A.logn : (size_t)j << A.logn;
+  const u64* ct = A.ct + t0 * A.ct_stride;
+  u64 r0[kDotGroups][kDotCts], r1[kDotGroups][kDotCts];
+#pragma unroll
+  for (u32 g = 0; g < kDotGroups; g++)
+#pragma unroll
+    for (u32 c = 0; c < kDotCts; c++) r0[g][c] = r1[g][c] = 0;
+  for (u32 i = 0; i < steps; i++) {
+    u64 v0[kDotCts], v1[kDotCts];
+    if (i == 0) {
+#pragma unroll
+      for (u32 c = 0; c < kDotCts; c++)
+        if (c < nt) {
+          v0[c] = ct[c * A.ct_stride + jo];
+          v1[c] = ct[c * A.ct_stride + part1 + jo];
+        }
+    } else {
+      const LtStep S = A.steps[i];
+      const u32 s = subst_source(o, S.exponent, A.logn);
+      const u64* k0 = S.k0 + (((size_t)j * A.L) << A.logn) + o;
+      const u64* k1 = S.k1 + (((size_t)j * A.L) << A.logn) + o;
+      const u64* d = A.D + t0 * plane + dbase + s;
+      Acc192 a0[kDotCts], a1[kDotCts], h0, h1;
+#pragma unroll
+      for (u32 c = 0; c < kDotCts; c++) {
+        a0[c].clear();
+        a1[c].clear();
+      }
+      h0.clear();
+      h1.clear();
+      for (u32 k = 0; k < A.L; k++) {
+        const u64 x = __ldg(k0 + ((size_t)k << A.logn)), y = __ldg(k1 + ((size_t)k << A.logn));
+        h0.mac(qk[k], x);
+        h1.mac(qk[k], y);
+#pragma unroll
+        for (u32 c = 0; c < kDotCts; c++)
+          if (c < nt) {
+            const u64 t = d[c * plane + k * dstride];
+            a0[c].mac(t, x);
+            a1[c].mac(t, y);
+          }
+      }
+      const u64 m = A.mrows[(((size_t)i * A.L + j) << A.logn) + o], e0 = h0.reduce(M), e1 = h1.reduce(M);
+#pragma unroll
+      for (u32 c = 0; c < kDotCts; c++)
+        if (c < nt) {
+          const int f = A.fallback ? A.fallback[(t0 + c) * A.baby + i] : -1;
+          if (f >= 0) {   // rot_i of this ciphertext, computed unhoisted
+            v0[c] = A.fb[f * A.ct_stride + jo];
+            v1[c] = A.fb[f * A.ct_stride + part1 + jo];
+            continue;
+          }
+          a0[c].mac(e0, m);
+          a1[c].mac(e1, m);
+          a0[c].add64(ct[c * A.ct_stride + ((size_t)j << A.logn) + s]);
+          v0[c] = a0[c].reduce(M);
+          v1[c] = a1[c].reduce(M);
+        }
+    }
+#pragma unroll
+    for (u32 g = 0; g < kDotGroups; g++) {
+      const u32 k = (g1 + g) * A.baby + i;
+      if (g >= ng || k >= A.n_diags) continue;
+#pragma unroll
+      for (u32 c = 0; c < kDotCts; c++)
+        if (c < nt) {
+          const size_t dk = (A.per_ct ? (size_t)(A.diag_ct0 + t0 + c) * A.n_diags : 0) + k;
+          const u64 w = A.diag[dk * part1 + jo];
+          r0[g][c] = csub(r0[g][c] + mulmod_limb(v0[c], w, M), M.p);
+          r1[g][c] = csub(r1[g][c] + mulmod_limb(v1[c], w, M), M.p);
+        }
+    }
+  }
+#pragma unroll
+  for (u32 g = 0; g < kDotGroups; g++)
+#pragma unroll
+    for (u32 c = 0; c < kDotCts; c++)
+      if (g < ng && c < nt) {
+        u64* out = A.out + ((size_t)(t0 + c) * A.n_groups + gt + g) * A.ct_stride + jo;
+        out[0] = r0[g][c];
+        out[part1] = r1[g][c];
+      }
+}
+
 struct SwitchDownArgs {
   SwitchDownDev S;
   const u64* in;
@@ -2271,6 +2389,24 @@ void launch_hoist_mac(const HoistOut* outs, u32 n, const u64* D, bool adjacent, 
     A.keys.slot[i - i0] = (unsigned char)s;
   }
   if (n > i0) flush(n);
+}
+
+void launch_hoist_dot(const LtStep* steps, const int* fallback, const u64* fb, const u64* D, bool adjacent,
+                      const u64* mrows, const u64* ct, size_t ct_stride, u32 cts, const u64* diag, u32 diag_ct0,
+                      bool per_ct, u32 n_diags, u32 baby, u32 g0, u32 n_groups, u64* out, u32 L, const RowIds& ids,
+                      const LimbDev* limbs, u32 logn, cudaStream_t st) {
+  if (!cts || !n_groups) return;
+  const u32 N = 1u << logn, threads = std::min(256u, N);
+  HoistDotArgs A;
+  std::memset(&A, 0, sizeof(A));
+  A.steps = steps; A.fallback = fallback; A.fb = fb; A.D = D; A.mrows = mrows; A.ct = ct; A.diag = diag; A.out = out;
+  A.ct_stride = ct_stride; A.cts = cts; A.ct_tiles = (cts + kDotCts - 1) / kDotCts; A.diag_ct0 = diag_ct0;
+  A.per_ct = per_ct ? 1 : 0; A.n_diags = n_diags; A.baby = baby; A.g0 = g0; A.n_groups = n_groups; A.L = L;
+  A.logn = logn; A.adjacent = adjacent ? 1 : 0; A.limbs = limbs;
+  copy_ids(A.ids, ids);
+  const u32 group_tiles = (n_groups + kDotGroups - 1) / kDotGroups;
+  hoist_dot_kernel<<<dim3(group_tiles * A.ct_tiles, (N + threads - 1) / threads, L), threads, 0, st>>>(A);
+  g_launches++;
 }
 
 void launch_pack(const PackDev& P, const u64* words, unsigned char* bytes, size_t n_rows, u32 logn, cudaStream_t st) {

@@ -544,6 +544,33 @@ int fhe_b200_galois_many(const fhe_b200_batch* ct, const uint32_t* source, const
 int fhe_b200_galois_many_hoisted(const fhe_b200_batch* ct, const uint32_t* source, const fhe_b200_ksk* const* gks,
                                  const uint32_t* exponents, uint32_t n_keys, const uint32_t* key_index,
                                  fhe_b200_batch* out, uint32_t* n_hoisted, void* stream);
+/* Plaintext-matrix x ciphertext-vector products by baby-step/giant-step diagonals, for every ciphertext c of ct:
+ *   out[c] = sum_{g < G} rot_{g b}( sum_{i < b, g b + i < n_diags} diags[g b + i] (.) B_i(ct[c]) ),  G = ceil(n_diags / b),
+ * with B_0 the identity (no key switch) and B_i = rot_i, rot_k = EvaluationKey::rotates_columns_by(k) (exponent
+ * 3^k mod 2N, keys/evaluation_key.rs:145-170).  The words are those of that composition of galois, mul_plain_batch and
+ * add calls.  ct: 2-part NTT batch; diags: 1-part NTT batch at ct's level (fhe_b200_encode) holding n_diags entries
+ * shared by every ciphertext, or ct.count * n_diags (entry c * n_diags + k is diagonal k of ciphertext c), already
+ * rotated for the giant steps; out: ct's shape, must not alias ct or diags, becomes NTT.  gks / exponents / n_keys: a
+ * key list as fhe_b200_galois_many takes it (one level, digit count and base); the call uses the keys of the steps
+ * 1 .. b - 1 and b, 2b, .., (G - 1) b and ignores the others.
+ * Keys at the ciphertext level with RNS digits run one hoisted digit decomposition per ciphertext and one kernel that
+ * multiplies each baby step's key switch by its diagonals and sums them, without writing the rotations; a baby-step
+ * term whose ciphertext fails the zero check of fhe_b200_galois_many_hoisted is rotated unhoisted instead.  Leveled
+ * keys and base-2^b keys run the composition itself.  n_fallback (host memory, nullable) receives how many
+ * (ciphertext, baby step >= 1) rotations were computed unhoisted: the zero-check failures, or count * (b - 1) for
+ * leveled and base-2^b keys.
+ * Errors: a step without a key, baby = 0, baby > n_diags, n_diags = 0 or > N/2, a diags count other than n_diags or
+ * ct.count * n_diags, an output of another shape, aliasing, a null key -> INVALID_ARGUMENT (a transform with
+ * n_diags = 1 needs no key and takes n_keys = 0); ct, diags,
+ * out or a key at different levels -> INVALID_LEVEL; power-basis operands -> INVALID_REPRESENTATION; even exponents
+ * -> INVALID_EXPONENT.  A refused call enqueues nothing.
+ * Synchronisation: with b >= 2 and keys at the ciphertext level without base-2^b digits, the call synchronises
+ * `stream` once, after the zero check, to read it on the host.
+ * Scratch: stream-ordered and released by the call; per chunk of ciphertexts their digits (L x L x N words each) and
+ * two buffers of partial sums, and b x L x N words of correction rows per call. */
+int fhe_b200_linear_transform(const fhe_b200_batch* ct, const fhe_b200_batch* diags, uint32_t n_diags, uint32_t baby,
+                              const fhe_b200_ksk* const* gks, const uint32_t* exponents, uint32_t n_keys,
+                              fhe_b200_batch* out, uint32_t* n_fallback, void* stream);
 /* EvaluationKey::computes_inner_sum (keys/evaluation_key.rs:56-100) of every ciphertext of ct into out (same shape,
  * must not alias ct; ct is left unchanged; out becomes NTT).  gks holds n_gks = log2 N keys: the Galois keys of the
  * column rotations by 1, 2, 4, ..., N/4 (exponents 3^i mod 2N), then of the row rotation (2N - 1); any other n_gks or a

@@ -690,6 +690,16 @@ class RGSWCiphertext {
 
 // fhe::bfv::EvaluationKey (keys/evaluation_key.rs:21-310): Galois keys by exponent, and the levels of the ciphertexts
 // it takes and of its keys (both 0 unless an EvaluationKeyBuilder or a message sets them)
+// the column rotation steps a linear transform of n_diags diagonals with baby step `baby` needs keys for (to enable in
+// EvaluationKeyBuilder): the baby steps 1 .. baby - 1, then the giant steps baby, 2 baby, ..
+inline std::vector<uint32_t> linear_transform_steps(uint32_t n_diags, uint32_t baby) {
+  if (baby < 1 || baby > n_diags) throw Error(FHE_B200_INVALID_ARGUMENT, "the baby step must be 1 .. n_diags");
+  std::vector<uint32_t> s;
+  for (uint32_t i = 1; i < baby; i++) s.push_back(i);
+  for (uint32_t g = baby; g < n_diags; g += baby) s.push_back(g);
+  return s;
+}
+
 class EvaluationKey {
  public:
   explicit EvaluationKey(std::shared_ptr<BfvParameters> par, uint32_t ciphertext_level = 0,
@@ -701,6 +711,23 @@ class EvaluationKey {
   void add_galois_key(std::shared_ptr<GaloisKey> gk) { gk_[gk->exponent % (2 * (uint32_t)par_->degree())] = std::move(gk); }
   Ciphertext rotates_rows(const Ciphertext& ct) const { return at(2 * (uint32_t)par_->degree() - 1).relinearize(ct); }
   Ciphertext rotates_columns_by(const Ciphertext& ct, uint32_t i) const { return at(column_exponent(i)).relinearize(ct); }
+  // sum_k diag_k (.) rotates_columns_by(ct, k) of every ciphertext by baby-step/giant-step diagonals in one device call
+  // (fhe_b200_linear_transform); diags from encode_diagonals, n_diags shared by every ciphertext or n_diags per one
+  Ciphertext linear_transform(const Ciphertext& ct, const Ciphertext& diags, uint32_t baby, uint32_t n_diags) const {
+    std::vector<const fhe_b200_ksk*> keys;
+    std::vector<uint32_t> exps;
+    for (uint32_t i : linear_transform_steps(n_diags, baby)) {
+      exps.push_back(column_exponent(i));
+      keys.push_back(at(exps.back()).ksk->handle());
+    }
+    Ciphertext out(ct.par(), ct.count(), 2, ct.level(), Representation::Ntt, ct.stream());
+    check(fhe_b200_linear_transform(ct.handle(), diags.handle(), n_diags, baby, keys.data(), exps.data(),
+                                    (uint32_t)keys.size(), out.handle(), nullptr, ct.stream()));
+    return out;
+  }
+  Ciphertext linear_transform(const Ciphertext& ct, const PlaintextVec& diags, uint32_t baby, uint32_t n_diags) const {
+    return linear_transform(ct, diags.batch(), baby, n_diags);
+  }
   // evaluation_key.rs:40-53
   bool supports_inner_sum() const {
     const uint32_t n = (uint32_t)par_->degree();
@@ -1090,6 +1117,49 @@ inline Ciphertext galois_many_hoisted(const Ciphertext& ct, const std::vector<co
   check(fhe_b200_galois_many_hoisted(ct.handle(), source.empty() ? nullptr : source.data(), h.data(), exps.data(),
                                      (uint32_t)gks.size(), index.data(), out.handle(), n_hoisted, ct.stream()));
   return out;
+}
+// out[c] = sum_g rot_{g baby}(sum_i diags[g baby + i] (.) rot_i(ct[c])), rot_0 the identity, word for word the
+// composition of rotates_columns_by, mul_plain and + (fhe_b200_linear_transform); gks: Galois keys holding at least the
+// steps of linear_transform_steps; *n_fallback (when given) receives how many baby-step rotations were unhoisted
+inline Ciphertext linear_transform(const Ciphertext& ct, const Ciphertext& diags, uint32_t n_diags, uint32_t baby,
+                                   const std::vector<const GaloisKey*>& gks, uint32_t* n_fallback = nullptr) {
+  const auto h = keyed_detail::handles(gks, [](const GaloisKey& k) { return k.ksk->handle(); });
+  std::vector<uint32_t> exps;
+  for (const GaloisKey* g : gks) exps.push_back(g ? g->exponent : 1);
+  Ciphertext out(ct.par(), ct.count(), 2, ct.level(), Representation::Ntt, ct.stream());
+  check(fhe_b200_linear_transform(ct.handle(), diags.handle(), n_diags, baby, gks.empty() ? nullptr : h.data(),
+                                  exps.empty() ? nullptr : exps.data(), (uint32_t)gks.size(), out.handle(), n_fallback,
+                                  ct.stream()));
+  return out;
+}
+// The diagonals of `count` slot-wise linear maps for linear_transform, SIMD-encoded at `level`: matrices holds count
+// pairs of (N/2) x (N/2) matrices, [count][2][N/2][N/2] (one per slot row), entries taken mod t.  Diagonal k of a map is
+// M[r][(r + k) mod N/2] in slot r of each row, rotated right by its giant step (k / baby) * baby; the result holds
+// diagonals 0 .. n_diags - 1 (0: N/2) of each map.  A non-zero diagonal from n_diags on is refused.
+inline PlaintextVec encode_diagonals(const std::shared_ptr<BfvParameters>& par, const std::vector<uint64_t>& matrices,
+                                     uint32_t count, uint32_t baby, uint32_t level = 0, uint32_t n_diags = 0) {
+  const size_t half = par->degree() / 2;
+  uint64_t t = 0;
+  const std::vector<uint8_t>& t_le = par->plaintext_le();
+  if (t_le.size() > 8) throw Error(FHE_B200_INVALID_ARGUMENT, "EncodingError::SimdUnavailable");
+  for (size_t i = t_le.size(); i-- > 0;) t = (t << 8) | t_le[i];
+  if (!n_diags) n_diags = (uint32_t)half;
+  if (matrices.size() != count * 2 * half * half || n_diags > half || baby < 1 || baby > n_diags)
+    throw Error(FHE_B200_INVALID_ARGUMENT, "expected [count][2][N/2][N/2] matrices, n_diags <= N/2, 1 <= baby <= n_diags");
+  std::vector<uint64_t> v((size_t)count * n_diags * 2 * half);
+  for (size_t c = 0; c < count; c++)
+    for (size_t q = 0; q < 2; q++)
+      for (size_t k = 0; k < half; k++)
+        for (size_t r = 0; r < half; r++) {
+          const uint64_t x = matrices[((c * 2 + q) * half + r) * half + (r + k) % half] % t;
+          if (k >= n_diags) {
+            if (x) throw Error(FHE_B200_INVALID_ARGUMENT, "a diagonal beyond the first n_diags is not zero");
+            continue;
+          }
+          const size_t shift = (k / baby) * baby;
+          v[((c * n_diags + k) * 2 + q) * half + (r + shift) % half] = x;
+        }
+  return PlaintextVec::try_encode(v, Encoding::simd_at_level(level), par);
 }
 // EvaluationKey::computes_inner_sum of ciphertext j with eks[index[j]] (fhe_b200_inner_sum_keyed)
 inline Ciphertext computes_inner_sum_keyed(const Ciphertext& ct, const std::vector<const EvaluationKey*>& eks,
